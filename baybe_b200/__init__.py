@@ -1,4 +1,4 @@
-"""baybe_b200 -- B200-native (sm_100a) GP-posterior + acquisition scoring engine that drops in
+"""baybe_b200 -- H100-native (sm_90a) GP-posterior + acquisition scoring engine that drops in
 behind BayBE's Surrogate / AcquisitionFunction / Recommender surfaces for purely discrete
 search spaces.  See DESIGN.md; the C ABI is declared in include/baybe_b200.h."""
 

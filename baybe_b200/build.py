@@ -1,4 +1,4 @@
-"""Build ``libbaybe_b200.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build ``libbaybe_b200.so`` (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 Usage: ``python -m baybe_b200.build [--force]``.  nvcc cross-compiles without a GPU.
 """
@@ -18,9 +18,9 @@ OUT_DIR = PKG / "_C"
 LIB_PATH = OUT_DIR / "libbaybe_b200.so"
 STAMP = OUT_DIR / "build.stamp"
 
-SOURCES = ["model.cu", "fused.cu", "fused_tc.cu", "fused_ts.cu", "wide.cu", "aux_kernels.cu", "acq.cu", "peer.cu", "stream.cu"]
+SOURCES = ["model.cu", "fused.cu", "wide.cu", "aux_kernels.cu", "acq.cu", "peer.cu", "stream.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]  # cudart is linked statically (nvcc default): the library adopts the caller's current context

@@ -105,15 +105,6 @@ __device__ __forceinline__ void mc_partial(const bb_acq_spec& a, float mu, float
   else if (a.kind == BB_ACQ_QPI) mc_partial_kind<BB_ACQ_QPI>(c0, c1, z4, n4, s0, s1);
 }
 
-// Accumulate the samples z4[0..n4) (4 per element) into (s0, s1) for pre-computed coefficients;
-// lets a caller spread one candidate's Monte-Carlo work over several program phases.
-__device__ __forceinline__ void mc_accumulate(int kind, float c0, float c1, const float4* __restrict__ z4,
-                                              int n4, float& s0, float& s1) {
-  if (kind == BB_ACQ_QLOGEI) mc_partial_kind<BB_ACQ_QLOGEI>(c0, c1, z4, n4, s0, s1);
-  else if (kind == BB_ACQ_QEI) mc_partial_kind<BB_ACQ_QEI>(c0, c1, z4, n4, s0, s1);
-  else if (kind == BB_ACQ_QPI) mc_partial_kind<BB_ACQ_QPI>(c0, c1, z4, n4, s0, s1);
-}
-
 // ------------------------------------------------------------------------------------------
 // qLogEI, tabulated fat-tail sum (q = 1, shared base samples).
 // With x_s = (o_s - best_f)/tau = c0 + c1 z_s, tau = 1e-6 and zeta = sign(c1) z sorted descending, a candidate
@@ -191,8 +182,8 @@ __device__ __forceinline__ void mc_table_setup(float* __restrict__ tab, const fl
   __syncthreads();
 }
 
-// The same table built by a GRID once per call (fused_ts.cu: rebuilding it in each of the 148 persistent CTAs took
-// ~23 us of every launch): every CTA repeats the cheap top-16 step, warp w of CTA b then fills entry 8 b + w with a
+// The same table built by a GRID once per call (rebuilding it in each persistent CTA of a full-size launch costs more
+// than it saves): every CTA repeats the cheap top-16 step, warp w of CTA b then fills entry 8 b + w with a
 // lane-parallel sum (fixed order: lane partials over e = lane, lane + 32, ..., xor-tree).  CTA 0 also stores the
 // top-16 block and the validity flag.  out: kMcRows floats in global memory.
 __device__ __forceinline__ void mc_table_grid_part(float* __restrict__ tab, const float* __restrict__ z_s, int S,
@@ -293,41 +284,6 @@ __device__ __forceinline__ bool mc_row_fast(const float* __restrict__ tab, float
   return fast;
 }
 
-// mc_row_fast split over the four lanes that share a row in fused_ts.cu: lane `sub` (0..3) evaluates the exact
-// terms k = sub, sub+4, sub+8, sub+12 of the sixteen, lane 0 adds the tabulated tail; the caller sums (s0, s1) over
-// the four lanes (fixed order: the value of a row does not depend on where it is evaluated).  The envelope test
-// is identical in the four lanes.
-__device__ __forceinline__ bool mc_row_fast_part(const float* __restrict__ tab, float c0, float c1, int sub,
-                                                 float& s0, float& s1) {
-  const float ac1 = fabsf(c1);
-  const float t9 = fmaf(ac1, tab[kMcTop + kMcJ], c0);
-  const float t17 = fmaf(ac1, tab[kMcTop + kMcK - 1], c0);
-  const bool fast = tab[kMcOk] != 0.f && ac1 > 1e-30f && t9 <= 0.f && t17 <= -1024.f;
-  s0 = 0.f;
-  s1 = 0.f;
-  if (fast) {
-#pragma unroll
-    for (int k = 0; k < kMcK / 4; ++k) {
-      const float t = fmaf(ac1, tab[kMcTop + sub + 4 * k], c0);
-      s0 += fmaxf(t, 0.f);
-      s1 += fast_rcp(fmaf(t, t, 1.0f));
-      if (fabsf(t) < 30.f) s0 += softplus_tail(fabsf(t));  // within 30 tau of the incumbent (rare)
-    }
-    if (sub == 0) {
-      const float inv = 1.0f / ac1;
-      const float a = fmaf(-t9, inv, 1.0f);  // w - zeta_(9) + 1 >= 1, no cancellation
-      const float v = 1.0f / a;
-      const float x = v * (float)kMcNT;
-      const int i = min((int)x, kMcNT - 1);
-      const float fr = x - (float)i;
-      const float f0 = tab[i], f1 = tab[i + 1];
-      const float q = v * inv;
-      s1 = fmaf(fmaf(fr, f1 - f0, f0), q * q, s1);
-    }
-  }
-  return fast;
-}
-
 // Exact (s0, s1) of one row by a whole warp: lane l takes samples l, l+32, ...; fixed reduction order, so a row's
 // value does not depend on where it is evaluated.  Result in every lane.
 __device__ __forceinline__ void mc_row_exact_warp(const float* __restrict__ z_s, int S, float c0, float c1, int lane,
@@ -348,21 +304,6 @@ __device__ __forceinline__ void mc_row_exact_warp(const float* __restrict__ z_s,
   }
   a0 += b0;
   a1 += b1;
-  for (int o = 16; o > 0; o >>= 1) {
-    a0 += __shfl_xor_sync(0xffffffffu, a0, o);
-    a1 += __shfl_xor_sync(0xffffffffu, a1, o);
-  }
-}
-
-// Per-sample kinds without a table (qEI, qPI, qLogEI outside the table's S range) by a whole warp: lane l takes the
-// float4 sample groups l, l + 32, ...; fixed reduction order; result in every lane.  S is a multiple of 16.
-__device__ __forceinline__ void mc_row_groups_warp(int kind, const float* __restrict__ z_s, int S, float c0,
-                                                   float c1, int lane, float& a0, float& a1) {
-  a0 = 0.f;
-  a1 = 0.f;
-  const float4* z4 = reinterpret_cast<const float4*>(z_s);
-  const int G = S >> 2;
-  for (int g = lane; g < G; g += 32) mc_accumulate(kind, c0, c1, z4 + g, 1, a0, a1);
   for (int o = 16; o > 0; o >>= 1) {
     a0 += __shfl_xor_sync(0xffffffffu, a0, o);
     a1 += __shfl_xor_sync(0xffffffffu, a1, o);

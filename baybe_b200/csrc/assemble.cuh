@@ -1,5 +1,5 @@
 // assemble.cuh -- the K(X*, X) assembly core shared by the fused scoring kernel (A operand of the
-// tcgen05 GEMM), the stand-alone kernel-matrix kernel and the pending cross-covariance kernel.
+// wgmma GEMM), the stand-alone kernel-matrix kernel and the pending cross-covariance kernel.
 //
 // Restates gpytorch MaternKernel/RBFKernel.forward + Distance._sq_dist (constructed by the
 // reference at /root/reference/baybe/kernels/base.py:173-178): scaled squared distance in the
@@ -10,17 +10,12 @@
 // Matern-1/2 is not differentiable in r^2 at 0, so for that family the distance is formed from
 // direct differences (exact near coincident points) at twice the FMA cost.
 //
-// Register tile: one thread = 2 candidates x 8 training points.  The inner product runs on
-// packed fp32x2 FMAs (FFMA2, sm_100): each 64-bit accumulator holds two neighbouring training
-// points of one candidate; training rows are stored pair-interleaved and the candidate values
-// duplicated so that every operand pair comes straight out of an LDS.128.
+// Register tile: one thread = 2 candidates x 8 training points.  Training rows are stored
+// pair-interleaved and the candidate values duplicated so that every operand pair comes straight
+// out of an LDS.128.
 #pragma once
 
 #include "common.cuh"
-
-#ifndef BB_FFMA2
-#define BB_FFMA2 1
-#endif
 
 namespace bb {
 
@@ -100,6 +95,41 @@ __device__ __forceinline__ float4 load_quad(const void* __restrict__ x, int64_t 
   return q;
 }
 
+// Rows that arrive while the kernel runs (gated host pass) are read with ld.global.cg: coherent at L2, where the
+// copy engine's writes land; ld.global.nc (__ldg) presumes data that is constant for the kernel's lifetime.
+// Level-coded rows (kLayoutCodes4: two columns per byte, low nibble = even column; kLayoutCodes8: one byte per
+// column) index the per-column value table [d][table_ld].
+__device__ __forceinline__ float4 load_quad_gated(const void* __restrict__ x, int layout, int64_t row, int j0, int d,
+                                                  int64_t ldx, bool row_ok, const float* __restrict__ table,
+                                                  int table_ld) {
+  float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (!row_ok || j0 >= d) return q;
+  if (layout == kLayoutCodes4) {
+    const uint8_t* c = reinterpret_cast<const uint8_t*>(x) + row * ldx + (j0 >> 1);
+    const uint32_t b0 = __ldcg(c), b1 = (j0 + 2 < d) ? (uint32_t)__ldcg(c + 1) : 0u;
+    const float* t = table + (size_t)j0 * table_ld;
+    q.x = __ldg(t + (b0 & 15u));
+    if (j0 + 1 < d) q.y = __ldg(t + table_ld + (b0 >> 4));
+    if (j0 + 2 < d) q.z = __ldg(t + 2 * table_ld + (b1 & 15u));
+    if (j0 + 3 < d) q.w = __ldg(t + 3 * table_ld + (b1 >> 4));
+  } else if (layout == kLayoutCodes8) {
+    const uint8_t* c = reinterpret_cast<const uint8_t*>(x) + row * ldx + j0;
+    const float* t = table + (size_t)j0 * table_ld;
+    q.x = __ldg(t + __ldcg(c));
+    if (j0 + 1 < d) q.y = __ldg(t + table_ld + __ldcg(c + 1));
+    if (j0 + 2 < d) q.z = __ldg(t + 2 * table_ld + __ldcg(c + 2));
+    if (j0 + 3 < d) q.w = __ldg(t + 3 * table_ld + __ldcg(c + 3));
+  } else {  // row-major fp32
+    const float* ptr = reinterpret_cast<const float*>(x) + row * ldx + j0;
+    if (j0 + 3 < d && ((reinterpret_cast<uintptr_t>(ptr) & 15) == 0)) return __ldcg(reinterpret_cast<const float4*>(ptr));
+    q.x = __ldcg(ptr);
+    if (j0 + 1 < d) q.y = __ldcg(ptr + 1);
+    if (j0 + 2 < d) q.z = __ldcg(ptr + 2);
+    if (j0 + 3 < d) q.w = __ldcg(ptr + 3);
+  }
+  return q;
+}
+
 __device__ __forceinline__ float4 load_quad_any(const void* __restrict__ x, int layout, int64_t row,
                                                 int j0, int d, int64_t ldx, bool row_ok) {
   switch (layout) {
@@ -118,7 +148,15 @@ struct StageCtx {
   const float* cscale;  // shared [d_pad]
   const float* cshift;
   int groups;           // nthreads / 128
+  bool gated;           // rows published while the kernel runs (level codes or row-major fp32)
+  const float* code_table;
+  int code_table_ld;
 };
+
+__device__ __forceinline__ float4 stage_load_quad(const StageCtx& c, int64_t row, int jq, bool row_ok) {
+  if (c.gated) return load_quad_gated(c.x, c.layout, row, jq * 4, c.d, c.ldx, row_ok, c.code_table, c.code_table_ld);
+  return load_quad_any(c.x, c.layout, row, jq * 4, c.d, c.ldx, row_ok);
+}
 
 // Issue the global loads of tile `row0` (first kStageQuads quads of this thread) into registers.
 __device__ __forceinline__ void stage_prefetch(const StageCtx& c, int dq, int64_t row0, int t,
@@ -129,8 +167,7 @@ __device__ __forceinline__ void stage_prefetch(const StageCtx& c, int dq, int64_
 #pragma unroll
   for (int u = 0; u < kStageQuads; ++u) {
     const int jq = jg + u * c.groups;
-    regs.v[u] = (jq < dq) ? load_quad_any(c.x, c.layout, row, jq * 4, c.d, c.ldx, ok)
-                          : make_float4(0.f, 0.f, 0.f, 0.f);
+    regs.v[u] = (jq < dq) ? stage_load_quad(c, row, jq, ok) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
 
@@ -161,8 +198,7 @@ __device__ __forceinline__ void stage_commit(const StageCtx& c, float4* a_s, int
   }
   const int64_t row = row0 + r;
   for (int jq = jg + kStageQuads * c.groups; jq < dq; jq += c.groups)
-    stage_store_quad(c, a_s, cand_task, T, r, jq,
-                     load_quad_any(c.x, c.layout, row, jq * 4, c.d, c.ldx, row < c.N));
+    stage_store_quad(c, a_s, cand_task, T, r, jq, stage_load_quad(c, row, jq, row < c.N));
 }
 
 __device__ __forceinline__ float cand_sqnorm(const AsmSmem& sm, int m) {
@@ -174,28 +210,13 @@ __device__ __forceinline__ float cand_sqnorm(const AsmSmem& sm, int m) {
   return s;
 }
 
-// packed fp32x2 FMA: {d.lo, d.hi} = {a.lo*b.lo + c.lo, a.hi*b.hi + c.hi}
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b,
-                                                   unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
-  return (unsigned long long)__float_as_uint(lo) | ((unsigned long long)__float_as_uint(hi) << 32);
-}
-__device__ __forceinline__ float lo_of(unsigned long long v) { return __uint_as_float((unsigned)v); }
-__device__ __forceinline__ float hi_of(unsigned long long v) {
-  return __uint_as_float((unsigned)(v >> 32));
-}
-
 // Kernel values of candidates (m0, m1) against the 8 training points i0..i0+7 (i0 % 8 == 0).
 template <int FAMILY>
 __device__ __forceinline__ void assemble_2x8(const AsmSmem& sm, int m0, int m1, float an0,
                                              float an1, int i0, float (&k0)[8], float (&k1)[8]) {
   constexpr bool kDirect = (FAMILY == BB_KERNEL_MATERN12);
   float t0[8], t1[8];
-  if constexpr (kDirect || !BB_FFMA2) {
+  {
     float acc0[8], acc1[8];
 #pragma unroll
     for (int ii = 0; ii < 8; ++ii) {
@@ -241,39 +262,6 @@ __device__ __forceinline__ void assemble_2x8(const AsmSmem& sm, int m0, int m1, 
     for (int ii = 0; ii < 8; ++ii) {
       t0[ii] = acc0[ii];
       t1[ii] = acc1[ii];
-    }
-  } else {
-    unsigned long long acc0[4], acc1[4];
-    const float2* tq = reinterpret_cast<const float2*>(sm.tsq + i0);
-#pragma unroll
-    for (int ip = 0; ip < 4; ++ip) {
-      const float2 t = tq[ip];
-      acc0[ip] = pack2(t.x + an0, t.y + an0);
-      acc1[ip] = pack2(t.x + an1, t.y + an1);
-    }
-    const ulonglong2* xt = reinterpret_cast<const ulonglong2*>(sm.xt4 + i0);
-    const ulonglong2* a0p = reinterpret_cast<const ulonglong2*>(sm.a_s + m0);
-    const ulonglong2* a1p = reinterpret_cast<const ulonglong2*>(sm.a_s + m1);
-#pragma unroll 1
-    for (int jc = 0; jc < sm.dq; ++jc) {
-      const ulonglong2 A00 = a0p[0], A01 = a0p[kTileM];
-      const ulonglong2 A10 = a1p[0], A11 = a1p[kTileM];
-#pragma unroll
-      for (int ip = 0; ip < 4; ++ip) {
-        const ulonglong2 P0 = xt[2 * ip], P1 = xt[2 * ip + 1];
-        acc0[ip] = fma2(A00.x, P0.x, fma2(A00.y, P0.y, fma2(A01.x, P1.x, fma2(A01.y, P1.y, acc0[ip]))));
-        acc1[ip] = fma2(A10.x, P0.x, fma2(A10.y, P0.y, fma2(A11.x, P1.x, fma2(A11.y, P1.y, acc1[ip]))));
-      }
-      xt += sm.np;
-      a0p += 2 * kTileM;
-      a1p += 2 * kTileM;
-    }
-#pragma unroll
-    for (int ip = 0; ip < 4; ++ip) {
-      t0[2 * ip] = lo_of(acc0[ip]);
-      t0[2 * ip + 1] = hi_of(acc0[ip]);
-      t1[2 * ip] = lo_of(acc1[ip]);
-      t1[2 * ip + 1] = hi_of(acc1[ip]);
     }
   }
 #pragma unroll

@@ -91,6 +91,9 @@ __device__ __forceinline__ AuxSmem aux_carve(uint8_t* base, const AuxParams& p, 
   r.sc.cscale = cscale_s;
   r.sc.cshift = cshift_s;
   r.sc.groups = nthreads / kTileM;
+  r.sc.gated = false;
+  r.sc.code_table = nullptr;
+  r.sc.code_table_ld = 0;
   return r;
 }
 
@@ -451,9 +454,9 @@ extern "C" int bb_kernel_matrix(const bb_model* m, const void* d_x, int32_t layo
   BB_CHECK_ARG(d_k != nullptr || N == 0, "bb_kernel_matrix: output pointer is null");
   BB_CHECK_ARG(ldk >= m->n, "bb_kernel_matrix: ldk=%lld smaller than n=%d", (long long)ldk, m->n);
   if (N == 0) return BB_OK;
-  {  // tensor-core distances + TMA tensor-map stores (fused_ts.cu: k_kmat_ts) where the shape allows
+  {  // tensor-core distances + TMA tensor stores (fused.cu: k_kmat_tma) where the model and the output allow
     bool handled = false;
-    rc = try_kmat_ts(m, d_x, layout, N, ldx, d_k, ldk, stream, &handled);
+    rc = try_kmat_tma(m, d_x, layout, N, ldx, d_k, ldk, stream, &handled);
     if (rc != BB_OK || handled) return rc;
   }
   p.kout = d_k;

@@ -1,5 +1,5 @@
-// common.cuh -- shared helpers: error plumbing, PTX wrappers for sm_100a (mbarrier, bulk copy
-// (TMA engine), tcgen05 MMA / TMEM), fp16 split, packed arg-max keys.
+// common.cuh -- shared helpers: error plumbing, PTX wrappers for sm_90a (mbarrier, bulk copy
+// (TMA engine), warpgroup MMA), fp16 split, packed arg-max keys.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -82,9 +82,12 @@ static inline int device_limits(int* sms, int* max_smem) {
     }                                                                                                      \
   } while (0)
 
-constexpr int kTileM = 128;     // candidates per tile = UMMA_M
+constexpr int kTileM = 128;     // candidates per tile = two 64-row warpgroup MMAs
 constexpr int kChunk = 64;      // training points per K chunk = one 128-byte swizzle row of fp16
-constexpr int kSMs = 148;
+constexpr int kSMs = 132;       // H100 SXM: grid caps of the grid-stride kernels
+
+// candidate layouts beyond bb_layout, internal to the single-launch host pass: level codes expanded while staging
+constexpr int kLayoutCodes4 = 16, kLayoutCodes8 = 17;
 
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
@@ -216,81 +219,60 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 }
 
 // ------------------------------------------------------------------------------------------
-// PTX: tcgen05 (5th-gen tensor cores) + tensor memory
+// PTX: warpgroup MMA (wgmma, sm_90a).  Operands are K-major fp16 tiles in shared memory; the fp32
+// accumulator lives in the registers of the issuing warpgroup (128 threads).
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, kind::f16 (fp16 operands, fp32 accumulate), one CTA.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of fp32 from TMEM: thread i gets row (lane base + i), 32 columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor: K-major operand, 128-byte swizzle, rows of 64 fp16 (128 B),
-// 8-row groups 1024 B apart (SBO), descriptor version 1 (Blackwell).
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
+// Shared-memory matrix descriptor of a K-major swizzled tile whose 8-row groups are contiguous:
+// K2 = 64 -> 128-byte rows / 128B swizzle, K2 = 32 -> 64-byte rows / 64B swizzle.  Advancing the
+// start address by 32 bytes (two 16-byte units) steps K by 16 inside the swizzle atom.
+template <int K2>
+__device__ __forceinline__ uint64_t make_wg_desc(uint32_t smem_addr) {
   uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);  // start address, 16-byte units
-  d |= (uint64_t)0 << 16;                       // leading byte offset (unused, one K atom)
-  d |= (uint64_t)(1024 >> 4) << 32;             // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                       // version = 1
-  d |= (uint64_t)2 << 61;                       // layout type: SWIZZLE_128B
+  d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);          // start address, 16-byte units
+  d |= (uint64_t)1 << 16;                               // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)((K2 == 64 ? 1024 : 512) >> 4) << 32;  // stride byte offset between 8-row groups
+  d |= (uint64_t)(K2 == 64 ? 1 : 2) << 62;              // 1: 128B swizzle, 2: 64B swizzle
   return d;
 }
-// Instruction descriptor for kind::f16: A,B = fp16 (format 0), D = fp32, both K-major.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4)                    // c_format = F32
-         | (0u << 7) | (0u << 10)     // a_format = b_format = F16
-         | (0u << 15) | (0u << 16)    // a_major = b_major = K
-         | ((uint32_t)(N >> 3) << 17) // n_dim
-         | ((uint32_t)(M >> 4) << 24);// m_dim
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// D[64 x 64] += A[64 x 16] * B[64 x 16]^T, fp16 operands, fp32 accumulate.  Fragment of thread t
+// (warp w = t / 32 of the warpgroup, lane l): d[i] is row 16 w + l / 4 + 8 ((i / 2) & 1), column
+// 8 (i / 4) + 2 (l & 3) + (i & 1).
+__device__ __forceinline__ void wgmma_64x64(float (&d)[32], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b));
+}
+// Same with A from registers: a[0..3] are the packed fp16 pairs of the A fragment, which has the layout of the
+// accumulator fragment of columns 16 k .. 16 k + 15 (a[0] = d[8k..8k+1], a[1] = d[8k+2..3], a[2] = d[8k+4..5],
+// a[3] = d[8k+6..7]): an accumulator converts into the next MMA's A operand without leaving the registers.
+__device__ __forceinline__ void wgmma_64x64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, 1, 1, 1, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b));
+}
+// Named barrier over the 128 threads of warpgroup `wg` (ids 2.. are free; 0 is __syncthreads, 1 bar_compute).
+__device__ __forceinline__ void bar_wg(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }
+
 // Byte offset of 16-byte chunk `c16` (0..7) of row `r` inside a 128B-swizzled tile whose rows are
 // 128 bytes (64 fp16): Swizzle<3,4,3> -- XOR the chunk index with (row mod 8).
 __host__ __device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t c16) {
@@ -304,16 +286,6 @@ __host__ __device__ __forceinline__ uint32_t swk_offset(uint32_t r, uint32_t c16
   if constexpr (K2 == 64) return r * 128u + ((c16 ^ (r & 7u)) << 4);
   else return r * 64u + ((c16 ^ ((r >> 1) & 3u)) << 4);  // Swizzle<2,4,3>: bits[5:4] ^= bits[8:7]
 }
-template <int K2>
-__device__ __forceinline__ uint64_t make_swk_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3ffff) >> 4);
-  d |= (uint64_t)((K2 == 64 ? 1024 : 512) >> 4) << 32;  // stride between 8-row groups
-  d |= (uint64_t)1 << 46;                                // descriptor version 1
-  d |= (uint64_t)(K2 == 64 ? 2 : 4) << 61;               // SWIZZLE_128B : SWIZZLE_64B
-  return d;
-}
-
 // fp16 hi/lo split of a non-negative-or-signed fp32 value: x ~= hi + lo, relative error 2^-22.
 __device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   __half2 h = __floats2half2_rn(x0, x1);

@@ -1,19 +1,23 @@
-// fused.cu -- the general-shape scoring kernel (fused_tc.cu is the headline kernel for n_pad <= 256, d_pad <= 64)
-// and the launcher that picks between the three paths: per tile of 128 candidates
+// fused.cu -- the scoring kernel and its launcher: per tile of 128 candidates
 //   K* = k(X*, X)                       CUDA cores (fp32, GEMM-form distance + Matern/RBF epilogue)
 //   mu~ = c + K* alpha                  CUDA cores (fp32, folded into the K* pass)
-//   V = K* L^-T                         tcgen05 tensor cores, fp16 hi/lo split x3, fp32 accum in TMEM,
-//                                       lower-triangular structure of L^-1 skipped tile-wise
-//   var~ = k** - |V|^2 ; un-standardise  TMEM -> registers epilogue
+//   V = K* L^-T                         warpgroup MMAs (wgmma), fp16 hi/lo split x3, fp32 accumulators in
+//                                       registers, lower-triangular structure of L^-1 skipped tile-wise
+//   var~ = k** - |V|^2 ; un-standardise  from the accumulator registers
 //   q=1 acquisition value (MC or analytic) + running arg-max
-// K* never leaves the SM.  One persistent CTA per SM, warp-specialised:
-//   warps 0..15  compute (assembly, epilogue, MC)      warp 16  bulk-copy (TMA engine) producer
-//   warp 17      tcgen05.mma issuer (one elected lane)
+// K* never leaves the SM.  One persistent CTA per SM:
+//   warpgroups 0, 1   rows 0-63 / 64-127 of the tile: assemble their K* rows chunk by chunk (64 training
+//                     points), write the fp16 hi/lo chunk to shared memory and issue the MMAs of that chunk;
+//                     the next chunk is assembled while those MMAs run.  Then moments and acquisition.
+//   warp 8            bulk-copy (TMA engine) producer of the L^-1 tiles
+// A warpgroup holds a 64 x 128 panel of V (64 fp32 registers per thread); a model with n_pad > 128 takes
+// several column panels per tile, each re-forming the K* chunks it needs (chunk c feeds sub-blocks s >= c).
 //
 // Reference path replaced: one chunk loop of botorch.optim.optimize_acqf_discrete
-// (/root/reference/baybe/recommenders/pure/bayesian/botorch/discrete.py:124-126) =
-// acqf(X[chunk].unsqueeze(-2)) -> SingleTaskGP.posterior (gaussian_process/core.py:268-269)
-// -> qLogExpectedImprovement.forward (class chosen at acquisition/base.py:162-181).
+// (baybe/recommenders/pure/bayesian/botorch/discrete.py) = acqf(X[chunk].unsqueeze(-2)) ->
+// SingleTaskGP.posterior (surrogates/gaussian_process/core.py) -> qLogExpectedImprovement.forward
+// (class chosen in acquisition/base.py).
+#include <cuda.h>
 #include <stdlib.h>
 
 #include "assemble.cuh"
@@ -21,9 +25,14 @@
 
 namespace bb {
 
-// Everything the compute warps keep in shared memory, carved from the dynamic allocation.
+// Tensor-core distances: K extent K2 = 32 (d <= 30) or 64 (d <= 62), the data columns followed by |a|^2 P and P1 in the
+// last two; one fp16 panel of 64 candidate rows is 64 x K2 x 2 bytes.
+template <int K2>
+__host__ __device__ constexpr uint32_t tc_panel() { return 64u * K2 * 2u; }
+
+// Everything the kernel keeps in shared memory, carved from the dynamic allocation.
 struct FusedSmem {
-  uint8_t *ring_a, *ring_b;
+  uint8_t *ring_b, *abuf;
   float4* xt4;
   float *tsq, *alpha_s;
   int32_t* ttask;
@@ -31,112 +40,235 @@ struct FusedSmem {
   float *z_s, *mean_part, *var_part, *mc_part, *tcov, *meanc;
   int32_t* cand_task;
   float *cscale_s, *cshift_s;
-  uint64_t *a_full, *a_empty, *b_full, *b_empty, *d_full, *d_empty;
-  uint32_t* tmem_ptr;
-  float* zstat;
+  uint8_t *bt, *a2;  // tensor-core distances: training image, per-warpgroup candidate panels
+  float* an_x;       // [2][128] |a|^2 halves of the candidate rows
+  uint64_t *b_full, *b_empty;
   long long* best_red;
+  float* zstat;
+  volatile unsigned* ready_cache;
 };
 
-__device__ __forceinline__ FusedSmem carve_fused(uint8_t* base, const FusedParams& p) {
-  FusedSmem s;
-  uint8_t* cur = base;
-  s.ring_a = cur;
-  cur += (size_t)p.slots_a * kSlotABytes;
-  s.ring_b = cur;
-  cur += (size_t)p.stages_b * p.stage_b_bytes;
-  s.xt4 = reinterpret_cast<float4*>(cur);
-  cur += (size_t)p.n_pad * p.d_pad * 4;
-  s.tsq = reinterpret_cast<float*>(cur);
-  cur += p.n_pad * 4;
-  s.alpha_s = reinterpret_cast<float*>(cur);
-  cur += p.n_pad * 4;
-  s.ttask = reinterpret_cast<int32_t*>(cur);
-  cur += p.n_pad * 4;
-  s.a_s = reinterpret_cast<float4*>(cur);
-  cur += (size_t)kTileM * p.d_pad * 8;  // duplicated candidate values
-  s.z_s = reinterpret_cast<float*>(cur);
-  cur += kMaxSamples * 4;
-  s.mean_part = reinterpret_cast<float*>(cur);  // [2][8][128]
-  cur += 2 * 8 * kTileM * 4;
-  s.var_part = reinterpret_cast<float*>(cur);   // [4][128]
-  cur += 4 * kTileM * 4;
-  s.mc_part = reinterpret_cast<float*>(cur);    // [4][128][2]
-  cur += 4 * kTileM * 2 * 4;
-  s.tcov = reinterpret_cast<float*>(cur);
-  cur += kMaxTasks * kMaxTasks * 4;
-  s.meanc = reinterpret_cast<float*>(cur);
-  cur += kMaxTasks * 4;
-  s.cand_task = reinterpret_cast<int32_t*>(cur);  // [2][128]
-  cur += 2 * kTileM * 4;
-  s.cscale_s = reinterpret_cast<float*>(cur);
-  cur += ((p.d_pad * 4 + 15) / 16) * 16;
-  s.cshift_s = reinterpret_cast<float*>(cur);
-  cur += ((p.d_pad * 4 + 15) / 16) * 16;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(cur);
-  s.a_full = bars;                          // [kMaxSlotsA]
-  s.a_empty = s.a_full + kMaxSlotsA;        // [kMaxSlotsA]
-  s.b_full = s.a_empty + kMaxSlotsA;        // [kMaxStagesB]
-  s.b_empty = s.b_full + kMaxStagesB;       // [kMaxStagesB]
-  s.d_full = s.b_empty + kMaxStagesB;       // [2]
-  s.d_empty = s.d_full + 2;                 // [2]
-  cur += 32 * 8;
-  s.best_red = reinterpret_cast<long long*>(cur);  // [4]
-  cur += 32;
-  s.tmem_ptr = reinterpret_cast<uint32_t*>(cur);
-  s.zstat = reinterpret_cast<float*>(cur + 8);  // mean z, mean |z - mean z|
-  return s;
+// stages_b = number of L^-1 tiles in flight; returns the byte count (base == nullptr: size only)
+static __host__ __device__ size_t carve_fused(uint8_t* base, const FusedParams& p, FusedSmem* s) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    const size_t o = off;
+    off += (bytes + 15) / 16 * 16;
+    return base + o;
+  };
+  uint8_t* ring_b = take((size_t)p.stages_b * kStageBBytes);  // first: 1024-byte aligned swizzled tiles
+  uint8_t* abuf = take(p.tc ? 0 : (size_t)kConsumerWGs * kABytes);
+  uint8_t* bt = take((size_t)3 * p.n_pad * p.tc * 2);  // 1024-byte aligned: swizzle atoms
+  uint8_t* a2 = take((size_t)kConsumerWGs * 3 * 64 * p.tc * 2);
+  uint8_t* an_x = take(p.tc ? 2 * kTileM * 4 : 0);
+  uint8_t* xt4 = take(p.tc ? 0 : (size_t)p.n_pad * p.d_pad * 4);
+  uint8_t* tsq = take((size_t)p.n_pad * 4);
+  uint8_t* alpha_s = take((size_t)p.n_pad * 4);
+  uint8_t* ttask = take((size_t)p.n_pad * 4);
+  uint8_t* a_s = take(p.tc ? 0 : (size_t)kTileM * p.d_pad * 8);  // duplicated candidate values
+  uint8_t* z_s = take(kMaxSamples * 4);
+  uint8_t* mean_part = take(4 * kTileM * 4);          // [4 octet groups][128]
+  uint8_t* var_part = take(kTileM * 4);
+  uint8_t* mc_part = take(1024 * 4);                  // qLogEI table + exact rows, or [2 groups][128][2]
+  uint8_t* tcov = take(kMaxTasks * kMaxTasks * 4);
+  uint8_t* meanc = take(kMaxTasks * 4);
+  uint8_t* cand_task = take(kTileM * 4);
+  uint8_t* cscale = take((size_t)p.d_pad * 4);
+  uint8_t* cshift = take((size_t)p.d_pad * 4);
+  uint8_t* bars = take(2 * kMaxStagesB * 8);
+  uint8_t* best = take(4 * 8);
+  uint8_t* misc = take(16);
+  if (s != nullptr) {
+    s->ring_b = ring_b;
+    s->abuf = abuf;
+    s->bt = bt;
+    s->a2 = a2;
+    s->an_x = reinterpret_cast<float*>(an_x);
+    s->xt4 = reinterpret_cast<float4*>(xt4);
+    s->tsq = reinterpret_cast<float*>(tsq);
+    s->alpha_s = reinterpret_cast<float*>(alpha_s);
+    s->ttask = reinterpret_cast<int32_t*>(ttask);
+    s->a_s = reinterpret_cast<float4*>(a_s);
+    s->z_s = reinterpret_cast<float*>(z_s);
+    s->mean_part = reinterpret_cast<float*>(mean_part);
+    s->var_part = reinterpret_cast<float*>(var_part);
+    s->mc_part = reinterpret_cast<float*>(mc_part);
+    s->tcov = reinterpret_cast<float*>(tcov);
+    s->meanc = reinterpret_cast<float*>(meanc);
+    s->cand_task = reinterpret_cast<int32_t*>(cand_task);
+    s->cscale_s = reinterpret_cast<float*>(cscale);
+    s->cshift_s = reinterpret_cast<float*>(cshift);
+    s->b_full = reinterpret_cast<uint64_t*>(bars);
+    s->b_empty = s->b_full + kMaxStagesB;
+    s->best_red = reinterpret_cast<long long*>(best);
+    s->zstat = reinterpret_cast<float*>(misc);  // mean z, mean |z - mean z|
+    s->ready_cache = reinterpret_cast<volatile unsigned*>(misc + 8);
+  }
+  return off;
 }
 
-static size_t fused_smem_bytes(const FusedParams& p) {
-  size_t b = 0;
-  b += (size_t)p.slots_a * kSlotABytes + (size_t)p.stages_b * p.stage_b_bytes;
-  b += (size_t)p.n_pad * p.d_pad * 4 + (size_t)p.n_pad * 12;
-  b += (size_t)kTileM * p.d_pad * 8 + kMaxSamples * 4;
-  b += 2 * 8 * kTileM * 4 + 4 * kTileM * 4 + 4 * kTileM * 2 * 4;
-  b += kMaxTasks * kMaxTasks * 4 + kMaxTasks * 4 + 2 * kTileM * 4;
-  b += 2 * (size_t)(((p.d_pad * 4 + 15) / 16) * 16);
-  b += 32 * 8 + 32 + 32;
-  return b;
+static size_t fused_smem_bytes(const FusedParams& p) { return carve_fused(nullptr, p, nullptr); }
+
+// Position of L^-1 tile (chunk c, sub-block sb >= c) in the c-major image of C chunks.
+__host__ __device__ __forceinline__ size_t rimg_tile(int c, int sb, int C) {
+  return (size_t)c * C - (size_t)c * (c - 1) / 2 + (size_t)(sb - c);
 }
 
-// LAG = 1: the epilogue of tile t runs after the assembly of tile t+1, so the tensor-core tail of
-// tile t is never waited for; needs two accumulators in TMEM (2 * n_pad <= 512 columns).
-// PRE = true (wide-feature path): the K* block was materialised by k_kmat_tc (wide.cu) and is read from
+// Gated pass: block until the copy stream has published the rows of `tile` (acquire at system scope: the data
+// was written by the copy engine before the counter).  Bounded: after ~2 s the status word is raised and the
+// kernel carries on (the host reports the pass as failed) -- a missing publication must not hang the GPU.
+// One thread per CTA polls and hands the value to the other consumer threads through shared memory; it is kept
+// in a register, since publications run far ahead of the tiles.  Called by all 256 consumer threads.
+__device__ __forceinline__ unsigned wait_rows(const FusedParams& p, volatile unsigned* cache_s, int tile, unsigned have) {
+  const long long last = (long long)(tile + 1) * kTileM;
+  const unsigned need = (unsigned)(last < p.N ? last : p.N);
+  if (have >= need) return have;
+  if (threadIdx.x == 0) {
+    unsigned v;
+    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p.ready_rows) : "memory");
+    if (v < need) {
+      unsigned long long t0, t1;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+      while (true) {
+        __nanosleep(256);
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p.ready_rows) : "memory");
+        if (v >= need) break;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
+        if (t1 - t0 > 2000000000ull) {
+          if (p.gate_status != nullptr) *p.gate_status = 1;
+          v = 0xffffffffu;  // give up waiting for good: the pass is reported as failed
+          break;
+        }
+      }
+    }
+    *cache_s = v;
+  }
+  bar_compute();  // also orders the other threads' loads of the rows behind thread 0's acquire
+  const unsigned v = *cache_s;
+  bar_compute();  // the word may be rewritten by the next call
+  return v;
+}
+
+// Tensor-core distances: warpgroup `wg` writes its 64 candidate rows of the tile at row0 as [sa a | |a|^2 P | P1] in
+// fp16 hi/mid/lo panels of K2 columns (a2w: three panels).  Thread t (r = t & 63, h = t >> 6) owns row r and the
+// dimension quads h K2/8 .. (h + 1) K2/8 - 1; the owner of the last quad appends |a|^2 P and P1.  Called by the 128
+// threads of the warpgroup; ends with the panels visible to the tensor cores.
+template <int K2>
+__device__ __forceinline__ void tc_stage_rows(const FusedParams& p, const StageCtx& sc, int64_t row0, int wg, int t,
+                                              uint8_t* a2w, float* an_x, int32_t* cand_task, const float* cscale,
+                                              const float* cshift) {
+  constexpr int QT = K2 / 8, QL = K2 / 4 - 1;  // quads per thread, last quad
+  constexpr uint32_t kPanel = tc_panel<K2>();
+  const int r = t & 63, h = t >> 6, tr = 64 * wg + r;
+  const int64_t row = row0 + tr;
+  const int dq = p.d_pad >> 2;
+  float an = 0.f, al[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+  for (int u = 0; u < QT; ++u) {
+    const int jq = QT * h + u, j0 = 4 * jq;
+    float a[4] = {0.f, 0.f, 0.f, 0.f};
+    if (jq < dq) {
+      const float4 q = stage_load_quad(sc, row, jq, row < p.N);
+      if (p.task_col >= j0 && p.task_col < j0 + 4) {
+        const float tv = (p.task_col == j0) ? q.x : (p.task_col == j0 + 1) ? q.y : (p.task_col == j0 + 2) ? q.z : q.w;
+        cand_task[tr] = min(max(__float2int_rn(tv), 0), p.n_tasks - 1);
+      }
+      a[0] = fmaf(q.x, cscale[j0], cshift[j0]);
+      a[1] = fmaf(q.y, cscale[j0 + 1], cshift[j0 + 1]);
+      a[2] = fmaf(q.z, cscale[j0 + 2], cshift[j0 + 2]);
+      a[3] = fmaf(q.w, cscale[j0 + 3], cshift[j0 + 3]);
+      an = fmaf(a[0], a[0], fmaf(a[1], a[1], fmaf(a[2], a[2], fmaf(a[3], a[3], an))));
+#pragma unroll
+      for (int e = 0; e < 4; ++e) a[e] *= p.ts_sa;  // exact: power of two
+    }
+    if (jq == QL) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) al[e] = a[e];
+    } else {
+      uint2 hi, mid, lo;
+      split3_quad(a, hi, mid, lo);
+      const uint32_t off = swk_offset<K2>((uint32_t)r, (uint32_t)(jq >> 1)) + (uint32_t)(jq & 1) * 8u;
+      *reinterpret_cast<uint2*>(a2w + off) = hi;
+      *reinterpret_cast<uint2*>(a2w + kPanel + off) = mid;
+      *reinterpret_cast<uint2*>(a2w + 2 * kPanel + off) = lo;
+    }
+  }
+  an_x[h * kTileM + tr] = an;
+  bar_wg(wg);
+  if (h == 1) {
+    al[2] = (an_x[tr] + an_x[kTileM + tr]) * p.ts_aug_sq;
+    al[3] = p.ts_aug_one;
+    uint2 hi, mid, lo;
+    split3_quad(al, hi, mid, lo);
+    const uint32_t off = swk_offset<K2>((uint32_t)r, (uint32_t)(QL >> 1)) + 8u;
+    *reinterpret_cast<uint2*>(a2w + off) = hi;
+    *reinterpret_cast<uint2*>(a2w + kPanel + off) = mid;
+    *reinterpret_cast<uint2*>(a2w + 2 * kPanel + off) = lo;
+  }
+  fence_proxy_async();
+  bar_wg(wg);
+}
+
+// D[64 x 64] = A2 (a warpgroup's 64 rows) . Bt(64 training rows)^T: six fp16 split products over K2 (issued and
+// committed, not waited for).
+template <int K2>
+__device__ __forceinline__ void tc_distances(float (&dacc)[32], uint32_t a2_addr, uint32_t bt_addr, uint32_t bsplit) {
+  constexpr uint32_t kPanel = tc_panel<K2>();
+#pragma unroll
+  for (int i = 0; i < 32; ++i) dacc[i] = 0.f;
+  wg_fence();
+#pragma unroll
+  for (int kk = 0; kk < K2 / 16; ++kk) {
+    const uint64_t ko = (uint64_t)(kk * 2);
+    const uint64_t ah = make_wg_desc<K2>(a2_addr) + ko, am = make_wg_desc<K2>(a2_addr + kPanel) + ko,
+                   al = make_wg_desc<K2>(a2_addr + 2 * kPanel) + ko;
+    const uint64_t bh = make_wg_desc<K2>(bt_addr) + ko, bm = make_wg_desc<K2>(bt_addr + bsplit) + ko,
+                   bl = make_wg_desc<K2>(bt_addr + 2 * bsplit) + ko;
+    wgmma_64x64(dacc, ah, bh);
+    wgmma_64x64(dacc, ah, bm);
+    wgmma_64x64(dacc, am, bh);
+    wgmma_64x64(dacc, ah, bl);
+    wgmma_64x64(dacc, al, bh);
+    wgmma_64x64(dacc, am, bm);
+  }
+  wg_commit();
+}
+
+// PRE = true (wide-feature path): the K* block was materialised by k_kmat_wg (wide.cu) and is read from
 // p.kpre instead of being assembled here; FAMILY is then irrelevant.
-// GMAX: L^-1 sub-blocks (64 output columns each) per ring stage / per MMA (N = 64 * group): every SS-form
-// tcgen05.mma re-reads its A slice from shared memory whatever N is, so wider groups cut the MMA time.
-template <int FAMILY, int LAG, bool PRE, int GMAX>
+// TCK = 32 / 64 (n_pad <= 256, d <= 62, Matern-3/2, -5/2, RBF): the distances of a chunk come from an augmented GEMM on
+// the tensor cores, and its accumulator, converted to kernel values in registers, is the register A operand of the
+// chunk's V MMAs.  Otherwise the distances run on the CUDA cores and the K* chunk goes through shared memory.
+template <int FAMILY, bool PRE, int TCK>
 __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p) {
+  constexpr bool TC = TCK > 0;
+  constexpr int K2 = TC ? TCK : 32;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const FusedSmem s = carve_fused(smem_raw, p);
+  FusedSmem s;
+  carve_fused(smem_raw, p, &s);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int C = p.c_count;  // K* chunks feeding this launch's column panel
-  const int ncol = (p.sb_hi - p.sb_lo) * kChunk;  // V columns of the panel
+  const int C = p.n_chunks;
   const int dq = p.d_pad >> 2;
   if (tid == 0 && (smem_u32(smem_raw) & 1023u) != 0u) __trap();  // swizzled tiles need 1024-B alignment
 
   // ---- one-time setup ----
-  if (warp == kWarpMma && lane == 0) {
-    for (int i = 0; i < p.slots_a; ++i) {
-      mbar_init(&s.a_full[i], kComputeWarps);
-      mbar_init(&s.a_empty[i], 1);
-    }
+  if (tid == 0) {
     for (int i = 0; i < p.stages_b; ++i) {
       mbar_init(&s.b_full[i], 1);
-      mbar_init(&s.b_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s.d_full[i], 1);
-      mbar_init(&s.d_empty[i], kComputeWarps);
+      mbar_init(&s.b_empty[i], kConsumerWGs);
     }
     fence_mbar_init();
   }
-  if (warp == kWarpProducer) {
-    tmem_alloc(s.tmem_ptr, p.tmem_cols);
-    tmem_relinquish();
-  }
   // model data resident in shared memory for the whole kernel
-  if constexpr (!PRE) load_train_rows(s.xt4, p.train_m2, p.n_pad, dq, tid, kFusedThreads);
+  if constexpr (TC) {
+    const uint4* src = reinterpret_cast<const uint4*>(p.timg_b);
+    uint4* dst = reinterpret_cast<uint4*>(s.bt);
+    for (int e = tid; e < 3 * p.n_pad * K2 * 2 / 16; e += kFusedThreads) dst[e] = __ldg(src + e);
+    for (int e = tid; e < 4 * kTileM; e += kFusedThreads) s.mean_part[e] = 0.f;  // only group 0 is written
+    fence_proxy_async();  // read by the tensor cores
+  } else if constexpr (!PRE) {
+    load_train_rows(s.xt4, p.train_m2, p.n_pad, dq, tid, kFusedThreads);
+  }
   for (int e = tid; e < p.d_pad; e += kFusedThreads) {
     s.cscale_s[e] = __ldg(p.cand_scale + e);
     s.cshift_s[e] = __ldg(p.cand_shift + e);
@@ -148,13 +280,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
   }
   for (int e = tid; e < p.n_tasks * p.n_tasks; e += kFusedThreads) s.tcov[e] = __ldg(p.task_covar + e);
   for (int e = tid; e < p.n_tasks; e += kFusedThreads) s.meanc[e] = __ldg(p.mean_const + e);
-  for (int e = tid; e < 2 * kTileM; e += kFusedThreads) s.cand_task[e] = 0;
+  for (int e = tid; e < kTileM; e += kFusedThreads) s.cand_task[e] = 0;
   if (p.has_acq && p.z != nullptr)
     for (int e = tid; e < p.S; e += kFusedThreads) s.z_s[e] = __ldg(p.z + e);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s.tmem_ptr;
   if (p.has_acq && warp == 0) {
     float sz = 0.f, sa = 0.f;
     for (int e = lane; e < p.S; e += 32) sz += s.z_s[e];
@@ -168,23 +297,26 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
     }
   }
 
-  // qLogEI: tabulated fat-tail sum (acq_math.cuh), as in fused_tc.cu.  The K*-reading variant is launched once per
-  // 37,888-row block of the wide path: rebuilding the table in every CTA of every short launch cost more than it
-  // saved (config-4 shard 5.3 -> 5.7 ms), so there the table is built once per call by k_mc_table and only copied.
-  const bool fast_mc = PRE ? (p.mc_table != nullptr) : mc_table_applicable(p.has_acq, p.acq, p.S);
-  if (fast_mc) {
-    if constexpr (PRE) {
-      for (int e = tid; e < kMcRows; e += kFusedThreads) s.mc_part[e] = __ldg(p.mc_table + e);
-      __syncthreads();
-    } else {
-      mc_table_setup(s.mc_part, s.z_s, p.S, p.acq.obj_scale < 0.f ? -1.f : 1.f);
-    }
+  // qLogEI: tabulated fat-tail sum (acq_math.cuh).  Built once per call by k_mc_table(_grid) where a launch has
+  // many CTAs (rebuilding it in every persistent CTA costs more than it saves), else here.
+  const bool fast_mc = p.mc_table != nullptr || (!PRE && mc_table_applicable(p.has_acq, p.acq, p.S));
+  if (p.mc_table != nullptr) {
+    asm volatile("griddepcontrol.wait;" ::: "memory");  // the table kernel may still be running (dependent launch)
+    for (int e = tid; e < kMcRows; e += kFusedThreads) s.mc_part[e] = __ldcg(p.mc_table + e);
+    __syncthreads();
+  } else if (fast_mc) {
+    mc_table_setup(s.mc_part, s.z_s, p.S, p.acq.obj_scale < 0.f ? -1.f : 1.f);
   }
 
-  if (warp < kComputeWarps) {
+  if (warp < kWarpProducer) {
     // =====================================================================================
-    // compute warps
+    // consumer warpgroups
     // =====================================================================================
+    const int wg = warp >> 2, t = tid & 127;
+    const int mp = t & 31, g = t >> 5;           // assembly: rows m0 = 64 wg + mp and m0 + 32, octets g, g + 4
+    const int m0 = 64 * wg + mp, m1 = m0 + 32;
+    const int row_e = tid & 127, sg = tid >> 7;  // epilogue: candidate row, sample group
+    const int ra = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // accumulator rows ra, ra + 8
     AsmSmem sm;
     sm.xt4 = s.xt4;
     sm.tsq = s.tsq;
@@ -205,56 +337,237 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
     sc.task_col = p.task_col;
     sc.cscale = s.cscale_s;
     sc.cshift = s.cshift_s;
-    sc.groups = kComputeThreads / kTileM;
+    sc.groups = kConsumerThreads / kTileM;
+    sc.gated = p.ready_rows != nullptr;
+    sc.code_table = p.code_table;
+    sc.code_table_ld = p.code_table_ld;
+    uint8_t* abuf = s.abuf + wg * kABytes;
+    const uint64_t a_hi = make_wg_desc<64>(smem_u32(abuf)), a_lo = make_wg_desc<64>(smem_u32(abuf + 8192));
+    const uint32_t ring_addr = smem_u32(s.ring_b);
+    uint32_t bcount = 0;  // L^-1 tiles consumed so far: ring slot bcount % stages_b, phase (bcount / stages_b) & 1
+    unsigned rows_have = 0;
     StageRegs regs;
+    uint8_t* a2w = s.a2 + wg * 3 * tc_panel<K2>();
     if constexpr (!PRE)
-      if ((int)blockIdx.x < p.num_tiles) stage_prefetch(sc, dq, (int64_t)blockIdx.x * kTileM, tid, regs);
-    const int mp = tid & 63, g = tid >> 6;       // assembly: candidates (mp, mp+64), i-octet g
-    const int row_e = tid & 127, sg = tid >> 7;  // epilogue: TMEM lane row_e, column/sample group
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
+      if ((int)blockIdx.x < p.num_tiles) {
+        if (sc.gated) rows_have = wait_rows(p, s.ready_cache, blockIdx.x, rows_have);
+        if constexpr (!TC) stage_prefetch(sc, dq, (int64_t)blockIdx.x * kTileM, tid, regs);
+      }
     long long best = kEmptyKey;
 
-    // ---- epilogue of tile number e_it (rows e_row0..): |V|^2 from TMEM, moments, acquisition ----
-    auto epilogue = [&](int e_it, int64_t e_row0) {
-      const int buf = LAG ? (e_it & 1) : 0;
-      const int use = LAG ? (e_it >> 1) : e_it;
-      mbar_wait(&s.d_full[buf], (uint32_t)(use & 1));
-      tc_fence_after();
-      {
-        float ss = 0.f;
-        const uint32_t col0 = tmem_base + lane_base + (uint32_t)(buf * ncol);
-        for (int cb = sg; cb * 32 < ncol; cb += 4) {
-          float v[32];
-          tmem_ld32(col0 + (uint32_t)(cb * 32), v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 32; ++e) ss = fmaf(v[e], v[e], ss);
+    int it = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+      const int64_t row0 = (int64_t)tile * kTileM;
+      if (tid == 0) trace_ev(p, it, 0);
+      float an0 = 0.f, an1 = 0.f;
+      if constexpr (PRE) {
+        if (p.task_col >= 0 && tid < kTileM) {  // task id of each candidate row (mean constant, prior variance)
+          const int64_t row = row0 + tid;
+          float tv = 0.f;
+          if (row < p.N) {
+            switch (p.layout) {
+              case BB_ROW_MAJOR_F32: tv = load_x<BB_ROW_MAJOR_F32>(p.x, row, p.task_col, p.ldx); break;
+              case BB_COL_MAJOR_F32: tv = load_x<BB_COL_MAJOR_F32>(p.x, row, p.task_col, p.ldx); break;
+              case BB_ROW_MAJOR_F64: tv = load_x<BB_ROW_MAJOR_F64>(p.x, row, p.task_col, p.ldx); break;
+              default: tv = load_x<BB_COL_MAJOR_F64>(p.x, row, p.task_col, p.ldx); break;
+            }
+          }
+          s.cand_task[tid] = min(max(__float2int_rn(tv), 0), p.n_tasks - 1);
         }
-        s.var_part[sg * kTileM + row_e] = ss;
+        bar_compute();
+      } else if constexpr (TC) {
+        tc_stage_rows<K2>(p, sc, row0, wg, t, a2w, s.an_x, s.cand_task, s.cscale_s, s.cshift_s);
+      } else {
+        stage_commit(sc, s.a_s, s.cand_task, p.n_tasks, dq, row0, tid, regs);
+        bar_compute();
+        an0 = cand_sqnorm(sm, m0);
+        an1 = cand_sqnorm(sm, m1);
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s.d_empty[buf]);
+      float mean0 = 0.f, mean1 = 0.f, vq0 = 0.f, vq1 = 0.f;
+      for (int lo = 0; lo < C; lo += kPanelSB) {
+        const int hi = min(C, lo + kPanelSB);
+        const bool last_panel = hi == C;  // covers every chunk: the mean is formed here
+        float acc[kPanelSB][32];
+#pragma unroll
+        for (int j = 0; j < kPanelSB; ++j)
+#pragma unroll
+          for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+        uint32_t b_prev = 0, n_prev = 0;  // tiles read by the MMAs in flight
+        for (int c = 0; c < hi; ++c) {
+          uint32_t ahi[4][4], alo[4][4];  // TC: the chunk's K* as the register A operand, one [4] per 16 k
+          if constexpr (TC) {
+            float dacc[32];
+            tc_distances<K2>(dacc, smem_u32(a2w), smem_u32(s.bt) + (uint32_t)c * tc_panel<K2>(),
+                             (uint32_t)p.n_pad * K2 * 2u);
+            wg_wait<0>();  // also completes the previous chunk's V MMAs: release their L^-1 tiles
+            if (t == 0)
+              for (uint32_t q = 0; q < n_prev; ++q) mbar_arrive(&s.b_empty[(b_prev + q) % (uint32_t)p.stages_b]);
+            // kernel values in the accumulator layout = the A-fragment layout of the V MMAs
+            const float* tc0 = s.tcov + s.cand_task[ra] * p.n_tasks;
+            const float* tc1 = s.tcov + s.cand_task[ra + 8] * p.n_tasks;
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+              for (int q = 0; q < 4; ++q) {
+                const int i = 8 * kk + 2 * q;
+                const int col = c * kChunk + 8 * (i >> 2) + 2 * (lane & 3);
+                const bool upper = (q & 1) != 0;  // accumulator rows ra + 8
+                float k0 = kernel_from_t<FAMILY>(dacc[i] * p.ts_g), k1 = kernel_from_t<FAMILY>(dacc[i + 1] * p.ts_g);
+                if (p.scaled) {
+                  const float* tcr = upper ? tc1 : tc0;
+                  k0 *= tcr[s.ttask[col]];
+                  k1 *= tcr[s.ttask[col + 1]];
+                }
+                if (last_panel) {
+                  const float2 al = *reinterpret_cast<const float2*>(s.alpha_s + col);
+                  const float mp = fmaf(k0, al.x, k1 * al.y);
+                  if (upper) mean1 += mp;
+                  else mean0 += mp;
+                }
+                split_pair(k0 * p.ts_kscale, k1 * p.ts_kscale, ahi[kk][q], alo[kk][q]);
+              }
+          } else {
+            uint4 h0[2], l0[2], h1[2], l1[2];
+  #pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const int i0 = c * kChunk + (g + 4 * u) * 8;
+              float k0[8], k1[8];
+              if constexpr (PRE) {
+                const float4* q0 = reinterpret_cast<const float4*>(p.kpre + (row0 + m0) * p.ldk + i0);
+                const float4* q1 = reinterpret_cast<const float4*>(p.kpre + (row0 + m1) * p.ldk + i0);
+                const float4 x0 = __ldg(q0), x1 = __ldg(q0 + 1), y0 = __ldg(q1), y1 = __ldg(q1 + 1);
+                k0[0] = x0.x; k0[1] = x0.y; k0[2] = x0.z; k0[3] = x0.w;
+                k0[4] = x1.x; k0[5] = x1.y; k0[6] = x1.z; k0[7] = x1.w;
+                k1[0] = y0.x; k1[1] = y0.y; k1[2] = y0.z; k1[3] = y0.w;
+                k1[4] = y1.x; k1[5] = y1.y; k1[6] = y1.z; k1[7] = y1.w;
+              } else {
+                assemble_2x8<FAMILY>(sm, m0, m1, an0, an1, i0, k0, k1);
+              }
+              if (last_panel) {
+                const float4 al0 = *reinterpret_cast<const float4*>(s.alpha_s + i0);
+                const float4 al1 = *reinterpret_cast<const float4*>(s.alpha_s + i0 + 4);
+                const float al[8] = {al0.x, al0.y, al0.z, al0.w, al1.x, al1.y, al1.z, al1.w};
+  #pragma unroll
+                for (int ii = 0; ii < 8; ++ii) {
+                  mean0 = fmaf(k0[ii], al[ii], mean0);
+                  mean1 = fmaf(k1[ii], al[ii], mean1);
+                }
+              }
+              split_pair(k0[0], k0[1], h0[u].x, l0[u].x);
+              split_pair(k0[2], k0[3], h0[u].y, l0[u].y);
+              split_pair(k0[4], k0[5], h0[u].z, l0[u].z);
+              split_pair(k0[6], k0[7], h0[u].w, l0[u].w);
+              split_pair(k1[0], k1[1], h1[u].x, l1[u].x);
+              split_pair(k1[2], k1[3], h1[u].y, l1[u].y);
+              split_pair(k1[4], k1[5], h1[u].z, l1[u].z);
+              split_pair(k1[6], k1[7], h1[u].w, l1[u].w);
+            }
+            // the previous chunk's MMAs are done: the A buffer and their L^-1 tiles are free
+            wg_wait<0>();
+            if (t == 0)
+              for (uint32_t q = 0; q < n_prev; ++q) mbar_arrive(&s.b_empty[(b_prev + q) % (uint32_t)p.stages_b]);
+            bar_wg(wg);
+  #pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const uint32_t o0 = sw128_offset((uint32_t)mp, (uint32_t)(g + 4 * u));
+              const uint32_t o1 = sw128_offset((uint32_t)(mp + 32), (uint32_t)(g + 4 * u));
+              *reinterpret_cast<uint4*>(abuf + o0) = h0[u];
+              *reinterpret_cast<uint4*>(abuf + 8192 + o0) = l0[u];
+              *reinterpret_cast<uint4*>(abuf + o1) = h1[u];
+              *reinterpret_cast<uint4*>(abuf + 8192 + o1) = l1[u];
+            }
+            fence_proxy_async();  // generic-proxy writes -> visible to the tensor-core (async) proxy
+            bar_wg(wg);
+          }
+          // V[:, sb] += K*[:, chunk c] Linv[sb, chunk c]^T for the panel's sub-blocks sb >= c
+          const int s0 = c > lo ? c : lo;
+          const uint32_t n_c = (uint32_t)(hi - s0);
+          for (uint32_t q = 0; q < n_c; ++q) {
+            const uint32_t idx = bcount + q;
+            mbar_wait(&s.b_full[idx % (uint32_t)p.stages_b], (idx / (uint32_t)p.stages_b) & 1u);
+          }
+          wg_fence();
+#pragma unroll
+          for (int j = 0; j < kPanelSB; ++j) {
+            const int sb = lo + j;
+            if (sb >= s0 && sb < hi) {
+              const uint32_t st = (bcount + (uint32_t)(sb - s0)) % (uint32_t)p.stages_b;
+              const uint32_t b_addr = ring_addr + st * kStageBBytes;
+              const uint64_t b_hi = make_wg_desc<64>(b_addr), b_lo = make_wg_desc<64>(b_addr + 8192);
+#pragma unroll
+              for (int kk = 0; kk < 4; ++kk) {
+                const uint64_t ko = (uint64_t)(kk * 2);  // 16 fp16 = 32 bytes = 2 x 16-byte units
+                if constexpr (TC) {
+                  wgmma_64x64_rs(acc[j], ahi[kk], b_hi + ko);
+                  wgmma_64x64_rs(acc[j], ahi[kk], b_lo + ko);
+                  wgmma_64x64_rs(acc[j], alo[kk], b_hi + ko);
+                } else {
+                  wgmma_64x64(acc[j], a_hi + ko, b_hi + ko);
+                  wgmma_64x64(acc[j], a_hi + ko, b_lo + ko);
+                  wgmma_64x64(acc[j], a_lo + ko, b_hi + ko);
+                }
+              }
+            }
+          }
+          wg_commit();
+          b_prev = bcount;
+          n_prev = n_c;
+          bcount += n_c;
+        }
+        wg_wait<0>();
+        if (t == 0)
+          for (uint32_t q = 0; q < n_prev; ++q) mbar_arrive(&s.b_empty[(b_prev + q) % (uint32_t)p.stages_b]);
+#pragma unroll
+        for (int j = 0; j < kPanelSB; ++j)
+          if (lo + j < hi)
+#pragma unroll
+            for (int i = 0; i < 32; i += 4) {
+              vq0 = fmaf(acc[j][i], acc[j][i], fmaf(acc[j][i + 1], acc[j][i + 1], vq0));
+              vq1 = fmaf(acc[j][i + 2], acc[j][i + 2], fmaf(acc[j][i + 3], acc[j][i + 3], vq1));
+            }
+      }
+      if (tid == 0) trace_ev(p, it, 1);
+      // |V|^2 per row: the four lanes of a quad hold the row's columns
+      vq0 += __shfl_xor_sync(0xffffffffu, vq0, 1);
+      vq0 += __shfl_xor_sync(0xffffffffu, vq0, 2);
+      vq1 += __shfl_xor_sync(0xffffffffu, vq1, 1);
+      vq1 += __shfl_xor_sync(0xffffffffu, vq1, 2);
+      if ((lane & 3) == 0) {
+        s.var_part[ra] = vq0;
+        s.var_part[ra + 8] = vq1;
+      }
+      if constexpr (TC) {  // rows ra, ra + 8: the four lanes of a quad hold the row's columns
+        mean0 += __shfl_xor_sync(0xffffffffu, mean0, 1);
+        mean0 += __shfl_xor_sync(0xffffffffu, mean0, 2);
+        mean1 += __shfl_xor_sync(0xffffffffu, mean1, 1);
+        mean1 += __shfl_xor_sync(0xffffffffu, mean1, 2);
+        if ((lane & 3) == 0) {
+          s.mean_part[ra] = mean0;
+          s.mean_part[ra + 8] = mean1;
+        }
+      } else {
+        s.mean_part[g * kTileM + m0] = mean0;
+        s.mean_part[g * kTileM + m1] = mean1;
+      }
+      // global loads of the next tile fly while the epilogue runs
+      if constexpr (!PRE)
+        if (tile + (int)gridDim.x < p.num_tiles) {
+          if (sc.gated) rows_have = wait_rows(p, s.ready_cache, tile + gridDim.x, rows_have);
+          if constexpr (!TC) stage_prefetch(sc, dq, (int64_t)(tile + gridDim.x) * kTileM, tid, regs);
+        }
       bar_compute();
-      // moments in original units
-      const float* mpart = s.mean_part + buf * 8 * kTileM;
-      const int ct = s.cand_task[buf * kTileM + row_e];
+
+      // ---- epilogue: moments in original units, acquisition, arg-max ----
+      const int ct = s.cand_task[row_e];
       float msum = s.meanc[ct];
 #pragma unroll
-      for (int gg = 0; gg < 8; ++gg) msum += mpart[gg * kTileM + row_e];
-      float vsum = (s.var_part[row_e] + s.var_part[kTileM + row_e]) +
-                   (s.var_part[2 * kTileM + row_e] + s.var_part[3 * kTileM + row_e]);
-      if (p.vacc_in != nullptr && e_row0 + row_e < p.N) vsum += p.vacc_in[e_row0 + row_e];
-      if (p.vacc_out != nullptr) {  // earlier column panel of a model with n_pad > 512: partial only
-        if (sg == 0 && e_row0 + row_e < p.N) p.vacc_out[e_row0 + row_e] = vsum;
-        bar_compute();  // partial buffers are rewritten by the next epilogue
-        return;
-      }
+      for (int gg = 0; gg < 4; ++gg) msum += s.mean_part[gg * kTileM + row_e];
+      const float vsum = s.var_part[row_e];
       const float kss = p.scaled ? s.tcov[ct * p.n_tasks + ct] : 1.0f;
       const float var_t = fmaxf(kss - vsum * p.inv_r_scale2, 1e-10f);
       const float mu = fmaf(p.y_std, msum, p.y_mean);
       const float var = p.y_std * p.y_std * var_t;
-      const int64_t row = e_row0 + row_e;
+      const int64_t row = row0 + row_e;
       const bool in_range = row < p.N;
       if (sg == 0 && in_range) {
         if (p.mu) p.mu[row] = mu;
@@ -266,7 +579,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
         bool fast_ok = true;
         if (is_mc && fast_mc) {
           // every thread of the row evaluates the table; rows outside its envelope get the exact sum from one
-          // of the four warps that share the row group (they see the same ballot; rank % 4 picks the warp)
+          // of the two warps that share the row group (they see the same ballot; rank % 2 picks the warp)
           float c0, c1;
           mc_coef(p.acq, mu, var, c0, c1);
           fast_ok = mc_row_fast(s.mc_part, c0, c1, s0f, s1f);
@@ -274,7 +587,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
           for (int rank = 0; need != 0u; ++rank) {
             const int b = __ffs(need) - 1;
             need &= need - 1u;
-            if ((rank & 3) != sg) continue;
+            if ((rank & 1) != sg) continue;
             const float cb0 = __shfl_sync(0xffffffffu, c0, b), cb1 = __shfl_sync(0xffffffffu, c1, b);
             float a0, a1;
             mc_row_exact_warp(s.z_s, p.S, cb0, cb1, lane, a0, a1);
@@ -285,7 +598,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
           }
         } else if (is_mc) {
           float s0, s1;
-          mc_partial(p.acq, mu, var, s.z_s, p.S, sg, 4, s0, s1);
+          mc_partial(p.acq, mu, var, s.z_s, p.S, sg, 2, s0, s1);
           *reinterpret_cast<float2*>(s.mc_part + (sg * kTileM + row_e) * 2) = make_float2(s0, s1);
         }
         bar_compute();
@@ -298,7 +611,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
               s1 = fast_ok ? s1f : s.mc_part[kMcRows + kTileM + row_e];
             } else {
 #pragma unroll
-              for (int gg = 0; gg < 4; ++gg) {
+              for (int gg = 0; gg < 2; ++gg) {
                 const float2 pr = *reinterpret_cast<const float2*>(s.mc_part + (gg * kTileM + row_e) * 2);
                 s0 += pr.x;
                 s1 += pr.y;
@@ -317,119 +630,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
             }
           }
         }
-      } else {
-        bar_compute();  // partial buffers are rewritten by the next epilogue
       }
-    };
-
-    uint32_t slot = 0, ph = 0;  // A-ring position and phase
-    int it = 0;
-    int64_t prev_row0 = 0;
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int buf = LAG ? (it & 1) : 0;
-      const int64_t row0 = (int64_t)tile * kTileM;
-      sm.cand_task = s.cand_task + buf * kTileM;
-      float an0 = 0.f, an1 = 0.f;
-      const float* kr0 = nullptr;
-      const float* kr1 = nullptr;
-      float4 nx[4];
-      if constexpr (PRE) {
-        if (p.task_col >= 0 && tid < kTileM) {  // task id of each candidate row (mean constant, prior variance)
-          const int64_t row = row0 + tid;
-          float tv = 0.f;
-          if (row < p.N) {
-            switch (p.layout) {
-              case BB_ROW_MAJOR_F32: tv = load_x<BB_ROW_MAJOR_F32>(p.x, row, p.task_col, p.ldx); break;
-              case BB_COL_MAJOR_F32: tv = load_x<BB_COL_MAJOR_F32>(p.x, row, p.task_col, p.ldx); break;
-              case BB_ROW_MAJOR_F64: tv = load_x<BB_ROW_MAJOR_F64>(p.x, row, p.task_col, p.ldx); break;
-              default: tv = load_x<BB_COL_MAJOR_F64>(p.x, row, p.task_col, p.ldx); break;
-            }
-          }
-          sm.cand_task[tid] = min(max(__float2int_rn(tv), 0), p.n_tasks - 1);
-        }
-        kr0 = p.kpre + (row0 + mp) * p.ldk + g * 8;
-        kr1 = kr0 + 64 * p.ldk;
-        nx[0] = __ldg(reinterpret_cast<const float4*>(kr0));
-        nx[1] = __ldg(reinterpret_cast<const float4*>(kr0) + 1);
-        nx[2] = __ldg(reinterpret_cast<const float4*>(kr1));
-        nx[3] = __ldg(reinterpret_cast<const float4*>(kr1) + 1);
-        bar_compute();
-      } else {
-        stage_commit(sc, s.a_s, sm.cand_task, p.n_tasks, dq, row0, tid, regs);
-        bar_compute();
-        an0 = cand_sqnorm(sm, mp);
-        an1 = cand_sqnorm(sm, mp + 64);
-      }
-      float mean0 = 0.f, mean1 = 0.f;
-      for (int c = 0; c < C; ++c) {
-        float k0[8], k1[8];
-        const int i0 = c * kChunk + g * 8;
-        if constexpr (PRE) {
-          k0[0] = nx[0].x; k0[1] = nx[0].y; k0[2] = nx[0].z; k0[3] = nx[0].w;
-          k0[4] = nx[1].x; k0[5] = nx[1].y; k0[6] = nx[1].z; k0[7] = nx[1].w;
-          k1[0] = nx[2].x; k1[1] = nx[2].y; k1[2] = nx[2].z; k1[3] = nx[2].w;
-          k1[4] = nx[3].x; k1[5] = nx[3].y; k1[6] = nx[3].z; k1[7] = nx[3].w;
-          if (c + 1 < C) {  // next chunk's K* values fly under this chunk's split / ring wait
-            const float4* q0 = reinterpret_cast<const float4*>(kr0 + (c + 1) * kChunk);
-            const float4* q1 = reinterpret_cast<const float4*>(kr1 + (c + 1) * kChunk);
-            nx[0] = __ldg(q0);
-            nx[1] = __ldg(q0 + 1);
-            nx[2] = __ldg(q1);
-            nx[3] = __ldg(q1 + 1);
-          }
-        } else {
-          assemble_2x8<FAMILY>(sm, mp, mp + 64, an0, an1, i0, k0, k1);
-        }
-        {
-          const float4 al0 = *reinterpret_cast<const float4*>(s.alpha_s + i0);
-          const float4 al1 = *reinterpret_cast<const float4*>(s.alpha_s + i0 + 4);
-          const float al[8] = {al0.x, al0.y, al0.z, al0.w, al1.x, al1.y, al1.z, al1.w};
-#pragma unroll
-          for (int ii = 0; ii < 8; ++ii) {
-            mean0 = fmaf(k0[ii], al[ii], mean0);
-            mean1 = fmaf(k1[ii], al[ii], mean1);
-          }
-        }
-        uint4 h0, l0, h1, l1;
-        split_pair(k0[0], k0[1], h0.x, l0.x);
-        split_pair(k0[2], k0[3], h0.y, l0.y);
-        split_pair(k0[4], k0[5], h0.z, l0.z);
-        split_pair(k0[6], k0[7], h0.w, l0.w);
-        split_pair(k1[0], k1[1], h1.x, l1.x);
-        split_pair(k1[2], k1[3], h1.y, l1.y);
-        split_pair(k1[4], k1[5], h1.z, l1.z);
-        split_pair(k1[6], k1[7], h1.w, l1.w);
-        mbar_wait(&s.a_empty[slot], ph ^ 1u);  // MMAs that read this slot last time are done
-        uint8_t* sa = s.ring_a + (size_t)slot * kSlotABytes;
-        const uint32_t o0 = sw128_offset((uint32_t)mp, (uint32_t)g);
-        const uint32_t o1 = sw128_offset((uint32_t)(mp + 64), (uint32_t)g);
-        *reinterpret_cast<uint4*>(sa + o0) = h0;
-        *reinterpret_cast<uint4*>(sa + 16384 + o0) = l0;
-        *reinterpret_cast<uint4*>(sa + o1) = h1;
-        *reinterpret_cast<uint4*>(sa + 16384 + o1) = l1;
-        fence_proxy_async();  // generic-proxy writes -> visible to the tensor-core (async) proxy
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s.a_full[slot]);
-        if (++slot == (uint32_t)p.slots_a) {
-          slot = 0;
-          ph ^= 1u;
-        }
-      }
-      float* mpart = s.mean_part + buf * 8 * kTileM;
-      mpart[g * kTileM + mp] = mean0;
-      mpart[g * kTileM + mp + 64] = mean1;
-      // global loads of the next tile fly while an epilogue and its MC run
-      if constexpr (!PRE)
-        if (tile + (int)gridDim.x < p.num_tiles)
-          stage_prefetch(sc, dq, (int64_t)(tile + gridDim.x) * kTileM, tid, regs);
-      if (LAG) {
-        if (it > 0) epilogue(it - 1, prev_row0);
-      } else {
-        epilogue(it, row0);
-      }
-      prev_row0 = row0;
+      bar_compute();  // shared partials are rewritten by the next tile
+      if (tid == 0) trace_ev(p, it, 2);
     }
-    if (LAG && it > 0) epilogue(it - 1, prev_row0);
 
     // ---- CTA-level arg-max ----
     if (p.best_key != nullptr && p.has_acq) {
@@ -447,101 +651,245 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
         if (b != kEmptyKey) atomicMax(p.best_key, b);
       }
     }
-  } else if (warp == kWarpProducer) {
-    // =====================================================================================
-    // producer: stream the fp16 image of L^-1 (B operand) through the TMA engine
-    // =====================================================================================
-    if (elect_one()) {  // elect.sync: straight UBLKCP, no ELECT/BRA.U.ANY wrapper (see fused_common.cuh)
-      uint32_t st = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        size_t off = 0;
-        for (int c = 0; c < C; ++c) {
-          for (int sb = c > p.sb_lo ? c : p.sb_lo; sb < p.sb_hi;) {
-            const int gsz = (p.sb_hi - sb) < GMAX ? (p.sb_hi - sb) : GMAX;
-            const uint32_t bytes = (uint32_t)gsz * kStageBBytes;
-            mbar_wait_relaxed(&s.b_empty[st], ph ^ 1u);
-            mbar_expect_tx(&s.b_full[st], bytes);
-            bulk_g2s(s.ring_b + (size_t)st * p.stage_b_bytes, p.rimg + off, bytes, &s.b_full[st]);
-            off += bytes;
-            sb += gsz;
-            if (++st == (uint32_t)p.stages_b) {
-              st = 0;
-              ph ^= 1u;
-            }
-          }
-        }
-      }
-    }
   } else {
     // =====================================================================================
-    // MMA issuer: D[128 x n_pad] (TMEM, fp32) = K*[128 x n_pad] (smem, fp16 hi+lo) * Linv^T
-    // The whole warp runs the loop converged and one lane issues under elect.sync: issued under `if (lane == 0)`
-    // every tcgen05.mma costs ~106 cycles of ELECT/R2UR/BRA.U.ANY wrapper (scripts/ubench/mma_rate.cu).
+    // producer: stream the fp16 image of L^-1 (B operand) through the TMA engine, in the order the
+    // consumers read it: per tile, per column panel, per chunk c, sub-blocks sb >= c of the panel
     // =====================================================================================
-    {
-      uint32_t slot = 0, pha = 0, st = 0, phb = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const int buf = LAG ? (it & 1) : 0;
-        const int use = LAG ? (it >> 1) : it;
-        // the epilogue that last read this accumulator has drained it
-        mbar_wait_relaxed(&s.d_empty[buf], (uint32_t)((use & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t d_base = tmem_base + (uint32_t)(buf * ncol);
-        for (int c = 0; c < C; ++c) {
-          mbar_wait_relaxed(&s.a_full[slot], pha);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(s.ring_a + (size_t)slot * kSlotABytes);
-          const uint64_t a_hi = make_sw128_desc(a_addr);
-          const uint64_t a_lo = make_sw128_desc(a_addr + 16384);
-          for (int sb = c > p.sb_lo ? c : p.sb_lo; sb < p.sb_hi;) {
-            const int gsz = (p.sb_hi - sb) < GMAX ? (p.sb_hi - sb) : GMAX;
-            const uint32_t idesc = make_idesc_f16(kTileM, gsz * kChunk);
-            mbar_wait_relaxed(&s.b_full[st], phb);
-            tc_fence_after();
-            const uint32_t b_addr = smem_u32(s.ring_b + (size_t)st * p.stage_b_bytes);
-            const uint64_t b_hi = make_sw128_desc(b_addr);
-            const uint64_t b_lo = make_sw128_desc(b_addr + (uint32_t)gsz * 8192u);
-            const uint32_t d_addr = d_base + (uint32_t)((sb - p.sb_lo) * kChunk);
-            sb += gsz;
-            if (elect_one()) {
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) {
-                const uint64_t ko = (uint64_t)(kk * 2);  // 16 fp16 = 32 bytes = 2 x 16-byte units
-                umma_f16(d_addr, a_hi + ko, b_hi + ko, idesc, (c > 0 || kk > 0) ? 1u : 0u);
-                umma_f16(d_addr, a_hi + ko, b_lo + ko, idesc, 1u);
-                umma_f16(d_addr, a_lo + ko, b_hi + ko, idesc, 1u);
-              }
-              umma_commit(&s.b_empty[st]);
+    if (elect_one()) {
+      uint32_t idx = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x)
+        for (int lo = 0; lo < C; lo += kPanelSB) {
+          const int hi = min(C, lo + kPanelSB);
+          for (int c = 0; c < hi; ++c)
+            for (int sb = c > lo ? c : lo; sb < hi; ++sb, ++idx) {
+              const uint32_t st = idx % (uint32_t)p.stages_b, ph = (idx / (uint32_t)p.stages_b) & 1u;
+              mbar_wait_relaxed(&s.b_empty[st], ph ^ 1u);
+              mbar_expect_tx(&s.b_full[st], kStageBBytes);
+              bulk_g2s(s.ring_b + (size_t)st * kStageBBytes, p.rimg + rimg_tile(c, sb, C) * kStageBBytes, kStageBBytes,
+                       &s.b_full[st]);
             }
-            __syncwarp();
-            if (++st == (uint32_t)p.stages_b) {
-              st = 0;
-              phb ^= 1u;
-            }
-          }
-          if (elect_one()) umma_commit(&s.a_empty[slot]);
-          __syncwarp();
-          if (++slot == (uint32_t)p.slots_a) {
-            slot = 0;
-            pha ^= 1u;
-          }
         }
-        if (elect_one()) umma_commit(&s.d_full[buf]);
-        __syncwarp();
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// bb_kernel_matrix for models with the augmented training image: per 128-row tile and 64-column chunk, the distances
+// on the tensor cores (tc_distances), the kernel values in the accumulator registers, and the 64 x 64 fp32 tile
+// stored through the TMA engine (cp.async.bulk.tensor, 128B-swizzled boxes of 64 rows x 32 columns; the tensor map
+// clips rows >= N and columns >= n).  Two output buffers per warpgroup: a tile is written while the previous
+// store still reads the other.
+// ------------------------------------------------------------------------------------------
+struct KmatSmem {
+  uint8_t *bt, *a2, *out;
+  float *an_x, *cscale, *cshift, *tcov;
+  int32_t *cand_task, *ttask;
+};
+
+static __host__ __device__ size_t kmat_carve(uint8_t* base, const FusedParams& p, KmatSmem* s) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    const size_t o = off;
+    off += (bytes + 1023) / 1024 * 1024;  // swizzled tiles and TMA boxes: 1024-byte aligned
+    return base + o;
+  };
+  uint8_t* out = take((size_t)kConsumerWGs * 2 * 16384);
+  uint8_t* bt = take((size_t)3 * p.n_pad * p.tc * 2);
+  uint8_t* a2 = take((size_t)kConsumerWGs * 3 * 64 * p.tc * 2);
+  uint8_t* an_x = take(2 * kTileM * 4);
+  uint8_t* cs = take((size_t)p.d_pad * 4);
+  uint8_t* sh = take((size_t)p.d_pad * 4);
+  uint8_t* tc = take(kMaxTasks * kMaxTasks * 4);
+  uint8_t* ct = take(kTileM * 4);
+  uint8_t* tt = take((size_t)p.n_pad * 4);
+  if (s != nullptr) {
+    s->out = out;
+    s->bt = bt;
+    s->a2 = a2;
+    s->an_x = reinterpret_cast<float*>(an_x);
+    s->cscale = reinterpret_cast<float*>(cs);
+    s->cshift = reinterpret_cast<float*>(sh);
+    s->tcov = reinterpret_cast<float*>(tc);
+    s->cand_task = reinterpret_cast<int32_t*>(ct);
+    s->ttask = reinterpret_cast<int32_t*>(tt);
+  }
+  return off;
+}
+
+template <int FAMILY, int K2>
+__global__ void __launch_bounds__(kConsumerThreads, 1) k_kmat_tma(const FusedParams p,
+                                                                  const __grid_constant__ CUtensorMap tm) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  KmatSmem s;
+  kmat_carve(smem_raw, p, &s);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, t = tid & 127;
+  if (tid == 0 && (smem_u32(smem_raw) & 1023u) != 0u) __trap();
+  {
+    const uint4* src = reinterpret_cast<const uint4*>(p.timg_b);
+    uint4* dst = reinterpret_cast<uint4*>(s.bt);
+    for (int e = tid; e < 3 * p.n_pad * K2 * 2 / 16; e += kConsumerThreads) dst[e] = __ldg(src + e);
+  }
+  for (int e = tid; e < p.d_pad; e += kConsumerThreads) {
+    s.cscale[e] = __ldg(p.cand_scale + e);
+    s.cshift[e] = __ldg(p.cand_shift + e);
+  }
+  for (int e = tid; e < p.n_pad; e += kConsumerThreads) s.ttask[e] = __ldg(p.train_task + e);
+  for (int e = tid; e < p.n_tasks * p.n_tasks; e += kConsumerThreads) s.tcov[e] = __ldg(p.task_covar + e);
+  for (int e = tid; e < kTileM; e += kConsumerThreads) s.cand_task[e] = 0;
+  fence_proxy_async();  // the training image is read by the tensor cores
+  __syncthreads();
+
+  StageCtx sc;
+  sc.x = p.x;
+  sc.layout = p.layout;
+  sc.N = p.N;
+  sc.ldx = p.ldx;
+  sc.d = p.d;
+  sc.task_col = p.task_col;
+  sc.cscale = s.cscale;
+  sc.cshift = s.cshift;
+  sc.groups = kConsumerThreads / kTileM;
+  sc.gated = false;
+  sc.code_table = nullptr;
+  sc.code_table_ld = 0;
+  uint8_t* a2w = s.a2 + wg * 3 * tc_panel<K2>();
+  const uint32_t bsplit = (uint32_t)p.n_pad * K2 * 2u;
+  const int rq = 16 * (warp & 3) + (lane >> 2);  // accumulator rows rq, rq + 8 of the warpgroup's 64
+  uint32_t n_stores = 0;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    const int64_t row0 = (int64_t)tile * kTileM;
+    tc_stage_rows<K2>(p, sc, row0, wg, t, a2w, s.an_x, s.cand_task, s.cscale, s.cshift);
+    const float* tc0 = s.tcov + s.cand_task[64 * wg + rq] * p.n_tasks;
+    const float* tc1 = s.tcov + s.cand_task[64 * wg + rq + 8] * p.n_tasks;
+    for (int c = 0; c < p.n_chunks; ++c, ++n_stores) {
+      float dacc[32];
+      tc_distances<K2>(dacc, smem_u32(a2w), smem_u32(s.bt) + (uint32_t)c * tc_panel<K2>(), bsplit);
+      wg_wait<0>();
+      uint8_t* ob = s.out + (size_t)(wg * 2 + (n_stores & 1)) * 16384;
+      if (t == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");  // the store two back has read ob
+      bar_wg(wg);
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int r = rq + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (lane & 3);
+        const float* tcr = (i >> 1) & 1 ? tc1 : tc0;
+        float k0 = kernel_from_t<FAMILY>(dacc[i] * p.ts_g), k1 = kernel_from_t<FAMILY>(dacc[i + 1] * p.ts_g);
+        if (p.scaled) {
+          k0 *= tcr[s.ttask[c * kChunk + col]];
+          k1 *= tcr[s.ttask[c * kChunk + col + 1]];
+        }
+        // 128B-swizzled box layout: 16-byte chunk index XOR (row mod 8)
+        const uint32_t o = (uint32_t)(col >> 5) * 8192u + (uint32_t)r * 128u +
+                           ((((uint32_t)(col & 31) >> 2) ^ ((uint32_t)r & 7u)) << 4) + (uint32_t)(col & 3) * 4u;
+        *reinterpret_cast<float2*>(ob + o) = make_float2(k0, k1);
+      }
+      fence_proxy_async();  // generic-proxy writes -> visible to the TMA engine
+      bar_wg(wg);
+      if (t == 0) {
+        const uint64_t map = reinterpret_cast<uint64_t>(&tm);
+        const int y = (int)(row0 + 64 * wg);
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%1, %2}], [%3];"
+                       ::"l"(map), "r"(c * kChunk + 32 * b), "r"(y), "r"(smem_u32(ob + b * 8192))
+                       : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       }
     }
   }
+  if (t == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
 
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWarpProducer) tmem_dealloc(tmem_base, p.tmem_cols);
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+template <int FAMILY, int K2>
+static int launch_kmat_tma_one(const FusedParams& p, const CUtensorMap& tm, int grid, size_t smem, cudaStream_t stream) {
+  BB_SMEM_OPTIN_ONCE((k_kmat_tma<FAMILY, K2>));
+  k_kmat_tma<FAMILY, K2><<<grid, kConsumerThreads, smem, stream>>>(p, tm);
+  BB_LAUNCH_CHECK();
+  return BB_OK;
+}
+
+// bb_kernel_matrix front door of k_kmat_tma: *handled = false when the model or the output is outside its envelope
+// (no augmented training image, Matern-1/2, bit-packed rows, ldk not a multiple of 4 or d_k not 16-byte aligned).
+int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, float* d_k, int64_t ldk,
+                 cudaStream_t stream, bool* handled) {
+  *handled = false;
+  if (m->wide || m->d_timg_b == nullptr || (m->dist_k != 32 && m->dist_k != 64) || m->family == BB_KERNEL_MATERN12 ||
+      layout == BB_BITS_U8 || (ldk & 3) != 0 || (reinterpret_cast<uintptr_t>(d_k) & 15) != 0 || m->n_tasks > kMaxTasks)
+    return BB_OK;
+  FusedParams p;
+  memset(&p, 0, sizeof(p));
+  p.x = d_x;
+  p.layout = layout;
+  p.N = N;
+  p.ldx = ldx;
+  p.num_tiles = (int)((N + kTileM - 1) / kTileM);
+  p.cand_scale = m->d_cand_scale;
+  p.cand_shift = m->d_cand_shift;
+  p.task_covar = m->d_task_covar;
+  p.train_task = m->d_train_task;
+  p.n_pad = m->n_pad;
+  p.d = m->d;
+  p.d_pad = m->d_pad;
+  p.n_chunks = m->n_chunks;
+  p.task_col = m->task_col;
+  p.n_tasks = m->n_tasks;
+  p.scaled = (m->task_col >= 0 || m->prior_scale != 1.0f) ? 1 : 0;
+  p.tc = m->dist_k;
+  p.timg_b = reinterpret_cast<const uint8_t*>(m->d_timg_b);
+  p.ts_sa = m->ts_sa;
+  p.ts_aug_sq = m->ts_aug_sq;
+  p.ts_aug_one = m->ts_aug_one;
+  p.ts_g = m->ts_g;
+  int sms = 0, max_smem = 0;
+  int rc = device_limits(&sms, &max_smem);
+  if (rc != BB_OK) return rc;
+  const size_t smem = kmat_carve(nullptr, p, nullptr);
+  if (smem > (size_t)max_smem) return BB_OK;
+  static EncodeTiledFn encode = nullptr;
+  if (encode == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    BB_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
+    BB_CHECK_SUPPORTED(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled is not available");
+    encode = reinterpret_cast<EncodeTiledFn>(fn);
+  }
+  CUtensorMap tm;
+  const cuuint64_t gdim[2] = {(cuuint64_t)m->n, (cuuint64_t)N};
+  const cuuint64_t gstride[1] = {(cuuint64_t)ldk * 4};
+  const cuuint32_t box[2] = {32, 64};
+  const cuuint32_t estr[2] = {1, 1};
+  const CUresult r = encode(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, d_k, gdim, gstride, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+    return BB_ERR_CUDA;
+  }
+  const int grid = p.num_tiles < sms ? p.num_tiles : sms;
+  if (p.tc == 32) {
+    switch (m->family) {
+      case BB_KERNEL_MATERN32: rc = launch_kmat_tma_one<BB_KERNEL_MATERN32, 32>(p, tm, grid, smem, stream); break;
+      case BB_KERNEL_MATERN52: rc = launch_kmat_tma_one<BB_KERNEL_MATERN52, 32>(p, tm, grid, smem, stream); break;
+      default: rc = launch_kmat_tma_one<BB_KERNEL_RBF, 32>(p, tm, grid, smem, stream); break;
+    }
+  } else {
+    switch (m->family) {
+      case BB_KERNEL_MATERN32: rc = launch_kmat_tma_one<BB_KERNEL_MATERN32, 64>(p, tm, grid, smem, stream); break;
+      case BB_KERNEL_MATERN52: rc = launch_kmat_tma_one<BB_KERNEL_MATERN52, 64>(p, tm, grid, smem, stream); break;
+      default: rc = launch_kmat_tma_one<BB_KERNEL_RBF, 64>(p, tm, grid, smem, stream); break;
+    }
+  }
+  if (rc == BB_OK) *handled = true;
+  return rc;
 }
 
 // The qLogEI table of acq_math.cuh for one set of base samples, built once per call (one CTA) into the model blob.
-__global__ void __launch_bounds__(kFusedThreads) k_mc_table(const float* __restrict__ z, int S, float sgn,
-                                                            float* __restrict__ out) {
+__global__ void __launch_bounds__(512) k_mc_table(const float* __restrict__ z, int S, float sgn,
+                                                  float* __restrict__ out) {
   __shared__ float z_s[512];
   __shared__ float tab[kMcRows];
   for (int e = threadIdx.x; e < S; e += blockDim.x) z_s[e] = __ldg(z + e);
@@ -550,7 +898,7 @@ __global__ void __launch_bounds__(kFusedThreads) k_mc_table(const float* __restr
   for (int e = threadIdx.x; e < kMcRows; e += blockDim.x) out[e] = tab[e];
 }
 
-// Grid version for the headline kernel: 65 CTAs x 8 warps, one table entry per warp (acq_math.cuh).
+// Grid version: 65 CTAs x 8 warps, one table entry per warp (acq_math.cuh).
 __global__ void __launch_bounds__(256) k_mc_table_grid(const float* __restrict__ z, int S, float sgn,
                                                        float* __restrict__ out) {
   __shared__ float z_s[512];
@@ -560,23 +908,38 @@ __global__ void __launch_bounds__(256) k_mc_table_grid(const float* __restrict__
   mc_table_grid_part(tab, z_s, S, sgn, out);
 }
 
-template <int FAMILY, int LAG, bool PRE = false, int GMAX = 1>
-static int launch_one(FusedParams& p, int grid, size_t smem, cudaStream_t stream) {
-  BB_SMEM_OPTIN_ONCE((k_fused<FAMILY, LAG, PRE, GMAX>));
-  k_fused<FAMILY, LAG, PRE, GMAX><<<grid, kFusedThreads, smem, stream>>>(p);
-  BB_LAUNCH_CHECK();
+// Launch on `stream`.  after_table: k_mc_table_grid was launched just before, so this is a programmatic dependent
+// launch: the prologue overlaps the table kernel and waits for it (griddepcontrol.wait) only before it reads it.
+template <int FAMILY, bool PRE, int TC = 0>
+static int launch_one(const FusedParams& p, int grid, size_t smem, cudaStream_t stream, bool after_table) {
+  BB_SMEM_OPTIN_ONCE((k_fused<FAMILY, PRE, TC>));
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3((unsigned)kFusedThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = after_table ? 1 : 0;
+  BB_CUDA(cudaLaunchKernelEx(&cfg, k_fused<FAMILY, PRE, TC>, p));
   return BB_OK;
 }
 
-template <int FAMILY>
-static int launch_family(FusedParams& p, int lag, int grid, size_t smem, cudaStream_t stream) {
-  if (lag) return launch_one<FAMILY, 1>(p, grid, smem, stream);
-  return p.stage_b_bytes == 2 * kStageBBytes ? launch_one<FAMILY, 0, false, 2>(p, grid, smem, stream)
-                                             : launch_one<FAMILY, 0>(p, grid, smem, stream);
+// As many L^-1 stages as fit (at least one column panel's worth); 0 if even that does not fit.
+static int pick_stages(FusedParams& p, int max_smem) {
+  for (int st = kMaxStagesB; st >= kMinStagesB; --st) {
+    p.stages_b = st;
+    if (fused_smem_bytes(p) <= (size_t)max_smem) return st;
+  }
+  p.stages_b = kMinStagesB;
+  return 0;
 }
 
-// Wide-feature models: per block of <= wide_ws_rows candidates, k_kmat_tc writes the K* block into the
-// (L2-sized) workspace inside the model blob and k_fused<PRE> consumes it; both on the caller's stream.
+// Wide-feature models: per block of <= wide_ws_rows candidates, k_kmat_wg writes the K* block into the
+// workspace inside the model blob (whole waves of work items, within 40 MB of L2 while one wave fits: n_pad <= 576) and k_fused<PRE> consumes it; both on the caller's stream.
 static int launch_wide_blocks(const bb_model* m, const FusedParams& full, int sms, int max_smem,
                               const WideCross* wc, cudaStream_t stream) {
   BB_CHECK_SUPPORTED(m->d_wide_ws != nullptr && m->wide_ws_rows >= 256, "wide model without workspace");
@@ -586,7 +949,7 @@ static int launch_wide_blocks(const bb_model* m, const FusedParams& full, int sm
   }
   const float* mc_table = nullptr;
   if (m->d_mc_table != nullptr && mc_table_applicable(full.has_acq, full.acq, full.S)) {
-    k_mc_table<<<1, kFusedThreads, 0, stream>>>(full.z, full.S, full.acq.obj_scale < 0.f ? -1.f : 1.f, m->d_mc_table);
+    k_mc_table<<<1, 512, 0, stream>>>(full.z, full.S, full.acq.obj_scale < 0.f ? -1.f : 1.f, m->d_mc_table);
     BB_LAUNCH_CHECK();
     mc_table = m->d_mc_table;
   }
@@ -605,65 +968,25 @@ static int launch_wide_blocks(const bb_model* m, const FusedParams& full, int sm
       rc = launch_cross_wide(m, xb, full.layout, nb, full.ldx, wc->pend_beta, wc->P, wc->cross + b0 * wc->P, stream);
       if (rc != BB_OK) return rc;
     }
-    // V column panels: TMEM holds 512 columns, so a model with n_pad > 512 takes two passes over the K* block
-    // (the first only leaves its |V|^2 partial in the workspace)
-    const int C = m->n_chunks;
-    const int n_pass = C > 8 ? 2 : 1;
-    size_t rimg_off = 0;
-    for (int pass = 0; pass < n_pass; ++pass) {
-      FusedParams p = full;
-      p.x = xb;
-      p.N = nb;
-      p.num_tiles = (int)((nb + kTileM - 1) / kTileM);
-      p.kpre = m->d_wide_ws;
-      p.ldk = m->n_pad;
-      p.mc_table = mc_table;
-      p.d = 0;
-      p.d_pad = 0;  // nothing of the feature dimension is staged by the K*-reading kernel
-      p.sb_lo = pass == 0 ? 0 : 8;
-      p.sb_hi = (n_pass == 2 && pass == 0) ? 8 : C;
-      p.c_count = p.sb_hi;
-      const bool last = pass == n_pass - 1;
-      if (last) {
-        if (p.mu) p.mu += b0;
-        if (p.var) p.var += b0;
-        if (p.score) p.score += b0;
-        if (p.keep) p.keep += b0;
-        p.index_offset = full.index_offset + b0;
-        p.vacc_in = pass > 0 ? m->d_wide_vacc : nullptr;
-      } else {
-        p.mu = p.var = p.score = nullptr;
-        p.keep = nullptr;
-        p.best_key = nullptr;
-        p.has_acq = 0;
-        p.vacc_out = m->d_wide_vacc;
-      }
-      const int ncol = (p.sb_hi - p.sb_lo) * kChunk;
-      const int plag = (2 * ncol <= 512) ? 1 : 0;
-      uint32_t cols = 32;
-      while ((int)cols < (plag ? 2 : 1) * ncol) cols <<= 1;
-      p.tmem_cols = cols;
-      p.rimg = reinterpret_cast<const uint8_t*>(m->d_rimg4) + rimg_off;
-      for (int c = 0; c < p.c_count; ++c)  // bytes of this panel's image = its (chunk, sub-block) tile count
-        rimg_off += (size_t)(p.sb_hi - (c > p.sb_lo ? c : p.sb_lo)) * kStageBBytes;
-      p.stage_b_bytes = 4 * kStageBBytes;  // groups of up to four sub-blocks: N = 256 MMAs
-      p.slots_a = 2;
-      p.stages_b = 2;
-      while (true) {
-        FusedParams t = p;
-        if (t.slots_a < 3) t.slots_a++;
-        else if (t.stages_b < 3) t.stages_b++;
-        else break;
-        if (fused_smem_bytes(t) > (size_t)max_smem) break;
-        p = t;
-      }
-      const size_t smem = fused_smem_bytes(p);
-      BB_CHECK_SUPPORTED(smem <= (size_t)max_smem, "shared-memory budget exceeded: need %zu bytes", smem);
-      const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-      rc = plag ? launch_one<BB_KERNEL_RBF, 1, true, 4>(p, grid, smem, stream)
-                : launch_one<BB_KERNEL_RBF, 0, true, 4>(p, grid, smem, stream);
-      if (rc != BB_OK) return rc;
-    }
+    FusedParams p = full;
+    p.x = xb;
+    p.N = nb;
+    p.num_tiles = (int)((nb + kTileM - 1) / kTileM);
+    p.kpre = m->d_wide_ws;
+    p.ldk = m->n_pad;
+    p.d = 0;
+    p.d_pad = 0;  // nothing of the feature dimension is staged by the K*-reading kernel
+    if (p.mu) p.mu += b0;
+    if (p.var) p.var += b0;
+    if (p.score) p.score += b0;
+    if (p.keep) p.keep += b0;
+    p.index_offset = full.index_offset + b0;
+    BB_CHECK_SUPPORTED(pick_stages(p, max_smem) > 0, "shared-memory budget exceeded: need %zu bytes",
+                       fused_smem_bytes(p));
+    p.mc_table = mc_table;
+    const int grid = p.num_tiles < sms ? p.num_tiles : sms;
+    rc = launch_one<BB_KERNEL_RBF, true>(p, grid, fused_smem_bytes(p), stream, false);
+    if (rc != BB_OK) return rc;
   }
   return BB_OK;
 }
@@ -714,19 +1037,11 @@ int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
   p.mean_const = m->d_mean_const;
   p.train_task = m->d_train_task;
   p.rimg = reinterpret_cast<const uint8_t*>(m->d_rimg);
-  p.bimg = reinterpret_cast<const uint8_t*>(m->d_bimg);
-  p.dist_scale_a = m->dist_scale_a;
-  p.inv_dist_scale = 1.0f / (m->dist_scale_a * m->dist_scale_b);
   p.family = m->family;
-  p.dist_k = m->dist_k;
-  p.rimg2 = reinterpret_cast<const uint8_t*>(m->d_rimg2);
   p.n_pad = m->n_pad;
   p.d = m->d;
   p.d_pad = m->d_pad;
   p.n_chunks = m->n_chunks;
-  p.sb_lo = 0;
-  p.sb_hi = m->n_chunks;
-  p.c_count = m->n_chunks;
   p.task_col = m->task_col;
   p.n_tasks = m->n_tasks;
   p.y_mean = m->y_mean;
@@ -744,30 +1059,26 @@ int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
   p.keep = d_keep;
   p.best_key = reinterpret_cast<long long*>(d_best_key);
   p.index_offset = index_offset;
-  p.stage_b_bytes = kStageBBytes;
   p.trace = g_trace_buf;
   p.trace_cap = g_trace_cap;
-  p.timg_l = reinterpret_cast<const uint8_t*>(m->d_timg_l);
-  p.timg_b = reinterpret_cast<const uint8_t*>(m->d_timg_b);
-  p.ts_alpha = m->d_ts_alpha;
-  p.ts_sa = m->ts_sa;
-  p.ts_aug_sq = m->ts_aug_sq;
-  p.ts_aug_one = m->ts_aug_one;
-  p.ts_g = m->ts_g;
-  p.ts_kscale = m->ts_kscale;
-  if (gate != nullptr) {  // overlapped host pass: rows are published while the kernel runs (fused_ts.cu only)
+  if (gate != nullptr) {  // overlapped host pass: rows are published while the kernel runs
     p.ready_rows = gate->ready_rows;
     p.gate_status = gate->status;
     p.code_table = gate->code_table;
     p.code_table_ld = gate->code_table_ld;
     p.layout = gate->layout;
   }
-  BB_CHECK_SUPPORTED(p.n_pad <= 512 || m->wide, "n_pad=%d exceeds the 512 TMEM columns", p.n_pad);
-  const int lag = (2 * p.n_pad <= 512) ? 1 : 0;  // two accumulators fit: defer the epilogue
-  uint32_t cols = 32;
-  while ((int)cols < (lag ? 2 : 1) * p.n_pad) cols <<= 1;
-  p.tmem_cols = cols;
-
+  // tensor-core distances where the model carries the augmented training image
+  if (!m->wide && m->d_timg_b != nullptr && m->family != BB_KERNEL_MATERN12 && (m->dist_k == 32 || m->dist_k == 64)) {
+    p.tc = m->dist_k;
+    p.timg_b = reinterpret_cast<const uint8_t*>(m->d_timg_b);
+    p.ts_sa = m->ts_sa;
+    p.ts_aug_sq = m->ts_aug_sq;
+    p.ts_aug_one = m->ts_aug_one;
+    p.ts_g = m->ts_g;
+    p.ts_kscale = m->ts_kscale;
+    p.inv_r_scale2 /= m->ts_kscale * m->ts_kscale;  // |V|^2 of ts_kscale K*
+  }
   int max_smem = 0, sms = 0;
   {
     const int rc_lim = device_limits(&sms, &max_smem);
@@ -775,86 +1086,55 @@ int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
   }
   BB_CHECK_SUPPORTED(gate == nullptr || !m->wide, "the overlapped host pass does not cover wide-feature models");
   if (m->wide) return launch_wide_blocks(m, p, sms, max_smem, wc, stream);
-  // diagnostic knob (tests / profiling only): BB_FORCE_KERNEL=tc keeps shapes the TS kernel covers on fused_tc.cu
-  static const bool ts_off = [] {
-    const char* e = getenv("BB_FORCE_KERNEL");
-    return e != nullptr && e[0] == 't' && e[1] == 'c';
-  }();
-  if (!ts_off && !m->wide && fused_ts_supported(p, max_smem)) {  // headline kernel (fused_ts.cu)
-    const int grid_ts = p.num_tiles < sms ? p.num_tiles : sms;
-    if (m->d_mc_table != nullptr && mc_table_applicable(p.has_acq, p.acq, p.S) && grid_ts > 8) {
-      // qLogEI table once per call instead of once per persistent CTA (short launches keep the in-kernel build)
-      k_mc_table_grid<<<(kMcNT + 8) / 8, 256, 0, stream>>>(p.z, p.S, p.acq.obj_scale < 0.f ? -1.f : 1.f, m->d_mc_table);
-      BB_LAUNCH_CHECK();
-      p.mc_table = m->d_mc_table;
-    }
-    return launch_fused_ts(p, grid_ts, stream);
+  if (p.tc && pick_stages(p, max_smem) == 0) {  // the resident training image does not fit: CUDA-core distances
+    p.tc = 0;
+    p.inv_r_scale2 *= p.ts_kscale * p.ts_kscale;
   }
-  BB_CHECK_SUPPORTED(gate == nullptr, "the overlapped host pass needs the headline kernel's shape envelope");
-  if (fused_tc_supported(p, max_smem)) {
-    const int grid_tc = p.num_tiles < sms ? p.num_tiles : sms;
-    return launch_fused_tc(p, grid_tc, stream);
-  }
-  // n_pad > 256 (single accumulator): pair the L^-1 sub-blocks (N = 128 MMAs) when two 32 KB stages fit
-  if (!lag && m->d_rimg2g != nullptr) {
-    FusedParams t = p;
-    t.slots_a = 2;
-    t.stages_b = 2;
-    t.stage_b_bytes = 2 * kStageBBytes;
-    if (fused_smem_bytes(t) <= (size_t)max_smem) {
-      p.stage_b_bytes = 2 * kStageBBytes;
-      p.rimg = reinterpret_cast<const uint8_t*>(m->d_rimg2g);
-    }
-  }
-  // ring sizes: as many as fit, B stages first (they hide L2 latency), then A slots
-  p.slots_a = 2;
-  p.stages_b = 2;
-  while (true) {
-    FusedParams t = p;
-    if (t.stages_b < 4) t.stages_b++;
-    else if (t.slots_a < 3) t.slots_a++;
-    else if (t.stages_b < kMaxStagesB) t.stages_b++;
-    else break;
-    if (fused_smem_bytes(t) > (size_t)max_smem) break;
-    p = t;
+  BB_CHECK_SUPPORTED(pick_stages(p, max_smem) > 0, "shared-memory budget exceeded: need %zu bytes, device allows %d",
+                     fused_smem_bytes(p), max_smem);
+  const int grid = p.num_tiles < sms ? p.num_tiles : sms;
+  if (m->d_mc_table != nullptr && mc_table_applicable(p.has_acq, p.acq, p.S) && grid > 8) {
+    // qLogEI table once per call instead of once per persistent CTA (short launches keep the in-kernel build)
+    k_mc_table_grid<<<(kMcNT + 8) / 8, 256, 0, stream>>>(p.z, p.S, p.acq.obj_scale < 0.f ? -1.f : 1.f, m->d_mc_table);
+    BB_LAUNCH_CHECK();
+    p.mc_table = m->d_mc_table;
   }
   const size_t smem = fused_smem_bytes(p);
-  BB_CHECK_SUPPORTED(smem <= (size_t)max_smem,
-                     "shared-memory budget exceeded: need %zu bytes, device allows %d", smem,
-                     max_smem);
-  const int grid = p.num_tiles < sms ? p.num_tiles : sms;
+  const bool dep = p.mc_table != nullptr;
+  if (p.tc == 32) {
+    switch (m->family) {
+      case BB_KERNEL_MATERN32: return launch_one<BB_KERNEL_MATERN32, false, 32>(p, grid, smem, stream, dep);
+      case BB_KERNEL_MATERN52: return launch_one<BB_KERNEL_MATERN52, false, 32>(p, grid, smem, stream, dep);
+      default: return launch_one<BB_KERNEL_RBF, false, 32>(p, grid, smem, stream, dep);
+    }
+  }
+  if (p.tc == 64) {
+    switch (m->family) {
+      case BB_KERNEL_MATERN32: return launch_one<BB_KERNEL_MATERN32, false, 64>(p, grid, smem, stream, dep);
+      case BB_KERNEL_MATERN52: return launch_one<BB_KERNEL_MATERN52, false, 64>(p, grid, smem, stream, dep);
+      default: return launch_one<BB_KERNEL_RBF, false, 64>(p, grid, smem, stream, dep);
+    }
+  }
   switch (m->family) {
-    case BB_KERNEL_MATERN12: return launch_family<BB_KERNEL_MATERN12>(p, lag, grid, smem, stream);
-    case BB_KERNEL_MATERN32: return launch_family<BB_KERNEL_MATERN32>(p, lag, grid, smem, stream);
-    case BB_KERNEL_MATERN52: return launch_family<BB_KERNEL_MATERN52>(p, lag, grid, smem, stream);
-    default: return launch_family<BB_KERNEL_RBF>(p, lag, grid, smem, stream);
+    case BB_KERNEL_MATERN12: return launch_one<BB_KERNEL_MATERN12, false>(p, grid, smem, stream, dep);
+    case BB_KERNEL_MATERN32: return launch_one<BB_KERNEL_MATERN32, false>(p, grid, smem, stream, dep);
+    case BB_KERNEL_MATERN52: return launch_one<BB_KERNEL_MATERN52, false>(p, grid, smem, stream, dep);
+    default: return launch_one<BB_KERNEL_RBF, false>(p, grid, smem, stream, dep);
   }
 }
 
-// Shape test of the single-launch gated pass: the same envelope as the headline kernel.
+// Shape test of the single-launch gated pass: k_fused over non-wide models.
 bool fused_gate_supported(const bb_model* m, const bb_acq_spec* acq, int32_t S) {
-  if (m == nullptr || m->wide) return false;
-  static const bool ts_off = [] {
-    const char* e = getenv("BB_FORCE_KERNEL");
-    return e != nullptr && e[0] == 't' && e[1] == 'c';
-  }();
-  if (ts_off) return false;
+  (void)acq;
+  (void)S;
+  if (m == nullptr || m->wide || m->n_tasks > kMaxTasks) return false;
   FusedParams p;
   memset(&p, 0, sizeof(p));
-  p.layout = BB_ROW_MAJOR_F32;
-  p.timg_l = reinterpret_cast<const uint8_t*>(m->d_timg_l);
-  p.timg_b = reinterpret_cast<const uint8_t*>(m->d_timg_b);
-  p.ts_alpha = m->d_ts_alpha;
   p.n_pad = m->n_pad;
-  p.d = m->d;
-  p.family = m->family;
-  p.n_tasks = m->n_tasks;
-  p.has_acq = acq ? 1 : 0;
-  if (acq) p.acq = *acq;
-  p.S = S;
+  p.d_pad = m->d_pad;
   int sms = 0, max_smem = 0;
   if (device_limits(&sms, &max_smem) != BB_OK) return false;
-  return fused_ts_supported(p, max_smem);
+  return pick_stages(p, max_smem) > 0;
 }
 
 }  // namespace bb

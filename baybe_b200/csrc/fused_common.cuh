@@ -1,8 +1,7 @@
 // fused_common.cuh -- parameters and helpers shared by the scoring kernels
-//   fused_tc.cu  k_fused_tc  distances AND posterior contraction on tcgen05 (n_pad <= 256, d_pad <= 64): headline
-//   fused.cu     k_fused     distances on CUDA cores (FFMA2), n_pad <= 512, training rows resident in shared
-//                            memory; its PRE variant reads a K* block instead (wide-feature path)
-//   wide.cu      k_kmat_tc   K-looped tcgen05 distance GEMM for wide / bit-packed feature spaces and n_pad > 512
+//   fused.cu  k_fused    distances on CUDA cores, V = K* L^-T on warpgroup MMAs (wgmma), q = 1 acquisition and
+//                        arg-max; its PRE variant reads a K* block instead (wide-feature path)
+//   wide.cu   k_kmat_wg  K-looped wgmma distance GEMM for wide / bit-packed feature spaces and n_pad > 512
 #pragma once
 
 #include "acq_math.cuh"
@@ -10,15 +9,17 @@
 
 namespace bb {
 
-constexpr int kComputeWarps = 16;
-constexpr int kComputeThreads = kComputeWarps * 32;  // 512
-constexpr int kFusedThreads = kComputeThreads + 64;  // + producer warp + MMA warp
-constexpr int kWarpProducer = 16;
-constexpr int kWarpMma = 17;
-constexpr int kMaxSlotsA = 4;
-constexpr int kMaxStagesB = 8;
-constexpr uint32_t kSlotABytes = 32768;  // [hi 16 KB | lo 16 KB], each 128 rows x 64 fp16, SW128
-constexpr uint32_t kStageBBytes = 16384; // [hi 8 KB | lo 8 KB],  each  64 rows x 64 fp16, SW128
+// Two consumer warpgroups (rows 0-63 and 64-127 of a 128-candidate tile) and one bulk-copy producer warp.
+constexpr int kConsumerWGs = 2;
+constexpr int kConsumerThreads = kConsumerWGs * 128;  // 256
+constexpr int kFusedThreads = kConsumerThreads + 32;  // + producer warp
+constexpr int kWarpProducer = kConsumerThreads / 32;  // 8
+// 64-column sub-blocks of V held in registers at once (a 64 x 128 fp32 panel, 64 registers per thread): nine warps
+// spread over the four SM sub-partitions put three warps on one of them, which caps a thread at 168 registers
+constexpr int kPanelSB = 2;
+constexpr int kMinStagesB = kPanelSB, kMaxStagesB = 8;
+constexpr uint32_t kABytes = 16384;      // one warpgroup's K* chunk: [hi 8 KB | lo 8 KB], 64 rows x 64 fp16, SW128
+constexpr uint32_t kStageBBytes = 16384; // one L^-1 tile: [hi 8 KB | lo 8 KB], 64 rows x 64 fp16, SW128
 constexpr int kMaxTasks = 16;
 constexpr int kMaxSamples = 1024;
 
@@ -31,19 +32,18 @@ struct FusedParams {
   // model
   const float *cand_scale, *cand_shift, *train_m2, *train_sq, *alpha, *task_covar, *mean_const;
   const int32_t* train_task;
-  const uint8_t* rimg;
-  const uint8_t* bimg;           // distance-GEMM B operand (fused_tc only)
-  const uint8_t* rimg2;          // pair-grouped L^-1 image (fused_tc only)
-  float dist_scale_a, inv_dist_scale;  // a is scaled by dist_scale_a; D2 * inv_dist_scale = -2 a.b
+  const uint8_t* rimg;  // fp16 hi/lo image of L^-1: tiles (chunk c, sub-block s >= c), c-major
   int family;
-  int dist_k;                    // 32 or 64: K extent of the distance-GEMM tiles (0: none)
   int n_pad, d, d_pad, n_chunks, task_col, n_tasks;
   float y_mean, y_std, prior_scale, inv_r_scale2;
   int scaled;  // task kernel or output scale present
-  // ring sizes
-  int slots_a, stages_b;
-  uint32_t stage_b_bytes;  // bytes of one L^-1 ring stage: GMAX * 16 KB
-  uint32_t tmem_cols;
+  int stages_b;  // L^-1 tiles in flight
+  // tensor-core distances (tc = 1): augmented training image [sb (-2b) | Q1 | |b|^2 Q] as fp16 hi/mid/lo panels of
+  // n_pad rows x 32 k (SW64); candidate rows become [sa a | |a|^2 P | P1], so the GEMM yields t / ts_g directly
+  int tc;
+  const uint8_t* timg_b;
+  float ts_sa, ts_aug_sq, ts_aug_one, ts_g;
+  float ts_kscale;  // power of two applied to K* before the fp16 hi/lo split (fp16 range and resolution)
   // acquisition (has_acq == 0: posterior only)
   int has_acq;
   bb_acq_spec acq;
@@ -54,34 +54,17 @@ struct FusedParams {
   const uint8_t* keep;
   long long* best_key;
   int64_t index_offset;
-  // column panel of V handled by this launch (TMEM holds 512 columns): sub-blocks [sb_lo, sb_hi) of 64 columns,
-  // fed by the first c_count K* chunks; a model with n_pad <= 512 is one panel (0, n_chunks, n_chunks)
-  int sb_lo, sb_hi, c_count;
-  const float* vacc_in;   // |V|^2 partial of the earlier panels (null: none)
-  float* vacc_out;        // non-null: this is not the last panel -- store the partial and stop
-  const float* mc_table;  // K*-reading variant: qLogEI table built once per call by k_mc_table (null: per-sample loop)
-  const float* kpre;  // wide-feature path: K* block already materialised by k_kmat_tc (else null)
+  const float* mc_table;  // qLogEI table built once per call by k_mc_table(_grid) (null: built in the kernel or unused)
+  const float* kpre;  // wide-feature path: K* block already materialised by k_kmat_wg (else null)
   int64_t ldk;
   long long* trace;  // test-only event trace (bb_debug_set_trace); null in normal operation
   int trace_cap;
-  // fused_ts.cu (A operand of the V contraction in tensor memory): operand images and folded constants
-  const uint8_t* timg_l;   // L^-1 image: [hi tiles, chunk c = 0..C-1][lo tiles], tile c = (n_pad - 64c) rows x 64 k, SW128
-  const uint8_t* timg_b;   // augmented training-row image: 3 splits x n_pad rows x 32 k (|b|^2 and 1 in k = 31, 30), SW64
-  const float* ts_alpha;   // alpha / ts_kscale
-  float ts_sa;             // power of two folded into the candidate rows of the A2 image
-  float ts_aug_sq;         // A2 column 30 = |a|^2 * ts_aug_sq
-  float ts_aug_one;        // A2 column 31 = ts_aug_one
-  float ts_g;              // D2 * ts_g = scaled squared distance t (family constant folded in)
-  float ts_kscale;         // power of two folded into K* before the fp16 hi/lo split
   // single-launch end-to-end pass (bb_score_fused_overlapped): rows arrive from the host WHILE the kernel runs
   const unsigned* ready_rows;  // rows [0, *ready_rows) of x have landed (published by the copy stream); null: all
   int32_t* gate_status;        // set to 1 if a tile's rows were not published within the time-out
   const float* code_table;     // level-coded layouts: value table [d][code_table_ld]
   int code_table_ld;
 };
-
-// candidate layouts beyond bb_layout, internal to the overlapped host pass: level codes expanded in the staging step
-constexpr int kLayoutCodes4 = 16, kLayoutCodes8 = 17;
 
 // optional request threaded through launch_fused by the overlapped host pass (null: none)
 struct StreamGate {
@@ -104,7 +87,8 @@ __device__ __forceinline__ void trace_ev(const FusedParams& p, int it, int ev) {
   }
 }
 
-__device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, 512;" ::: "memory"); }
+// the 256 consumer threads
+__device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 
 // Wait used by the single-lane helper warps: mbarrier.try_wait with a suspend-time hint parks the
@@ -124,19 +108,6 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity
   }
 }
 
-// 16 consecutive fp32 columns of this thread's TMEM lane.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-
 // fp16 hi/mid/lo split of four fp32 values -> three 8-byte packets.
 __device__ __forceinline__ void split3_quad(const float (&x)[4], uint2& hi, uint2& mid, uint2& lo) {
   __half2 h01 = __floats2half2_rn(x[0], x[1]), h23 = __floats2half2_rn(x[2], x[3]);
@@ -150,16 +121,7 @@ __device__ __forceinline__ void split3_quad(const float (&x)[4], uint2& hi, uint
   lo = make_uint2(*reinterpret_cast<uint32_t*>(&l01), *reinterpret_cast<uint32_t*>(&l23));
 }
 
-int launch_fused_tc(FusedParams& p, int grid, cudaStream_t stream);
-int launch_fused_ts(FusedParams& p, int grid, cudaStream_t stream);
-bool fused_ts_supported(const FusedParams& p, int max_smem);
-bool kmat_ts_supported(const FusedParams& p, const float* d_k, int64_t ldk, int max_smem);
-int launch_kmat_ts(FusedParams& p, float* d_k, int64_t ldk, int n_cols, int grid, cudaStream_t stream);
-int try_kmat_ts(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, float* d_k, int64_t ldk,
-                cudaStream_t stream, bool* handled);
-// elect.sync: true in exactly one lane of a converged warp.  tcgen05.mma / cp.async.bulk / tcgen05.commit issued
-// under this predicate compile to straight uniform-datapath code; the same instructions under `if (lane == 0)` are
-// wrapped by ptxas in an ELECT / R2UR / BRA.U.ANY loop that costs ~106 cycles per MMA (scripts/ubench/mma_rate.cu).
+// elect.sync: true in exactly one lane of a converged warp (the bulk-copy producers issue under it).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred = 0;
   asm volatile(
@@ -169,7 +131,8 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-bool fused_tc_supported(FusedParams& p, int max_smem);
+int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, float* d_k, int64_t ldk,
+                 cudaStream_t stream, bool* handled);
 int launch_pend_images(const bb_model* m, int32_t layout, const float* d_pend_x, int32_t P, cudaStream_t stream);
 int launch_cross_wide(const bb_model* m, const void* d_x, int32_t layout, int64_t nb, int64_t ldx,
                       const float* d_pend_beta, int32_t P, float* d_cross_blk, cudaStream_t stream);
@@ -180,7 +143,7 @@ struct WideCross {
   int32_t P;
   float* cross;
 };
-// true when the single-launch gated pass can run this model (headline kernel envelope)
+// true when the single-launch gated pass can run this model
 bool fused_gate_supported(const bb_model* m, const bb_acq_spec* acq, int32_t S);
 int launch_kmat_wide(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx,
                      float* d_out, int64_t ldk, int64_t out_rows, int out_cols, cudaStream_t stream);

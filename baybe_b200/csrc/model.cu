@@ -30,9 +30,9 @@ const char* last_error() { return g_err; }
 // ------------------------------------------------------------------------------------------
 struct BlobLayout {
   size_t cand_scale, cand_shift, train_m2, train_sq, alpha, train_task, task_covar, mean_const,
-      rimg, linv, alpha64, xn64, linv32, kmat, resid, noise_row, tcov64, cnorm, pend_norm, pend_w64, bimg, rimg2, flags,
-      wimg, wimg_bits, wnorm_bits, wsrc, wide_ws, rimg4, rimg2g, pend_img, pend_norm2, pend_task, kpend_ws, vacc, mc_table, timg_l, timg_b, ts_alpha, total;
-  int ts;  // operand images of fused_ts.cu present (n_pad <= 256, d <= 30)
+      rimg, linv, alpha64, xn64, linv32, kmat, resid, noise_row, tcov64, cnorm, pend_norm, pend_w64, flags,
+      wimg, wimg_bits, wnorm_bits, wsrc, wide_ws, pend_img, pend_norm2, pend_task, kpend_ws, mc_table, timg_b, total;
+  int ts;  // K extent (32 or 64) of the augmented training image of the tensor-core distances, 0: none
   int n_pad, d_pad, n_chunks, n_tiles;
   int wide, d_wide;
   int64_t wide_ws_rows;
@@ -41,7 +41,14 @@ struct BlobLayout {
 // The CUDA-core assembly keeps the scaled training rows in shared memory (n_pad*d_pad*4 <= 56 KB);
 // anything larger takes the K-chunked tensor-core path of wide.cu.
 constexpr size_t kResidentTrainBytes = 56 * 1024;
-constexpr int64_t kWideWsRows = 148 * 256;  // one wave of 256-row work items per SM
+// K* workspace of the wide path: whole waves of 128-row work items over the 132 SMs of an H100, as many as keep the
+// block within 40 MB of the 50 MB L2 (at least one wave: from n_pad = 640 on, one wave alone is larger than that)
+constexpr int64_t kWideWave = 132 * 128;
+constexpr size_t kWideWsBytes = (size_t)40 << 20;
+static int64_t wide_ws_rows(int n_pad) {
+  const int64_t waves = (int64_t)(kWideWsBytes / ((size_t)n_pad * 4)) / kWideWave;
+  return (waves < 1 ? 1 : waves) * kWideWave;
+}
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
@@ -77,14 +84,11 @@ static BlobLayout make_layout(int n, int d, int T) {
   L.cnorm = take(sizeof(float) * 2 * d);
   L.pend_norm = take(sizeof(double) * BB_MAX_PENDING * d);
   L.pend_w64 = take(sizeof(double) * BB_MAX_PENDING * n);
-  L.bimg = take((size_t)L.n_chunks * 24576);
-  L.rimg2 = take((size_t)L.n_tiles * 16384);
   L.flags = take(64);
-  L.rimg2g = L.n_chunks > 4 ? take((size_t)L.n_tiles * 16384) : 0;
   L.wide = ((size_t)L.n_pad * L.d_pad * 4 > kResidentTrainBytes || L.n_pad > 512) ? 1 : 0;
   L.d_wide = round_up(d, 32);
-  L.wimg = L.wimg_bits = L.wnorm_bits = L.wsrc = L.wide_ws = L.rimg4 = 0;
-  L.pend_img = L.pend_norm2 = L.pend_task = L.kpend_ws = L.vacc = L.mc_table = 0;
+  L.wimg = L.wimg_bits = L.wnorm_bits = L.wsrc = L.wide_ws = 0;
+  L.pend_img = L.pend_norm2 = L.pend_task = L.kpend_ws = L.mc_table = 0;
   L.wide_ws_rows = 0;
   if (L.wide) {
     const size_t img = (size_t)L.n_pad * L.d_wide * 2 * 3;
@@ -92,25 +96,20 @@ static BlobLayout make_layout(int n, int d, int T) {
     L.wimg_bits = take(img);
     L.wnorm_bits = take(sizeof(float) * L.n_pad);
     L.wsrc = take(sizeof(float) * (size_t)L.n_pad * L.d_wide);
-    L.rimg4 = take((size_t)L.n_tiles * 16384);
-    L.wide_ws_rows = kWideWsRows;
+    L.wide_ws_rows = wide_ws_rows(L.n_pad);
     L.wide_ws = take(sizeof(float) * (size_t)L.wide_ws_rows * L.n_pad);
     L.pend_img = take((size_t)64 * L.d_wide * 2 * 3);
     L.pend_norm2 = take(sizeof(float) * 64);
     L.pend_task = take(sizeof(int32_t) * 64);
     L.kpend_ws = take(sizeof(float) * (size_t)L.wide_ws_rows * 64);
-    L.vacc = take(sizeof(float) * (size_t)L.wide_ws_rows);
     L.mc_table = take(sizeof(float) * 1024);
   }
-  // fused_ts.cu: hi/lo images of L^-1 in per-chunk tiles of (n_pad - 64c) rows, augmented training-row image
-  L.ts = (L.n_pad <= 256 && d <= 30) ? 1 : 0;
-  L.timg_l = L.timg_b = L.ts_alpha = 0;
+  // k_fused with tensor-core distances: augmented training-row image
+  // (n_pad <= 256; K = 32 for d <= 30, K = 64 for d <= 62: the last two K columns carry |a|^2 + |b|^2)
+  L.ts = L.n_pad > 256 ? 0 : d <= 30 ? 32 : d <= 62 ? 64 : 0;
+  L.timg_b = 0;
   if (L.ts) {
-    size_t tile_bytes = 0;
-    for (int r = L.n_pad; r > 0; r -= kChunk) tile_bytes += (size_t)r * 128;
-    L.timg_l = take(2 * tile_bytes);
-    L.timg_b = take((size_t)3 * L.n_pad * 64);
-    L.ts_alpha = take(sizeof(float) * L.n_pad);
+    L.timg_b = take((size_t)3 * L.n_pad * L.ts * 2);
     if (!L.wide) L.mc_table = take(sizeof(float) * 1024);  // per-call qLogEI table (k_mc_table_grid)
   }
   L.total = off;
@@ -393,135 +392,32 @@ __global__ void k_build_rimg(const double* __restrict__ Linv, int n, int n_chunk
   }
 }
 
-// Second layout of the (scale * L^-1) image for the fused_tc kernel: per K chunk c the column
-// sub-blocks s >= c are grouped so that one tcgen05.mma covers up to 128 output columns -- a
-// leading single tile if c is odd, then pairs (s, s+1) with s even, then a trailing single.
-// A pair block is [hi: 128 rows x 64 k | lo: same] = 32 KB, a single block [hi 8 KB | lo 8 KB];
-// blocks follow each other in consumption order.  One CTA per block (blockIdx.x = group index).
-// gmax = 2: aligned pairs as described above (fused_tc); gmax = 4: greedy groups of up to four
-// sub-blocks starting at s = c (N = 256 MMAs; the K*-reading kernel of the wide path).
-// gmax = -2: greedy groups of two (k_fused with N = 128 MMAs when n_pad > 256).
-__host__ __device__ inline int rimg_group(int gmax, int s, int n_chunks) {
-  if (gmax == 2) return ((s & 1) == 0 && s + 1 < n_chunks) ? 2 : 1;  // n_chunks: end of the panel
-  const int g = gmax < 0 ? -gmax : gmax;
-  return (n_chunks - s) < g ? (n_chunks - s) : g;
-}
-
-// [sb_lo, sb_hi): the column panel the image serves (fed by chunks c < c_count); whole matrix = (0, C, C).
-__global__ void k_build_rimg2(const double* __restrict__ Linv, int n, int n_chunks, double scale,
-                              int gmax, int sb_lo, int sb_hi, int c_count, uint8_t* __restrict__ rimg2) {
-  // decode group -> (c, first sub-block s, size g) and byte offset
-  int grp = blockIdx.x, c = 0, s0 = 0, g = 1;
-  size_t off = 0;
-  bool found = false;
-  int idx = 0;
-  for (c = 0; c < c_count && !found; ++c) {
-    int s = c > sb_lo ? c : sb_lo;
-    while (s < sb_hi) {
-      const int gg = rimg_group(gmax, s, sb_hi);
-      if (idx == grp) {
-        s0 = s;
-        g = gg;
-        found = true;
-        break;
-      }
-      off += (size_t)gg * 16384;
-      s += gg;
-      ++idx;
-    }
-    if (found) break;
-  }
-  if (!found) return;
-  uint8_t* base = rimg2 + off;
-  const uint32_t lo_off = (uint32_t)g * 8192u;
-  const int rows = 64 * g;
-  for (int e = threadIdx.x; e < rows * 64; e += blockDim.x) {
-    const int r = e >> 6, kk = e & 63;
-    const int j = s0 * 64 + r, i = c * 64 + kk;
-    const double v = (j < n && i < n && i <= j) ? Linv[(size_t)j * n + i] * scale : 0.0;
-    const float vf = (float)v;
-    const __half hi = __float2half_rn(vf);
-    const __half lo = __float2half_rn((float)(v - (double)__half2float(hi)));
-    const uint32_t o = sw128_offset((uint32_t)r, (uint32_t)(kk >> 3)) + (uint32_t)(kk & 7) * 2u;
-    *reinterpret_cast<__half*>(base + o) = hi;
-    *reinterpret_cast<__half*>(base + lo_off + o) = lo;
-  }
-}
-
-// fp16 hi/mid/lo image of (scale * -2b) for the tensor-core distance GEMM: three panels
-// [hi | mid | lo], each [n_pad training rows][K2 dims] fp16, K-major, swizzled (K2 = 32: 64-byte
-// rows / SWIZZLE_64B; K2 = 64: 128-byte rows / SWIZZLE_128B); 8-row groups contiguous; dims >= d
-// are zero.  D2[m][i] = sum_j a[m][j] * (-2 b[i][j]).
+// Augmented training-row image of the tensor-core distances (k_fused, k_kmat_tma): three panels [hi | mid | lo] of
+// [n_pad rows][K2 k] fp16 (K2 = 32: 64-byte rows, SWIZZLE_64B; K2 = 64: 128-byte rows, SWIZZLE_128B):
+//     k < d: scale_b * (-2 b_ij); k = K2 - 2: q_one (pairs with |a|^2 * P in the candidate tile);
+//     k = K2 - 1: |b_i|^2 * q_sq (pairs with P1).  Rows i >= n are zero.
 template <int K2>
-__global__ void k_build_bimg(const float* __restrict__ train_m2, int n_pad, int d_pad, float scale,
-                             uint8_t* __restrict__ bimg) {
-  const uint32_t split = (uint32_t)n_pad * K2 * 2u;
-  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n_pad * K2; e += gridDim.x * blockDim.x) {
-    const int i = e / K2, j = e - i * K2;
-    const float v = (j < d_pad) ? train_m2[(size_t)i * d_pad + j] * scale : 0.f;
-    const __half h = __float2half_rn(v);
-    const float r1 = v - __half2float(h);
-    const __half m = __float2half_rn(r1);
-    const __half l = __float2half_rn(r1 - __half2float(m));
-    const uint32_t off = swk_offset<K2>((uint32_t)i, (uint32_t)(j >> 3)) + (uint32_t)(j & 7) * 2u;
-    *reinterpret_cast<__half*>(bimg + off) = h;
-    *reinterpret_cast<__half*>(bimg + split + off) = m;
-    *reinterpret_cast<__half*>(bimg + 2 * split + off) = l;
-  }
-}
-
-// Operand images of fused_ts.cu.
-// (a) L^-1: for K chunk c one tile of R_c = n_pad - 64c rows (output columns j = 64c + r) x 64 k (training
-//     points i = 64c + kk), K-major, SWIZZLE_128B; all hi tiles first (resident in shared memory), then all lo tiles
-//     (streamed).  B[r][kk] = scale * Linv[j][i], zero above the diagonal.  One block per (chunk, 64-row group).
-__global__ void k_build_timg_l(const double* __restrict__ Linv, int n, int n_pad, double scale,
-                               uint8_t* __restrict__ img, uint32_t hi_total) {
-  int c = 0, grp = blockIdx.x;
-  uint32_t off = 0;
-  while (grp >= (n_pad - c * kChunk) / kChunk) {
-    grp -= (n_pad - c * kChunk) / kChunk;
-    off += (uint32_t)(n_pad - c * kChunk) * 128u;
-    ++c;
-  }
-  for (int e = threadIdx.x; e < 64 * 64; e += blockDim.x) {
-    const int r = grp * 64 + (e >> 6), kk = e & 63;
-    const int j = c * kChunk + r, i = c * kChunk + kk;
-    const double v = (j < n && i < n && i <= j) ? Linv[(size_t)j * n + i] * scale : 0.0;
-    const __half hi = __float2half_rn((float)v);
-    const __half lo = __float2half_rn((float)(v - (double)__half2float(hi)));
-    const uint32_t o = off + sw128_offset((uint32_t)r, (uint32_t)(kk >> 3)) + (uint32_t)(kk & 7) * 2u;
-    *reinterpret_cast<__half*>(img + o) = hi;
-    *reinterpret_cast<__half*>(img + hi_total + o) = lo;
-  }
-}
-// (b) training rows: three panels [hi | mid | lo] of [n_pad rows][32 k] fp16 (64-byte rows, SWIZZLE_64B):
-//     k < d: scale_b * (-2 b_ij); k = 30: q_one (pairs with |a|^2 * P in the candidate tile); k = 31: |b_i|^2 * q_sq
-//     (pairs with P1).  Rows i >= n are zero.
 __global__ void k_build_timg_b(const float* __restrict__ train_m2, const float* __restrict__ train_sq, int n, int n_pad,
                                int d, int d_pad, float scale_b, float q_one, float q_sq, uint8_t* __restrict__ img) {
-  const uint32_t split = (uint32_t)n_pad * 64u;
-  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n_pad * 32; e += gridDim.x * blockDim.x) {
-    const int i = e >> 5, j = e & 31;
+  const uint32_t split = (uint32_t)n_pad * K2 * 2u;
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n_pad * K2; e += gridDim.x * blockDim.x) {
+    const int i = e / K2, j = e % K2;
     float v = 0.f;
     if (i < n) {
       if (j < d) v = train_m2[(size_t)i * d_pad + j] * scale_b;
-      else if (j == 30) v = q_one;
-      else if (j == 31) v = train_sq[i] * q_sq;
+      else if (j == K2 - 2) v = q_one;
+      else if (j == K2 - 1) v = train_sq[i] * q_sq;
     }
     const __half h = __float2half_rn(v);
     const float r1 = v - __half2float(h);
     const __half m = __float2half_rn(r1);
     const __half l = __float2half_rn(r1 - __half2float(m));
-    const uint32_t o = swk_offset<32>((uint32_t)i, (uint32_t)(j >> 3)) + (uint32_t)(j & 7) * 2u;
+    const uint32_t o = swk_offset<K2>((uint32_t)i, (uint32_t)(j >> 3)) + (uint32_t)(j & 7) * 2u;
     *reinterpret_cast<__half*>(img + o) = h;
     *reinterpret_cast<__half*>(img + split + o) = m;
     *reinterpret_cast<__half*>(img + 2 * split + o) = l;
   }
 }
-__global__ void k_scale_vec(const float* __restrict__ src, int n, float f, float* __restrict__ dst) {
-  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) dst[e] = src[e] * f;
-}
-
 // K-chunked fp16 hi/mid/lo image of scale * src[n_pad][d_wide] for wide.cu: per (256-row half,
 // 32-column K stage) `panels` panels [hi | mid (| lo)], each [ncols rows][32 fp16], 64-byte rows,
 // SWIZZLE_64B, 8-row groups contiguous -- one contiguous bulk copy per stage.
@@ -817,57 +713,8 @@ extern "C" int bb_model_build(const bb_model_desc* desc, void* d_blob, size_t bl
   k_build_rimg<<<L.n_tiles, 256, 0, stream>>>(dLinv, n, L.n_chunks, scale, B + L.rimg,
                                               (float*)(B + L.linv32), L.n_pad);
   BB_LAUNCH_CHECK();
-  {
-    int n_groups = 0;
-    for (int c = 0; c < L.n_chunks; ++c)
-      for (int sb = c; sb < L.n_chunks;) {
-        const int g = ((sb & 1) == 0 && sb + 1 < L.n_chunks) ? 2 : 1;
-        sb += g;
-        ++n_groups;
-      }
-    k_build_rimg2<<<n_groups, 256, 0, stream>>>(dLinv, n, L.n_chunks, scale, 2, 0, L.n_chunks, L.n_chunks,
-                                                B + L.rimg2);
-    BB_LAUNCH_CHECK();
-    if (L.n_chunks > 4) {  // n_pad > 256: k_fused pairs the V sub-blocks greedily
-      int n_groups2 = 0;
-      for (int c = 0; c < L.n_chunks; ++c)
-        for (int sb = c; sb < L.n_chunks; sb += rimg_group(-2, sb, L.n_chunks)) ++n_groups2;
-      k_build_rimg2<<<n_groups2, 256, 0, stream>>>(dLinv, n, L.n_chunks, scale, -2, 0, L.n_chunks, L.n_chunks,
-                                                   B + L.rimg2g);
-      BB_LAUNCH_CHECK();
-    }
-    if (L.wide) {
-      // one image per V column panel (<= 8 sub-blocks = 512 TMEM columns), stored back to back
-      size_t off4 = 0;
-      for (int lo = 0; lo < L.n_chunks; lo += 8) {
-        const int hi = L.n_chunks < lo + 8 ? L.n_chunks : lo + 8;
-        int n_groups4 = 0;
-        size_t tiles = 0;
-        for (int c = 0; c < hi; ++c) {
-          const int s0 = c > lo ? c : lo;
-          tiles += (size_t)(hi - s0);
-          for (int sb = s0; sb < hi; sb += rimg_group(4, sb, hi)) ++n_groups4;
-        }
-        k_build_rimg2<<<n_groups4, 256, 0, stream>>>(dLinv, n, L.n_chunks, scale, 4, lo, hi, hi, B + L.rimg4 + off4);
-        BB_LAUNCH_CHECK();
-        off4 += tiles * 16384;
-      }
-    }
-  }
-  int dist_k = 0;
-  if (L.d_pad <= 32) {
-    dist_k = 32;
-    k_build_bimg<32><<<L.n_chunks, 256, 0, stream>>>((const float*)(B + L.train_m2), L.n_pad,
-                                                     L.d_pad, dist_scale_b, B + L.bimg);
-    BB_LAUNCH_CHECK();
-  } else if (L.d_pad <= 64) {
-    dist_k = 64;
-    k_build_bimg<64><<<L.n_chunks, 256, 0, stream>>>((const float*)(B + L.train_m2), L.n_pad,
-                                                     L.d_pad, dist_scale_b, B + L.bimg);
-    BB_LAUNCH_CHECK();
-  }
 
-  // ---- fused_ts.cu operand images and their power-of-two scales ----
+  // ---- augmented training image of the tensor-core distances and its power-of-two scales ----
   // A2 = [sa * a | asq * P | P1], Bt = [sb * (-2b) | Q1 | bsq * Q] with sa*sb = P*Q1 = P1*Q = G, so that the
   // distance GEMM accumulates D = G * (|a|^2 + |b|^2 - 2 a.b) = G * t.  All fp16 operands stay below 2^15.
   float ts_sa = 0.f, ts_aug_sq = 0.f, ts_aug_one = 0.f, ts_g = 0.f, ts_kscale = 1.f;
@@ -900,18 +747,12 @@ extern "C" int bb_model_build(const bb_model_desc* desc, void* d_blob, size_t bl
     int e_k = (int)floor(log2(30000.0 / kmax));
     if (e_k > 10) e_k = 10;
     ts_kscale = ldexpf(1.0f, e_k);
-    uint32_t hi_total = 0;
-    int n_groups = 0;
-    for (int r = L.n_pad; r > 0; r -= kChunk) {
-      hi_total += (uint32_t)r * 128u;
-      n_groups += r / kChunk;
-    }
-    k_build_timg_l<<<n_groups, 256, 0, stream>>>(dLinv, n, L.n_pad, scale, B + L.timg_l, hi_total);
-    BB_LAUNCH_CHECK();
-    k_build_timg_b<<<32, 256, 0, stream>>>((const float*)(B + L.train_m2), (const float*)(B + L.train_sq), n, L.n_pad, d,
-                                           L.d_pad, ts_sb, q_one, q_sq, B + L.timg_b);
-    BB_LAUNCH_CHECK();
-    k_scale_vec<<<4, 256, 0, stream>>>((const float*)(B + L.alpha), L.n_pad, 1.0f / ts_kscale, (float*)(B + L.ts_alpha));
+    if (L.ts == 32)
+      k_build_timg_b<32><<<32, 256, 0, stream>>>((const float*)(B + L.train_m2), (const float*)(B + L.train_sq), n,
+                                                 L.n_pad, d, L.d_pad, ts_sb, q_one, q_sq, B + L.timg_b);
+    else
+      k_build_timg_b<64><<<32, 256, 0, stream>>>((const float*)(B + L.train_m2), (const float*)(B + L.train_sq), n,
+                                                 L.n_pad, d, L.d_pad, ts_sb, q_one, q_sq, B + L.timg_b);
     BB_LAUNCH_CHECK();
   }
 
@@ -990,16 +831,11 @@ extern "C" int bb_model_build(const bb_model_desc* desc, void* d_blob, size_t bl
   out->d_alpha64 = (const double*)(B + L.alpha64);
   out->d_xn64 = (const double*)(B + L.xn64);
   out->d_linv32 = (const float*)(B + L.linv32);
-  out->d_bimg = B + L.bimg;
   out->dist_scale_a = dist_scale_a;
   out->dist_scale_b = dist_scale_b;
-  out->dist_k = dist_k;
-  out->d_rimg2 = B + L.rimg2;
-  out->d_rimg2g = L.n_chunks > 4 ? B + L.rimg2g : nullptr;
   if (L.ts) {
-    out->d_timg_l = B + L.timg_l;
     out->d_timg_b = B + L.timg_b;
-    out->d_ts_alpha = (const float*)(B + L.ts_alpha);
+    out->dist_k = L.ts;
     if (!L.wide) out->d_mc_table = (float*)(B + L.mc_table);
     out->ts_sa = ts_sa;
     out->ts_aug_sq = ts_aug_sq;
@@ -1014,12 +850,10 @@ extern "C" int bb_model_build(const bb_model_desc* desc, void* d_blob, size_t bl
     out->d_wimg_bits = B + L.wimg_bits;
     out->d_wnorm_bits = (const float*)(B + L.wnorm_bits);
     out->d_wide_ws = (float*)(B + L.wide_ws);
-    out->d_rimg4 = B + L.rimg4;
     out->d_pend_img = B + L.pend_img;
     out->d_pend_norm = (float*)(B + L.pend_norm2);
     out->d_pend_task = (int32_t*)(B + L.pend_task);
     out->d_kpend_ws = (float*)(B + L.kpend_ws);
-    out->d_wide_vacc = (float*)(B + L.vacc);
     out->d_mc_table = (float*)(B + L.mc_table);
     out->dist_scale_p = dist_scale_p;
     out->dist_scale_wp = dist_scale_wp;

@@ -152,9 +152,8 @@ extern "C" int bb_score_fused_overlapped(const bb_model* m, const bb_acq_spec* a
   //   0  a 4-byte H2D copy from a constant pinned table of cumulative block ends (plain DMA, ordered behind the
   //      block's copy on the same stream): default
   //   1  cuStreamWriteValue32 (stream-ordered memory operation with a system-wide memory barrier in front)
-  // On an idle GPU both cost the same (profiles/r02_time_e2e.txt: 0.44 / 0.41 ms per pass); issued while earlier
-  // work is still draining on the compute stream, as in bench.py's timed loop, the write-value form doubled the pass
-  // (0.80 ms against 0.40 ms).  BB_GATE_PUBLISH=1 selects it for diagnosis.
+  // Issued while earlier work is still draining on the compute stream, as in bench.py's timed loop, the write-value
+  // form can serialise the pass behind that work.  BB_GATE_PUBLISH=1 selects it for diagnosis.
   static const int publish_mode = [] {
     const char* e = getenv("BB_GATE_PUBLISH");
     return (e != nullptr && e[0] == '1') ? 1 : 0;

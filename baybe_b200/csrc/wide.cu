@@ -1,10 +1,10 @@
 // wide.cu -- K(X*, X) for WIDE feature spaces (d in the hundreds or thousands: substance fingerprints,
 // BASELINE config 4) on the tensor cores, and the two-stage scoring path built on it.
 //
-//   stage 1  k_kmat_tc   t[m][i] = |a_m|^2 + |b_i|^2 - 2 a_m.b_i  with the inner product as a
-//                        K-looped tcgen05 GEMM (fp16 split operands, fp32 accumulators in TMEM),
-//                        Matern/RBF epilogue, K* block -> L2-resident workspace (or the caller's
-//                        matrix for bb_kernel_matrix)
+//   stage 1  k_kmat_wg   t[m][i] = |a_m|^2 + |b_i|^2 - 2 a_m.b_i  with the inner product as a
+//                        K-looped warpgroup-MMA GEMM (fp16 split operands, fp32 accumulators in
+//                        registers), Matern/RBF epilogue, K* block -> workspace sized to stay in L2 up to n_pad = 576 (or the
+//                        caller's matrix for bb_kernel_matrix)
 //   stage 2  k_fused<PRE> (fused.cu) posterior GEMM + acquisition + arg-max reading that K* block
 //
 // Candidate layouts: the four float layouts (operand split hi/mid/lo, six products, error 2^-33)
@@ -14,21 +14,23 @@
 // 0/1 matrix (one fp16 panel, no split) and only W is split (hi/mid: W takes at most two distinct
 // values per column, 2^-22 relative is ample): two products.
 //
-// Work item = 256 candidates x <=256 training columns: two UMMA_M=128 accumulators share every
-// B slice (halves the L2 traffic per flop), 2 x 256 TMEM columns.  Warp roles as in fused.cu.
+// Work item = 128 candidates x <= 128 training columns: each consumer warpgroup stages its 64 candidate
+// rows and holds a 64 x 128 fp32 accumulator (64 registers per thread); both share every B slice.  Warp
+// roles as in fused.cu.
 //
 // Reference path replaced: gpytorch Kernel.forward over the comp-rep of a SubstanceParameter space
-// (/root/reference/baybe/kernels/base.py:173-178, parameters/substance.py comp_df), reached from
-// SingleTaskGP.posterior (surrogates/gaussian_process/core.py:268-269).
+// (baybe/kernels/base.py, parameters/substance.py comp_df), reached from SingleTaskGP.posterior
+// (surrogates/gaussian_process/core.py).
 #include "fused_common.cuh"
 
 namespace bb {
 
-constexpr int kWTileM = 256;   // candidates per work item
-constexpr int kWHalfN = 256;   // training columns per work item
+constexpr int kWTileM = 128;   // candidates per work item
+constexpr int kWHalfN = 256;   // training columns per block of the B image
+constexpr int kWItemN = 128;   // training columns per work item
 constexpr int kWK = 32;        // fp16 per K stage: 64-byte rows, SWIZZLE_64B
-constexpr uint32_t kWPanelA = kWTileM * kWK * 2;  // 16 KB: 256 rows x 64 B
-constexpr uint32_t kWPanelB = kWHalfN * kWK * 2;  // 16 KB: 256 rows x 64 B; a stage holds [hi | mid | lo] (floats) or [hi | mid] (bits)
+constexpr uint32_t kWPanelA = kWTileM * kWK * 2;  // 8 KB: 128 rows x 64 B; a stage holds [hi | mid | lo] (floats) or [0/1] (bits)
+constexpr uint32_t kWPanelB = kWItemN * kWK * 2;  // 8 KB: 128 rows x 64 B; a stage holds [hi | mid | lo] (floats) or [hi | mid] (bits)
 
 struct WideParams {
   const void* x;
@@ -36,7 +38,7 @@ struct WideParams {
   int64_t N, ldx;
   int d, n, n_pad, n_halves, n_kc;
   const float *cand_scale, *cand_shift;  // [d]
-  const uint8_t* wimg;                   // B image: per (half, K stage) [hi|mid|lo] swizzled panels
+  const uint8_t* wimg;                   // B image: per (256-column block, K stage) [hi|mid|lo] swizzled panels
   const float* wnorm;                    // [n_pad] additive per-training-row term (|b|^2 or c_i)
   float a_scale, inv_scale;
   const int32_t* train_task;
@@ -51,10 +53,9 @@ struct WideParams {
 struct WideSmem {
   uint8_t* ring;
   float *wnorm_s, *tcov;
-  double* an_part;  // [2 buffers][2 K halves][256 rows], float64: |a|^2 sums d terms
+  double* an_part;  // [2 K halves][128 rows], float64: |a|^2 sums d terms
   int32_t* ttask;
-  uint64_t *full, *empty, *acc_full, *acc_empty;
-  uint32_t* tmem_ptr;
+  uint64_t *full, *empty;
 };
 
 template <bool BITS>
@@ -68,8 +69,8 @@ __host__ __device__ inline size_t wide_carve(uint8_t* base, const WideParams& p,
   };
   const size_t o_ring = take((size_t)p.stages * kStage);
   const size_t o_wn = take((size_t)p.n_pad * 4), o_tt = take((size_t)p.n_pad * 4);
-  const size_t o_an = take(2 * 2 * kWTileM * 8), o_tc = take(kMaxTasks * kMaxTasks * 4);
-  const size_t o_bar = take(16 * 8), o_misc = take(16);
+  const size_t o_an = take(2 * kWTileM * 8), o_tc = take(kMaxTasks * kMaxTasks * 4);
+  const size_t o_bar = take(16 * 8);
   if (s) {
     s->ring = base + o_ring;
     s->wnorm_s = reinterpret_cast<float*>(base + o_wn);
@@ -77,11 +78,8 @@ __host__ __device__ inline size_t wide_carve(uint8_t* base, const WideParams& p,
     s->an_part = reinterpret_cast<double*>(base + o_an);
     s->tcov = reinterpret_cast<float*>(base + o_tc);
     uint64_t* b = reinterpret_cast<uint64_t*>(base + o_bar);
-    s->full = b;           // [<=4]
-    s->empty = b + 4;      // [<=4]
-    s->acc_full = b + 8;   // [1]
-    s->acc_empty = b + 9;  // [1]
-    s->tmem_ptr = reinterpret_cast<uint32_t*>(base + o_misc);
+    s->full = b;       // [<=4]
+    s->empty = b + 4;  // [<=4]
   }
   return off;
 }
@@ -140,7 +138,7 @@ __device__ __forceinline__ uint32_t wide_load_bits16(const WideParams& p, int64_
 }
 
 template <int FAMILY, bool BITS>
-__global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_tc(const WideParams p) {
+__global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_wg(const WideParams p) {
   constexpr int PA = BITS ? 1 : 3;
   constexpr int PB = BITS ? 2 : 3;  // W of the bit-linear form has <= 2 distinct values per column: hi+mid (2^-22) suffices
   constexpr uint32_t kStageA = PA * kWPanelA;
@@ -151,48 +149,43 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_tc(const WideParams p
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0 && (smem_u32(smem_raw) & 1023u) != 0u) __trap();
 
-  if (warp == kWarpMma && lane == 0) {
+  if (tid == 0) {
     for (int i = 0; i < p.stages; ++i) {
-      mbar_init(&s.full[i], kComputeWarps + 1);  // 16 staging warps + the producer's expect_tx
-      mbar_init(&s.empty[i], 1);
+      mbar_init(&s.full[i], kConsumerThreads / 32 + 1);  // 8 staging warps + the producer's expect_tx
+      mbar_init(&s.empty[i], kConsumerWGs);
     }
-    mbar_init(s.acc_full, 1);
-    mbar_init(s.acc_empty, kComputeWarps);
     fence_mbar_init();
-  }
-  if (warp == kWarpProducer) {
-    tmem_alloc(s.tmem_ptr, 512);
-    tmem_relinquish();
   }
   for (int e = tid; e < p.n_pad; e += kFusedThreads) {
     s.wnorm_s[e] = __ldg(p.wnorm + e);
     s.ttask[e] = __ldg(p.train_task + e);
   }
   for (int e = tid; e < p.n_tasks * p.n_tasks; e += kFusedThreads) s.tcov[e] = __ldg(p.task_covar + e);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *s.tmem_ptr;
 
-  if (warp < kComputeWarps) {
+  if (warp < kWarpProducer) {
     // =====================================================================================
-    // compute warps: stage the A operand (candidate rows -> fp16 panels), then the epilogue
+    // consumer warpgroups: stage the A operand (candidate rows -> fp16 panels), issue the MMAs of each
+    // K stage (the next stage is staged while they run), then the epilogue from the accumulators
     // =====================================================================================
-    const int r = tid & 255, kh = tid >> 8;        // staging: row of the item, 16-feature half of the stage
-    const int row_e = tid & 127, cg = tid >> 7;    // epilogue: TMEM lane, 64-column group
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
+    const int wg = warp >> 2, t = tid & 127;
+    const int r = 64 * wg + (t & 63), kh = t >> 6;  // staging: row of the item, 16-feature half of the stage
+    const int ra = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // accumulator rows ra, ra + 8
     uint32_t st = 0, ph = 0;
-    int it = 0;
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x, ++it) {
+    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
       const int tile = item / p.n_halves, half = item - tile * p.n_halves;
       const int64_t row0 = (int64_t)tile * kWTileM;
       const int64_t row = row0 + r;
-      const int ncols = min(kWHalfN, p.n_pad - half * kWHalfN);
+      const int ncols = min(kWItemN, p.n_pad - half * kWItemN);
+      float acc[2][32];
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
       double an = 0.0;
       float cur[16];
       uint32_t curb = 0;
       // bit rows 16-byte aligned: one 128-bit load covers four K stages and is issued four stages ahead
-      // (a one-stage-ahead load would put a full L2/HBM latency on every stage of the staging warps)
       uint4 cur4 = make_uint4(0u, 0u, 0u, 0u), nxt4 = cur4;
       const uint4* brow = nullptr;
       if constexpr (BITS) {
@@ -207,6 +200,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_tc(const WideParams p
         }
       }
       else wide_load16(p, row, kh * 16, cur);
+      uint32_t st_prev = 0;
       for (int kc = 0; kc < p.n_kc; ++kc) {
         const int k0 = kc * kWK + kh * 16;
         uint4 pk[PA][2];
@@ -258,25 +252,64 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_tc(const WideParams p
           *reinterpret_cast<uint4*>(sa + pa * kWPanelA + swk_offset<kWK>((uint32_t)r, (uint32_t)(kh * 2))) = pk[pa][0];
           *reinterpret_cast<uint4*>(sa + pa * kWPanelA + swk_offset<kWK>((uint32_t)r, (uint32_t)(kh * 2 + 1))) = pk[pa][1];
         }
-        fence_proxy_async();
+        fence_proxy_async();  // generic-proxy writes -> visible to the tensor-core (async) proxy
         __syncwarp();
         if (lane == 0) mbar_arrive(&s.full[st]);
+        mbar_wait(&s.full[st], ph);  // both warpgroups' rows staged, B slice landed
+        {
+          const uint32_t a_base = smem_u32(sa) + (uint32_t)wg * (64u * kWK * 2), b_base = smem_u32(sa) + kStageA;
+          const uint32_t bsplit = kWPanelB;
+          wg_fence();
+#pragma unroll
+          for (int kk = 0; kk < 2; ++kk) {
+            const uint64_t ko = (uint64_t)(kk * 2);  // 16 fp16 = 32 bytes
+            const uint64_t a_h = make_wg_desc<kWK>(a_base) + ko;
+            const uint64_t a_md = make_wg_desc<kWK>(a_base + (PA > 1 ? kWPanelA : 0)) + ko;
+            const uint64_t a_l = make_wg_desc<kWK>(a_base + (PA > 2 ? 2 * kWPanelA : 0)) + ko;
+            // both 64-column halves always: a uniform issue (no serialisation); columns beyond ncols read stale
+            // rows of the stage and are never stored
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+              {
+                const uint32_t bj = b_base + (uint32_t)j * (64u * kWK * 2);
+                const uint64_t b_h = make_wg_desc<kWK>(bj) + ko, b_m = make_wg_desc<kWK>(bj + bsplit) + ko;
+                if constexpr (BITS) {
+                  wgmma_64x64(acc[j], a_h, b_h);
+                  wgmma_64x64(acc[j], a_h, b_m);
+                } else {
+                  const uint64_t b_l = make_wg_desc<kWK>(bj + 2 * bsplit) + ko;
+                  wgmma_64x64(acc[j], a_h, b_h);
+                  wgmma_64x64(acc[j], a_h, b_m);
+                  wgmma_64x64(acc[j], a_md, b_h);
+                  wgmma_64x64(acc[j], a_h, b_l);
+                  wgmma_64x64(acc[j], a_l, b_h);
+                  wgmma_64x64(acc[j], a_md, b_m);
+                }
+              }
+            }
+          }
+          wg_commit();
+        }
+        // the previous stage's MMAs are done: release it (this stage's run while the next one is staged)
+        wg_wait<1>();
+        if (kc > 0 && t == 0) mbar_arrive(&s.empty[st_prev]);
+        st_prev = st;
         if (++st == (uint32_t)p.stages) {
           st = 0;
           ph ^= 1u;
         }
       }
-      double* anp = s.an_part + (it & 1) * 2 * kWTileM;
-      anp[kh * kWTileM + r] = an;
+      wg_wait<0>();
+      if (t == 0) mbar_arrive(&s.empty[st_prev]);
+      s.an_part[kh * kWTileM + r] = an;
+      bar_wg(wg);  // an_part of this warpgroup's rows complete
 
       // ---- epilogue: t -> k(t) -> K* block ----
-      mbar_wait(s.acc_full, (uint32_t)(it & 1));
-      tc_fence_after();
-      bar_compute();  // an_part complete
-#pragma unroll 1
-      for (int m = 0; m < 2; ++m) {
-        const int64_t grow = row0 + m * 128 + row_e;
-        const float an_r = (float)(anp[m * 128 + row_e] + anp[kWTileM + m * 128 + row_e]);
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const int rl = ra + 8 * hr;
+        const int64_t grow = row0 + rl;
+        const float an_r = (float)(s.an_part[rl] + s.an_part[kWTileM + rl]);
         int ct = 0;
         if (p.scaled && p.task_col >= 0 && grow < p.N) {
           float tv;
@@ -289,134 +322,71 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_tc(const WideParams p
           ct = min(max(__float2int_rn(tv), 0), p.n_tasks - 1);
         }
         const float* tcrow = s.tcov + ct * p.n_tasks;
-#pragma unroll 1
-        for (int j = 0; j < 4; ++j) {
-          const int col = cg * 64 + j * 16;
-          if (col >= ncols) break;  // warp-uniform: cg and ncols are
-          float v[16];
-          tmem_ld16(tmem_base + lane_base + (uint32_t)(m * kWHalfN + col), v);
-          tmem_ld_wait();
-          const int i0 = half * kWHalfN + col;
-          float k[16];
+        if (grow >= p.out_rows) continue;
+        float* dst = p.out + grow * p.ldk;
 #pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const float t = fmaf(v[e], p.inv_scale, an_r + s.wnorm_s[i0 + e]);
-            float kv = kernel_from_t<FAMILY>(t);
-            if (p.scaled) kv *= tcrow[s.ttask[i0 + e]];
-            k[e] = (i0 + e < p.n) ? kv : 0.f;
-          }
-          if (grow < p.out_rows) {
-            float* dst = p.out + grow * p.ldk + i0;
-            if (p.vec_ok && i0 + 16 <= p.out_cols) {
+        for (int j = 0; j < 2; ++j) {
+          if (j * 64 >= ncols) break;  // warp-uniform
 #pragma unroll
-              for (int q = 0; q < 4; ++q)
-                *reinterpret_cast<float4*>(dst + 4 * q) = make_float4(k[4 * q], k[4 * q + 1], k[4 * q + 2], k[4 * q + 3]);
+          for (int q = 0; q < 8; ++q) {
+            const int i0 = half * kWItemN + j * 64 + 8 * q + 2 * (lane & 3);
+            float k[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float tt = fmaf(acc[j][4 * q + 2 * hr + e], p.inv_scale, an_r + s.wnorm_s[i0 + e]);
+              float kv = kernel_from_t<FAMILY>(tt);
+              if (p.scaled) kv *= tcrow[s.ttask[i0 + e]];
+              k[e] = (i0 + e < p.n) ? kv : 0.f;
+            }
+            if (p.vec_ok && i0 + 2 <= p.out_cols) {
+              *reinterpret_cast<float2*>(dst + i0) = make_float2(k[0], k[1]);
             } else {
-#pragma unroll
-              for (int e = 0; e < 16; ++e)
-                if (i0 + e < p.out_cols) dst[e] = k[e];
+              if (i0 < p.out_cols) dst[i0] = k[0];
+              if (i0 + 1 < p.out_cols) dst[i0 + 1] = k[1];
             }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s.acc_empty);
-    }
-  } else if (warp == kWarpProducer) {
-    // =====================================================================================
-    // producer: one bulk copy (TMA engine) per K stage of the B image
-    // =====================================================================================
-    if (elect_one()) {  // elect.sync: straight UBLKCP (fused_common.cuh)
-      uint32_t st = 0, ph = 0;
-      for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-        const int half = item % p.n_halves;
-        const int ncols = min(kWHalfN, p.n_pad - half * kWHalfN);
-        const uint32_t bytes = (uint32_t)PB * (uint32_t)ncols * (kWK * 2);
-        const uint8_t* src = p.wimg + (size_t)half * p.n_kc * (PB * kWPanelB);  // only the last half is narrower
-        for (int kc = 0; kc < p.n_kc; ++kc) {
-          mbar_wait_relaxed(&s.empty[st], ph ^ 1u);
-          mbar_expect_tx(&s.full[st], bytes);
-          bulk_g2s(s.ring + (size_t)st * kStage + kStageA, src + (size_t)kc * bytes, bytes, &s.full[st]);
-          if (++st == (uint32_t)p.stages) {
-            st = 0;
-            ph ^= 1u;
-          }
-        }
-      }
+      bar_wg(wg);  // an_part is rewritten by the next item
     }
   } else {
     // =====================================================================================
-    // MMA issuer: D[m] (128 x ncols, fp32, TMEM) += A_panel[m] (128 x 32) * B_panel^T
-    // converged warp, one lane issues under elect.sync (no ELECT/R2UR/BRA.U.ANY wrapper per MMA, fused_common.cuh)
+    // producer: one bulk copy (TMA engine) per K stage of the B image
     // =====================================================================================
-    {
+    if (elect_one()) {
       uint32_t st = 0, ph = 0;
-      int it = 0;
-      for (int item = blockIdx.x; item < p.num_items; item += gridDim.x, ++it) {
-        const int half = item % p.n_halves;
-        const int ncols = min(kWHalfN, p.n_pad - half * kWHalfN);
-        const uint32_t idesc = make_idesc_f16(kTileM, ncols);
-        const uint32_t bsplit = (uint32_t)ncols * (kWK * 2);
-        mbar_wait_relaxed(s.acc_empty, (uint32_t)((it & 1) ^ 1));  // previous epilogue drained TMEM
-        tc_fence_after();
+      for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
+        // columns [128 h, 128 h + ncols) = rows sub * 128.. of each panel of 256-column block h / 2
+        const int half = item % p.n_halves, blk = half >> 1, sub = half & 1;
+        const int ncols = min(kWItemN, p.n_pad - half * kWItemN);
+        const int bcols = min(kWHalfN, p.n_pad - blk * kWHalfN);
+        const uint32_t pbytes = (uint32_t)bcols * (kWK * 2), bytes = (uint32_t)ncols * (kWK * 2);
+        const uint8_t* src = p.wimg + (size_t)blk * p.n_kc * (PB * 2 * kWPanelB) + (size_t)sub * kWPanelB;
         for (int kc = 0; kc < p.n_kc; ++kc) {
-          mbar_wait_relaxed(&s.full[st], ph);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(s.ring + (size_t)st * kStage), b_base = a_base + kStageA;
-          const uint64_t b_h = make_swk_desc<kWK>(b_base), b_m = make_swk_desc<kWK>(b_base + bsplit),
-                         b_l = make_swk_desc<kWK>(b_base + (PB > 2 ? 2 : 0) * bsplit);
-          if (elect_one()) {
+          mbar_wait_relaxed(&s.empty[st], ph ^ 1u);
+          mbar_expect_tx(&s.full[st], (uint32_t)PB * bytes);
 #pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {
-              const uint64_t ko = (uint64_t)(kk * 2);  // 16 fp16 = 32 bytes
-#pragma unroll
-              for (int m = 0; m < 2; ++m) {
-                const uint32_t d_addr = tmem_base + (uint32_t)(m * kWHalfN);
-                const uint32_t a_m0 = a_base + (uint32_t)m * (128u * kWK * 2);
-                const uint32_t acc = (kc > 0 || kk > 0) ? 1u : 0u;
-                const uint64_t a_h = make_swk_desc<kWK>(a_m0);
-                if constexpr (BITS) {
-                  umma_f16(d_addr, a_h + ko, b_h + ko, idesc, acc);
-                  umma_f16(d_addr, a_h + ko, b_m + ko, idesc, 1u);
-                } else {
-                  const uint64_t a_md = make_swk_desc<kWK>(a_m0 + kWPanelA), a_l = make_swk_desc<kWK>(a_m0 + 2 * kWPanelA);
-                  umma_f16(d_addr, a_h + ko, b_h + ko, idesc, acc);
-                  umma_f16(d_addr, a_h + ko, b_m + ko, idesc, 1u);
-                  umma_f16(d_addr, a_md + ko, b_h + ko, idesc, 1u);
-                  umma_f16(d_addr, a_h + ko, b_l + ko, idesc, 1u);
-                  umma_f16(d_addr, a_l + ko, b_h + ko, idesc, 1u);
-                  umma_f16(d_addr, a_md + ko, b_m + ko, idesc, 1u);
-                }
-              }
-            }
-            umma_commit(&s.empty[st]);
-          }
-          __syncwarp();
+          for (int pb = 0; pb < PB; ++pb)
+            bulk_g2s(s.ring + (size_t)st * kStage + kStageA + pb * kWPanelB, src + (size_t)(kc * PB + pb) * pbytes,
+                     bytes, &s.full[st]);
           if (++st == (uint32_t)p.stages) {
             st = 0;
             ph ^= 1u;
           }
         }
-        if (elect_one()) umma_commit(s.acc_full);
-        __syncwarp();
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kWarpProducer) tmem_dealloc(tmem_base, 512);
 }
 
 template <int FAMILY, bool BITS>
 static int launch_kmat_one(WideParams& p, int sms, int max_smem, cudaStream_t stream) {
-  p.stages = BITS ? 4 : 2;
+  p.stages = 4;
   const size_t smem = wide_carve<BITS>(nullptr, p, nullptr);
   BB_CHECK_SUPPORTED(smem <= (size_t)max_smem, "wide kernel-matrix path: shared-memory budget exceeded (%zu bytes)", smem);
-  BB_SMEM_OPTIN_ONCE((k_kmat_tc<FAMILY, BITS>));
+  BB_SMEM_OPTIN_ONCE((k_kmat_wg<FAMILY, BITS>));
   const int grid = p.num_items < sms ? p.num_items : sms;
-  k_kmat_tc<FAMILY, BITS><<<grid, kFusedThreads, smem, stream>>>(p);
+  k_kmat_wg<FAMILY, BITS><<<grid, kFusedThreads, smem, stream>>>(p);
   BB_LAUNCH_CHECK();
   return BB_OK;
 }
@@ -449,7 +419,7 @@ static int launch_kmat_cols(const bb_model* m, const WideColumns& c, const void*
   p.d = m->d;
   p.n = c.n;
   p.n_pad = c.n_pad;
-  p.n_halves = (c.n_pad + kWHalfN - 1) / kWHalfN;
+  p.n_halves = (c.n_pad + kWItemN - 1) / kWItemN;
   p.n_kc = m->d_wide / kWK;
   p.cand_scale = m->d_cand_scale;
   p.cand_shift = m->d_cand_shift;
@@ -466,7 +436,7 @@ static int launch_kmat_cols(const bb_model* m, const WideColumns& c, const void*
   p.ldk = ldk;
   p.out_rows = out_rows;
   p.out_cols = out_cols;
-  p.vec_ok = ((ldk & 3) == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0) ? 1 : 0;
+  p.vec_ok = ((ldk & 1) == 0 && (reinterpret_cast<uintptr_t>(d_out) & 7) == 0) ? 1 : 0;
   p.num_items = (int)((N + kWTileM - 1) / kWTileM) * p.n_halves;
   p.bits_vec = (bits && (ldx & 15) == 0 && (reinterpret_cast<uintptr_t>(d_x) & 15) == 0 && (m->d & 127) == 0) ? 1 : 0;
   int max_smem = 0, sms = 0;
@@ -604,7 +574,7 @@ int launch_pend_images(const bb_model* m, int32_t layout, const float* d_pend_x,
   return BB_OK;
 }
 
-// One block of candidates: k(x*, pending) through k_kmat_tc, then the cross-covariances from the K* block
+// One block of candidates: k(x*, pending) through k_kmat_wg, then the cross-covariances from the K* block
 // that launch_kmat_wide left in the workspace.
 int launch_cross_wide(const bb_model* m, const void* d_x, int32_t layout, int64_t nb, int64_t ldx,
                       const float* d_pend_beta, int32_t P, float* d_cross_blk, cudaStream_t stream) {
@@ -621,7 +591,10 @@ int launch_cross_wide(const bb_model* m, const void* d_x, int32_t layout, int64_
   if (rc != BB_OK) return rc;
   const size_t smem = (size_t)P * m->n_pad * sizeof(float);
   BB_CUDA(cudaFuncSetAttribute(k_cross_pre, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_cross_pre<<<148 * 4, 256, smem, stream>>>(m->d_wide_ws, m->d_kpend_ws, d_pend_beta, P, m->n_pad, nb,
+  int sms = 0, max_smem = 0;
+  rc = device_limits(&sms, &max_smem);
+  if (rc != BB_OK) return rc;
+  k_cross_pre<<<sms * 4, 256, smem, stream>>>(m->d_wide_ws, m->d_kpend_ws, d_pend_beta, P, m->n_pad, nb,
                                               m->y_std * m->y_std, d_cross_blk);
   BB_LAUNCH_CHECK();
   return BB_OK;

@@ -1,5 +1,5 @@
 """Host side of the scoring engine: PyTorch owns device memory and streams, every numeric step
-is a C-ABI call into ``libbaybe_b200.so`` (hand-written sm_100a CUDA).  The calls are exposed
+is a C-ABI call into ``libbaybe_b200.so`` (hand-written sm_90a CUDA).  The calls are exposed
 as ``torch.library`` custom ops in the ``baybe_b200::`` namespace so that they compose with
 ``torch.no_grad`` code the way the reference's BoTorch calls do.
 
@@ -44,7 +44,7 @@ def _ptr(t: torch.Tensor | None) -> C.c_void_p:
 def _require_cuda(device: torch.device | str | None) -> torch.device:
     if not torch.cuda.is_available():
         raise RuntimeError(
-            "baybe_b200 needs a CUDA device (sm_100a); there is no CPU fallback for the scoring path"
+            "baybe_b200 needs a CUDA device (sm_90a); there is no CPU fallback for the scoring path"
         )
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     if dev.type != "cuda":

@@ -6,7 +6,7 @@ the batch, and for each discrete configuration a multi-start L-BFGS over the con
 (``hybrid.py:110``) on an acquisition function built by ``acquisition/_builder.py:195-334`` (``X_baseline`` = the
 training inputs for the noisy-EI family, ``:319-324``).
 
-B200-first design: no gradient ascent.  The scoring path runs at 10^8-10^9 candidates per second, so a greedy step
+Design: no gradient ascent.  The scoring path runs at 10^8-10^9 candidates per second, so a greedy step
 is a *search by scoring*: every discrete configuration x a shared scrambled-Sobol set of continuous points is scored
 in one sweep, the best seeds are refined by sweeps over shrinking boxes, and the winner joins the pending set.  The
 result is deterministic for a seed and is judged the way a stochastic multi-start optimiser has to be: by the
@@ -16,7 +16,7 @@ qNEI (``acquisition/acqfs.py:227-232``) is evaluated in its conditional form.  W
 joint Cholesky taken in the order [C; x],
     f_x,s = mu_x + r_x . Z_C[s] + sqrt(var_x - |r_x|^2) z_x,s,   r_x = Sigma_xC L_C^-T,
     value(x) = mean_s relu(o(f_x,s) - g_s),   g_s = max_C o(f_C,s)
-so one sweep over N candidates is: K(X, X_train) (``bb_kernel_matrix``, hand-written, 5 TB/s), the posterior
+so one sweep over N candidates is: K(X, X_train) (``bb_kernel_matrix``, hand-written), the posterior
 moments and the covariance with the pending points (``bb_posterior``), ONE dense GEMM Sigma_XC @ [W | L_C^-T]
 (cuBLAS through ``torch.matmul``: a plain library GEMM) and ``bb_nei_reduce`` (hand-written).  The m x m setup
 (posterior covariance of C, its Cholesky, W = L_C^-T Z_C^T) is float64 torch on the device, once per greedy step.

@@ -5,7 +5,7 @@ its context, ``posterior`` / ``posterior_stats`` take candidates in experimental
 and the model owns input Normalize / output Standardize (core.py:130-141 "Scaling Workaround").
 
 The fitted model lives on the GPU as a ``DeviceGP`` (caches built by ``bb_model_build``); every
-posterior evaluation runs the tcgen05 kernel.  Hyper-parameter fitting (SURVEY.md row f1, *before*
+posterior evaluation runs the wgmma kernel.  Hyper-parameter fitting (SURVEY.md row f1, *before*
 the hot path) evaluates the fit criterion -- exact marginal likelihood, or the leave-one-out pseudo-likelihood
 for transfer-learning search spaces -- and its gradient on the GPU (``bb_fit_eval[_loo]``, float64)
 under scipy's L-BFGS-B on the BayBE preset's MAP objective

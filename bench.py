@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- candidates/sec scored (qLogEI, 1M x 20D discrete space), BASELINE.json's metric.
 
-    python bench.py --gpus N --steps K --warmup W              # our arm (CUDA, sm_100a), BASELINE config 2
+    python bench.py --gpus N --steps K --warmup W              # our arm (CUDA, sm_90a), BASELINE config 2
     python bench.py --config 4|5 --gpus N ...                  # the other single-path configs (extra lines)
     python bench.py --impl reference --steps K --warmup W      # reference arm (CPU restatement)
 
@@ -12,6 +12,11 @@ the candidate set is row-sharded, SURVEY.md 8e) and the global winner comes out 
 per rank folding the packed (score, index) key into every peer's slot over NVLink (no host-issued collective).
 The same run also reports STRONG scaling (the 1M set split N ways).  The only place this file touches
 ``oracle/`` is the CPU-baseline leg and the ``--impl reference`` arm.
+
+``--dump-outputs DIR`` (config 2) writes what the timed path returned in its last timed step -- the global arg-max
+as ``DIR/best_value.npy`` and ``DIR/best_index.npy`` -- and the posterior mean, variance and score of a fixed, seeded
+sample of 65,536 rows (``sample_*.npy``), all float64, so that two builds can be compared on the same inputs.  The
+sample comes from one more (untimed) call of the same deterministic path on the same inputs after the timed loop.
 """
 from __future__ import annotations
 
@@ -55,32 +60,12 @@ def _workload(n_rows: int, shard: int = 0):
     return base, other.candidates
 
 
-def _ncu_traffic_bytes():
-    """dram__bytes_read.sum + dram__bytes_write.sum of the headline kernel from the committed ncu
-    --set full capture (profiles/, one launch at this exact workload): the newest k_fused_ts summary."""
-    names = sorted(p.name for p in (ROOT / "profiles").glob("r0*_k_fused_ts*_ncu_full_summary.txt"))[::-1]
-    for name in names + ["r01_k_fused_tc_ncu_full_summary.txt"]:
-        f = ROOT / "profiles" / name
-        if not f.exists():
-            continue
-        tot, found = 0.0, 0
-        for line in f.read_text().splitlines():
-            parts = line.split()
-            if parts and parts[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                mult = {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1.0}.get(parts[2], 1.0)
-                tot += float(parts[1]) * mult
-                found += 1
-        if found == 2:
-            return tot, name
-    return None, None
-
-
 def _peaks() -> dict:
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
         return {"bf16_tflops": d["bf16_tflops"], "hbm_gbs": d["hbm_gbs"], "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense fp16, 700 W card)"}
 
 
 class ClockSampler:
@@ -222,7 +207,7 @@ class _Timer:
         import torch
 
         self.torch, self.dev, self.world = torch, dev, world
-        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+        self.flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def __call__(self, fn, k, w_, idle_start=False):
         """idle_start: synchronise after the (untimed) L2 flush, so that the timed call starts on an idle device and
@@ -332,6 +317,16 @@ def run_b200(args):
     with ClockSampler(local_rank) as clocks:
         total_ms = timed(step_device, steps, warmup)
     best_val, best_idx = unpack_best(int(key_host.item()))
+    if args.dump_outputs and rank == 0:
+        # besides the arg-max the timed step returns: posterior moments and scores of the same inputs at a fixed,
+        # seeded sample of 65,536 rows, so that two builds are compared value by value and not only by their winner
+        import numpy as np
+
+        rows = torch.from_numpy(np.sort(np.random.default_rng(0).choice(N_PER_GPU, 65_536, replace=False))).to(dev)
+        scores, _ = gp.score(acq, x_dev, z, index_offset=offset)
+        mu, var = gp.posterior(x_dev)
+        _dump(args.dump_outputs, best_value=best_val, best_index=best_idx, sample_rows=rows.cpu(),
+              sample_mu=mu[rows].cpu(), sample_var=var[rows].cpu(), sample_score=scores[rows].cpu())
     e2e_ms = timed(step_e2e, steps, warmup, idle_start=True)
     key_coded = int(key_host.item())
     e2e32_ms = timed(step_e2e_f32, max(3, steps // 4), 2, idle_start=True) / max(3, steps // 4)
@@ -369,7 +364,6 @@ def run_b200(args):
         peaks = _peaks()
         flops = N_PER_GPU * (2.0 * N_TRAIN * N_TRAIN + 2.0 * N_TRAIN * D)  # SURVEY 8d: 2n^2 + 2nd per candidate
         achieved = flops / (kern_ms * 1e-3) / 1e12
-        traffic, traffic_src = _ncu_traffic_bytes()
         cpu = None
         if world == 1 and not args.no_cpu_baseline:
             r = _cpu_reference(6, 1, full_steps=1)
@@ -391,8 +385,9 @@ def run_b200(args):
                               "bb_allreduce_best: one warp per rank, atomicMax.sys into every peer's slot over NVLink "
                               "(CUDA IPC mapped), no host-issued collective" if peer.kind == "peer" else
                               "BB_PEER_REDUCE=0: host-issued ncclAllReduce(MAX, int64) per step"),
-                "precision": "distance GEMM (fp16 hi/mid/lo split, 2^-33) and K* L^-T (fp16 hi/lo split, A operand "
-                             "in tensor memory) on tcgen05, fp32 TMEM accumulate; packed-fp32 Matern epilogue and MC",
+                "precision": "augmented distance GEMM (fp16 hi/mid/lo split, six products, K = 32) and K* L^-T (fp16 "
+                             "hi/lo split, three products, K* as the register A operand) on wgmma with fp32 register "
+                             "accumulators; fp32 Matern epilogue and MC",
                 "best": {"value": best_val, "index": best_idx},
                 "e2e_coded_matches_resident": key_coded == int(key_host.item()) if world == 1 else None,
             },
@@ -409,14 +404,12 @@ def run_b200(args):
             "gpu_launches": launches,
             "clocks": clocks.summary(),
             "roofline": {
-                "bound": "tensor", "kernel": "k_fused_ts<matern52>", "achieved": achieved,
+                "bound": "tensor", "kernel": "k_fused<matern52>", "achieved": achieved,
                 "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": achieved / peaks["bf16_tflops"],
-                "traffic": traffic, "traffic_unit": "bytes per launch (ncu --set full, profiles/)",
-                "traffic_source": traffic_src,
                 "algorithmic_bytes": N_PER_GPU * (4 * D + 4), "kernel_ms": kern_ms, "peak_source": peaks["source"],
                 "note": "algorithmic flops = N*(2n^2 + 2nd) (SURVEY 8d); the tensor pipe executes 3 split products "
-                        "over 8.5/16 of the n^2 (triangular skip at 16-column granularity) plus 6 split products of "
-                        "the distance GEMM over K = 32; see DESIGN.md",
+                        "over 10/16 of the n^2 (triangular skip at 64-column granularity) plus 6 split products "
+                        "of the distance GEMM over K = 32",
             },
             "cpu_baseline": cpu,
         }
@@ -466,9 +459,9 @@ def run_other(args):
         name = "BASELINE config 4: 10M x 2048-bit Morgan-like fingerprints (bit-packed), n=512, ScaleKernel(RBF), qLogEI S=512"
         scaling, metric = "strong", "candidates/sec scored (qLogEI, 10M x 2048-bit fingerprint space)"
         kern_rows = min(hi - lo, 262_144)
-        kernel_fn = lambda: gp.kernel_matrix(x[:kern_rows])  # noqa: E731  (k_kmat_tc alone: the dominant kernel)
+        kernel_fn = lambda: gp.kernel_matrix(x[:kern_rows])  # noqa: E731  (k_kmat_wg alone: the dominant kernel)
         kern_flops = kern_rows * 2.0 * n_tr * d_feat
-        kern_name = "k_kmat_tc<rbf,bits> (distance GEMM of one 262,144-row block)"
+        kern_name = "k_kmat_wg<rbf,bits> (distance GEMM of one 262,144-row block)"
         rl_note = ("algorithmic flops = rows*2*n*d; the bit-linear form issues 2 fp16 split products, so the tensor "
                    "pipe executes 2x this")
         total = total_rows
@@ -486,7 +479,7 @@ def run_other(args):
         scaling, metric = "strong", "candidates/sec scored (qLogEI, 4 x 250k transfer-learning space)"
         kernel_fn = lambda: gp.score(acq, x, z, want_scores=False)  # noqa: E731
         kern_flops = (hi - lo) * (2.0 * n_tr * n_tr + 2.0 * n_tr * d_feat)
-        kern_name = "k_fused<matern52> (FFMA2 distances, tcgen05 V contraction, n_pad=512)"
+        kern_name = "k_fused<matern52> (CUDA-core distances, wgmma V contraction, n_pad=512)"
         rl_note = "algorithmic flops = rows*(2n^2 + 2nd)"
         total = total_rows
     acq = AcqConfig(kind="qLogEI", best_f=gp.best_f(AcqConfig(kind="qLogEI")))
@@ -532,6 +525,16 @@ def run_other(args):
         dist.destroy_process_group()
 
 
+def _dump(out_dir: str, **arrays) -> None:
+    """The arrays a caller of the timed path receives, as float64 .npy files under out_dir."""
+    import numpy as np
+
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    for name, v in arrays.items():
+        np.save(d / f"{name}.npy", np.asarray(v, dtype=np.float64).reshape(-1))
+
+
 def _emit(line: dict) -> None:
     """Write the ONE JSON line to the real stdout (fd saved before libraries could print to it)."""
     os.write(_REAL_STDOUT, (json.dumps(line) + "\n").encode())
@@ -568,7 +571,7 @@ def run_hybrid(args):
     rows_per_step = 16 * (len(disc) * min(search.n_sobol, search.max_rows // len(disc))
                           + search.n_rounds * search.n_seeds * search.n_local)
     cb = np.array([[0.0] * d_cont, [1.0] * d_cont])
-    steps, warmup = max(1, min(args.steps, 5)), 1
+    steps, warmup = args.steps, 1
 
     def step():
         return hy.recommend_hybrid(gp, acq, disc, cb, 16, None, S, 3, search)
@@ -605,7 +608,11 @@ def main():
     ap.add_argument("--impl", choices=["b200", "reference"], default="b200")
     ap.add_argument("--config", type=int, choices=[2, 3, 4, 5], default=2)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (config 2)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "b200" or args.config != 2):
+        ap.error("--dump-outputs is implemented for the CUDA arm of config 2")
     if args.impl == "reference":
         run_reference(args)
     elif args.config == 2:

@@ -1,5 +1,5 @@
 /*
- * baybe_b200.h -- C ABI of libbaybe_b200.so: the B200-native (sm_100a) replacement for the
+ * baybe_b200.h -- C ABI of libbaybe_b200.so: the H100-native (sm_90a) replacement for the
  * recommend-time hot path of emdgroup/baybe (GP posterior over a full discrete candidate set
  * + acquisition scoring + arg-max / top-k).
  *
@@ -133,21 +133,20 @@ typedef struct bb_model {
   const int32_t* d_train_task; /* [n_pad]                                                 */
   const float* d_task_covar; /* [T*T] fp32, prior_scale folded in                         */
   const float* d_mean_const; /* [T]                                                       */
-  const void* d_rimg;        /* fp16 hi/lo swizzled tiles of L^-1 (tcgen05 B operand)     */
+  const void* d_rimg;        /* fp16 hi/lo swizzled tiles of L^-1 (wgmma B operand)       */
   const double* d_linv;      /* [n*n] row-major L^-1, float64                             */
   const double* d_alpha64;   /* [n]                                                       */
   const double* d_xn64;      /* [n*d] normalised training inputs, float64                 */
   const float* d_linv32;     /* [n_pad*n_pad] row-major L^-1, fp32 (zero padded)          */
-  const void* d_bimg;        /* fp16 hi/mid/lo swizzled tiles of the (-2 x) scaled training
-                                rows: B operand of the tensor-core distance GEMM            */
+  const void* d_bimg;        /* unused (NULL); kept for the ABI                             */
   float dist_scale_a;        /* power-of-two scales folded into the fp16 images of the      */
   float dist_scale_b;        /* candidate rows (a) and training rows (b)                    */
-  int32_t dist_k;            /* K extent of the d_bimg tiles: 32 (d_pad<=32), 64, or 0 = none */
+  int32_t dist_k;            /* K extent of d_timg_b: 32 (d <= 30), 64 (d <= 62), 0 = none */
   int32_t pad_;
-  const void* d_rimg2;       /* L^-1 image grouped in 128-column pair tiles (fused_tc kernel)   */
+  const void* d_rimg2;       /* unused (NULL); kept for the ABI                                 */
   /* wide-feature path (n_pad*d_pad*4 > 56 KB, e.g. fingerprint spaces): K-chunked operand images of
-   * the tensor-core distance GEMM and an L2-sized K* workspace, all inside the blob */
-  int32_t wide;              /* 1: scoring runs k_kmat_tc + the K*-reading posterior kernel     */
+   * the tensor-core distance GEMM and a K* workspace (whole waves, <= 40 MB up to n_pad = 640), all inside the blob */
+  int32_t wide;              /* 1: scoring runs k_kmat_wg + the K*-reading posterior kernel     */
   int32_t d_wide;            /* d rounded up to 32 (K extent of the images)                     */
   const void* d_wimg;        /* fp16 hi/mid/lo image of (-2 x) scaled training rows             */
   const void* d_wimg_bits;   /* same for the bit-linear form t = sum_j x_j W_ij + c_i           */
@@ -156,8 +155,8 @@ typedef struct bb_model {
   int64_t wide_ws_rows;
   float dist_scale_w;        /* power-of-two scale folded into d_wimg_bits                      */
   int32_t pad2_;
-  const void* d_rimg4;       /* L^-1 image grouped in <=256-column tiles (K*-reading kernel)    */
-  const void* d_rimg2g;      /* L^-1 image in greedy 128-column pairs (k_fused, n_pad > 256), or NULL */
+  const void* d_rimg4;       /* unused (NULL); kept for the ABI                                 */
+  const void* d_rimg2g;      /* unused (NULL); kept for the ABI                                 */
   /* wide path, pending points (sequential greedy): scratch images of <=31 pending rows as extra K columns */
   void* d_pend_img;          /* [64 rows] K-chunked split image, rebuilt per bb_posterior call          */
   float* d_pend_norm;        /* [64]                                                                    */
@@ -166,15 +165,15 @@ typedef struct bb_model {
   float dist_scale_p;        /* power-of-two scales of the pending images (float form / bit-linear form) */
   float dist_scale_wp;
   float* d_mc_table;         /* [1024] per-call qLogEI table of the K*-reading kernel (acq_math.cuh)             */
-  float* d_wide_vacc;        /* [wide_ws_rows] |V|^2 partial between the two column-panel passes (n_pad > 512) */
-  /* fused_ts.cu (n_pad <= 256, d <= 30; NULL otherwise): operand images of the kernel that keeps the K* operand
-   * in tensor memory, and the power-of-two scales folded into them */
-  const void* d_timg_l;      /* L^-1: hi tiles (chunk c: n_pad - 64c rows x 64 k, SW128), then the lo tiles        */
-  const void* d_timg_b;      /* training rows [-2b | q | |b|^2 q'] as hi/mid/lo panels of 32 k (SW64)              */
-  const float* d_ts_alpha;   /* [n_pad] alpha / ts_kscale                                                          */
+  float* d_wide_vacc;        /* unused (NULL); kept for the ABI                                                 */
+  /* tensor-core distances (n_pad <= 256, d <= 62; NULL otherwise): augmented training image
+   * and the power-of-two scales folded into it */
+  const void* d_timg_l;      /* unused (NULL); kept for the ABI                                                    */
+  const void* d_timg_b;      /* training rows [-2b | q | |b|^2 q'] as hi/mid/lo panels of dist_k k (SW64 / SW128)   */
+  const float* d_ts_alpha;   /* unused (NULL); kept for the ABI                                                    */
   float ts_sa;               /* candidate rows are multiplied by ts_sa                                             */
-  float ts_aug_sq;           /* K column 30 of the candidate tile = |a|^2 * ts_aug_sq                              */
-  float ts_aug_one;          /* K column 31 of the candidate tile = ts_aug_one                                     */
+  float ts_aug_sq;           /* K column dist_k - 2 of the candidate tile = |a|^2 * ts_aug_sq                      */
+  float ts_aug_one;          /* K column dist_k - 1 of the candidate tile = ts_aug_one                             */
   float ts_g;                /* accumulator * ts_g = scaled squared distance                                       */
   float ts_kscale;           /* K* is multiplied by ts_kscale before the fp16 hi/lo split                          */
   int32_t pad3_;
@@ -354,7 +353,7 @@ int bb_nei_reduce(const float* d_out, int64_t ld, int32_t S, int32_t m, const fl
                   void* stream);
 
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
- * tests to separate tcgen05-path errors from formula errors.  Not called by the product. -- */
+ * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
 int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
                             int64_t ldx, float* d_mu, float* d_var, void* stream);
 /* test-only: record pipeline events of CTA 0 of the following fused launches into d_buf

@@ -1,4 +1,4 @@
-"""pytest configuration: ``gpu`` marker = needs a real B200; everything else runs on CPU."""
+"""pytest configuration: ``gpu`` marker = needs a real H100; everything else runs on CPU."""
 import sys
 from pathlib import Path
 
@@ -10,7 +10,7 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (sm_100a)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (sm_90a)")
 
 
 @pytest.fixture(scope="session")

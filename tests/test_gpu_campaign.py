@@ -1,6 +1,6 @@
 """The real ``Campaign`` -> ``B200BotorchRecommender`` flow of tests/test_campaign_binding.py on the CUDA engine
-(no stand-in: ``torch.cuda.is_available()`` keeps ``DeviceGP``).  ``baybe`` comes from ``baseline/_ref`` (the
-offline ``pip install --no-deps --target`` of the reference, which travels to the GPU box) with the cattrs
+(no stand-in: ``torch.cuda.is_available()`` keeps ``DeviceGP``).  ``baybe`` comes from ``oracle/_ref`` (the
+offline ``pip install --no-deps --target`` of the reference made by ``build()``) with the cattrs
 stand-in of ``tests/shims``; skipped when the reference package is not on the box."""
 from __future__ import annotations
 
@@ -14,7 +14,7 @@ from tests.test_campaign_binding import (REF, bb, test_campaign_posterior_stats_
                                          test_subset_generating_constraint_is_honoured)
 
 pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(REF is None, reason="the reference package (baybe) is not available on this box")]
+              pytest.mark.skipif(REF is None, reason="the reference package (baybe) is not installed under oracle/_ref")]
 
 
 def test_engine_is_the_cuda_one(bb, cuda_device):  # noqa: F811

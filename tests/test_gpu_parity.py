@@ -46,6 +46,8 @@ WORKLOADS = {
     "n300_d12_m32": lambda: numeric_grid_workload(N=2000, d=12, n=300, family="matern32", seed=4,
                                                   lengthscale=0.8),
     "n512_d20_m52": lambda: numeric_grid_workload(N=3000, d=20, n=512, seed=5),
+    # 30 < d <= 62 with n_pad <= 256: the K = 64 augmented distance GEMM
+    "n200_d48_m52": lambda: numeric_grid_workload(N=2000, d=48, n=200, seed=7, lengthscale=2.0),
     "n33_d3_m12": lambda: numeric_grid_workload(N=700, d=3, n=33, family="matern12", seed=6,
                                                 lengthscale=0.5, levels=9),
     "task4": lambda: task_workload(N_per_task=800, n_tasks=4, d_num=6, n_per_task=40, seed=2),

@@ -1,6 +1,6 @@
 """Round-2 additions that run LAST in the GPU suite (the driver runs it with ``-x``): the multi-target surrogate
 flow and the hybrid-space flow of tests/test_campaign_binding.py on the CUDA engine, under the reference's real
-``Campaign`` (``baseline/_ref``); skipped when the reference package is not on the box."""
+``Campaign`` (``oracle/_ref``); skipped when the reference package is not installed there."""
 from __future__ import annotations
 
 import numpy as np
@@ -10,7 +10,7 @@ from tests.test_campaign_binding import (REF, bb,  # noqa: F401
                                          test_multi_target_objectives_get_per_target_engine_surrogates)
 
 pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(REF is None, reason="the reference package (baybe) is not available on this box")]
+              pytest.mark.skipif(REF is None, reason="the reference package (baybe) is not installed under oracle/_ref")]
 
 
 def test_hybrid_campaign_recommends_a_batch_on_the_device(bb, cuda_device):  # noqa: F811
