@@ -9,9 +9,12 @@
 //   warpgroups 0, 1   rows 0-63 / 64-127 of the tile: assemble their K* rows chunk by chunk (64 training
 //                     points), write the fp16 hi/lo chunk to shared memory and issue the MMAs of that chunk;
 //                     the next chunk is assembled while those MMAs run.  Then moments and acquisition.
-//   warp 8            bulk-copy (TMA engine) producer of the L^-1 tiles
-// A warpgroup holds a 64 x 128 panel of V (64 fp32 registers per thread); a model with n_pad > 128 takes
-// several column panels per tile, each re-forming the K* chunks it needs (chunk c feeds sub-blocks s >= c).
+//   warpgroup 2       bulk-copy (TMA engine) producer of the L^-1 tiles (one elected thread; 24 registers, so
+//                     that a consumer thread can hold 240)
+// A warpgroup holds a 64 x 256 panel of V (128 fp32 registers per thread); a model with n_pad > 256 takes several
+// column panels per tile, each re-forming the K* chunks it needs (chunk c feeds sub-blocks s >= c).  The consumer
+// warpgroups are independent within a tile; on the tensor-core path they alternate their MMA issue (ping-pong), so
+// that one forms kernel values while the other's MMAs run.
 //
 // Reference path replaced: one chunk loop of botorch.optim.optimize_acqf_discrete
 // (baybe/recommenders/pure/bayesian/botorch/discrete.py) = acqf(X[chunk].unsqueeze(-2)) ->
@@ -117,13 +120,15 @@ __host__ __device__ __forceinline__ size_t rimg_tile(int c, int sb, int C) {
 // Gated pass: block until the copy stream has published the rows of `tile` (acquire at system scope: the data
 // was written by the copy engine before the counter).  Bounded: after ~2 s the status word is raised and the
 // kernel carries on (the host reports the pass as failed) -- a missing publication must not hang the GPU.
-// One thread per CTA polls and hands the value to the other consumer threads through shared memory; it is kept
-// in a register, since publications run far ahead of the tiles.  Called by all 256 consumer threads.
-__device__ __forceinline__ unsigned wait_rows(const FusedParams& p, volatile unsigned* cache_s, int tile, unsigned have) {
+// One thread per warpgroup polls and hands the value to the warpgroup's other threads through its word of shared
+// memory; it is kept in a register, since publications run far ahead of the tiles.  Called by the 128 threads of
+// warpgroup wg (t: thread within the warpgroup), so neither warpgroup waits for the other.
+__device__ __forceinline__ unsigned wait_rows(const FusedParams& p, volatile unsigned* cache_s, int tile, unsigned have,
+                                              int wg, int t) {
   const long long last = (long long)(tile + 1) * kTileM;
   const unsigned need = (unsigned)(last < p.N ? last : p.N);
   if (have >= need) return have;
-  if (threadIdx.x == 0) {
+  if (t == 0) {
     unsigned v;
     asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p.ready_rows) : "memory");
     if (v < need) {
@@ -141,11 +146,11 @@ __device__ __forceinline__ unsigned wait_rows(const FusedParams& p, volatile uns
         }
       }
     }
-    *cache_s = v;
+    cache_s[wg] = v;
   }
-  bar_compute();  // also orders the other threads' loads of the rows behind thread 0's acquire
-  const unsigned v = *cache_s;
-  bar_compute();  // the word may be rewritten by the next call
+  bar_wg(wg);  // also orders the other threads' loads of the rows behind thread 0's acquire
+  const unsigned v = cache_s[wg];
+  bar_wg(wg);  // the word may be rewritten by the next call
   return v;
 }
 
@@ -312,10 +317,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
     // =====================================================================================
     // consumer warpgroups
     // =====================================================================================
+    setmaxnreg_inc<kConsumerRegs>();
     const int wg = warp >> 2, t = tid & 127;
     const int mp = t & 31, g = t >> 5;           // assembly: rows m0 = 64 wg + mp and m0 + 32, octets g, g + 4
     const int m0 = 64 * wg + mp, m1 = m0 + 32;
-    const int row_e = tid & 127, sg = tid >> 7;  // epilogue: candidate row, sample group
+    const int row_e = 64 * wg + (t & 63), sg = t >> 6;  // epilogue: candidate row of the warpgroup, sample group
     const int ra = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // accumulator rows ra, ra + 8
     AsmSmem sm;
     sm.xt4 = s.xt4;
@@ -350,15 +356,19 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
     uint8_t* a2w = s.a2 + wg * 3 * tc_panel<K2>();
     if constexpr (!PRE)
       if ((int)blockIdx.x < p.num_tiles) {
-        if (sc.gated) rows_have = wait_rows(p, s.ready_cache, blockIdx.x, rows_have);
+        if (sc.gated) rows_have = wait_rows(p, s.ready_cache, blockIdx.x, rows_have, wg, t);
         if constexpr (!TC) stage_prefetch(sc, dq, (int64_t)blockIdx.x * kTileM, tid, regs);
       }
     long long best = kEmptyKey;
+    // TC: the warpgroups take turns issuing their MMAs (distances of a chunk, V of the previous one), so that one
+    // warpgroup forms its kernel values on the CUDA cores while the other's MMAs run.  Warpgroup 0 goes first.
+    if constexpr (TC)
+      if (wg == 1) mma_turn_pass(wg);
 
     int it = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
       const int64_t row0 = (int64_t)tile * kTileM;
-      if (tid == 0) trace_ev(p, it, 0);
+      if (t == 0) trace_ev(p, it, 100 * wg + kEvTileStart);
       float an0 = 0.f, an1 = 0.f;
       if constexpr (PRE) {
         if (p.task_col >= 0 && tid < kTileM) {  // task id of each candidate row (mean constant, prior variance)
@@ -384,8 +394,8 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
         an1 = cand_sqnorm(sm, m1);
       }
       float mean0 = 0.f, mean1 = 0.f, vq0 = 0.f, vq1 = 0.f;
-      for (int lo = 0; lo < C; lo += kPanelSB) {
-        const int hi = min(C, lo + kPanelSB);
+      for (int lo = 0; lo < C; lo += p.panel_sb) {
+        const int hi = min(C, lo + p.panel_sb);
         const bool last_panel = hi == C;  // covers every chunk: the mean is formed here
         float acc[kPanelSB][32];
 #pragma unroll
@@ -397,8 +407,14 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
           uint32_t ahi[4][4], alo[4][4];  // TC: the chunk's K* as the register A operand, one [4] per 16 k
           if constexpr (TC) {
             float dacc[32];
+            if (c == 0) {  // the panel's first turn: distances only (later turns start with the V MMAs below)
+              mma_turn_wait(wg);
+              if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnBegin);
+            }
             tc_distances<K2>(dacc, smem_u32(a2w), smem_u32(s.bt) + (uint32_t)c * tc_panel<K2>(),
                              (uint32_t)p.n_pad * K2 * 2u);
+            mma_turn_pass(wg);
+            if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnEnd);
             wg_wait<0>();  // also completes the previous chunk's V MMAs: release their L^-1 tiles
             if (t == 0)
               for (uint32_t q = 0; q < n_prev; ++q) mbar_arrive(&s.b_empty[(b_prev + q) % (uint32_t)p.stages_b]);
@@ -486,6 +502,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
             const uint32_t idx = bcount + q;
             mbar_wait(&s.b_full[idx % (uint32_t)p.stages_b], (idx / (uint32_t)p.stages_b) & 1u);
           }
+          if constexpr (TC) {  // this turn also issues the next chunk's distances (or ends after the last V MMAs)
+            mma_turn_wait(wg);
+            if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnBegin);
+          }
           wg_fence();
 #pragma unroll
           for (int j = 0; j < kPanelSB; ++j) {
@@ -510,6 +530,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
             }
           }
           wg_commit();
+          if constexpr (TC)
+            if (c == hi - 1) {
+              mma_turn_pass(wg);
+              if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnEnd);
+            }
           b_prev = bcount;
           n_prev = n_c;
           bcount += n_c;
@@ -526,7 +551,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
               vq1 = fmaf(acc[j][i + 2], acc[j][i + 2], fmaf(acc[j][i + 3], acc[j][i + 3], vq1));
             }
       }
-      if (tid == 0) trace_ev(p, it, 1);
+      if (t == 0) trace_ev(p, it, 100 * wg + kEvChunksDone);
       // |V|^2 per row: the four lanes of a quad hold the row's columns
       vq0 += __shfl_xor_sync(0xffffffffu, vq0, 1);
       vq0 += __shfl_xor_sync(0xffffffffu, vq0, 2);
@@ -552,12 +577,13 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
       // global loads of the next tile fly while the epilogue runs
       if constexpr (!PRE)
         if (tile + (int)gridDim.x < p.num_tiles) {
-          if (sc.gated) rows_have = wait_rows(p, s.ready_cache, tile + gridDim.x, rows_have);
+          if (sc.gated) rows_have = wait_rows(p, s.ready_cache, tile + gridDim.x, rows_have, wg, t);
           if constexpr (!TC) stage_prefetch(sc, dq, (int64_t)(tile + gridDim.x) * kTileM, tid, regs);
         }
-      bar_compute();
+      bar_wg(wg);
 
-      // ---- epilogue: moments in original units, acquisition, arg-max ----
+      // ---- epilogue of the warpgroup's 64 rows (two threads per row): moments in original units, acquisition,
+      // arg-max ----
       const int ct = s.cand_task[row_e];
       float msum = s.meanc[ct];
 #pragma unroll
@@ -601,7 +627,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
           mc_partial(p.acq, mu, var, s.z_s, p.S, sg, 2, s0, s1);
           *reinterpret_cast<float2*>(s.mc_part + (sg * kTileM + row_e) * 2) = make_float2(s0, s1);
         }
-        bar_compute();
+        bar_wg(wg);
         if (sg == 0) {
           float score;
           if (is_mc) {
@@ -631,18 +657,23 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
           }
         }
       }
-      bar_compute();  // shared partials are rewritten by the next tile
-      if (tid == 0) trace_ev(p, it, 2);
+      // the warpgroup's shared partials are rewritten by its next tile; the CUDA-core paths also stage the next
+      // tile's candidate rows (PRE: task ids) for both warpgroups at once
+      if constexpr (TC) bar_wg(wg);
+      else bar_compute();
+      if (t == 0) trace_ev(p, it, 100 * wg + kEvEpilogueDone);
     }
+    if constexpr (TC)
+      if (wg == 0) mma_turn_wait(wg);  // consumes warpgroup 1's hand-over after its last turn
 
     // ---- CTA-level arg-max ----
     if (p.best_key != nullptr && p.has_acq) {
-      if (sg == 0) {
+      if (sg == 0) {  // warps 0, 1 of each warpgroup
         for (int o = 16; o > 0; o >>= 1) {
           const long long other = __shfl_xor_sync(0xffffffffu, best, o);
           best = other > best ? other : best;
         }
-        if (lane == 0) s.best_red[warp] = best;
+        if (lane == 0) s.best_red[2 * wg + (warp & 1)] = best;
       }
       bar_compute();
       if (tid == 0) {
@@ -656,11 +687,12 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
     // producer: stream the fp16 image of L^-1 (B operand) through the TMA engine, in the order the
     // consumers read it: per tile, per column panel, per chunk c, sub-blocks sb >= c of the panel
     // =====================================================================================
-    if (elect_one()) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kWarpProducer && elect_one()) {
       uint32_t idx = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x)
-        for (int lo = 0; lo < C; lo += kPanelSB) {
-          const int hi = min(C, lo + kPanelSB);
+        for (int lo = 0; lo < C; lo += p.panel_sb) {
+          const int hi = min(C, lo + p.panel_sb);
           for (int c = 0; c < hi; ++c)
             for (int sb = c > lo ? c : lo; sb < hi; ++sb, ++idx) {
               const uint32_t st = idx % (uint32_t)p.stages_b, ph = (idx / (uint32_t)p.stages_b) & 1u;
@@ -928,13 +960,21 @@ static int launch_one(const FusedParams& p, int grid, size_t smem, cudaStream_t 
   return BB_OK;
 }
 
-// As many L^-1 stages as fit (at least one column panel's worth); 0 if even that does not fit.
+// The widest V panel (kPanelSB sub-blocks, else 2) whose ring fits, with as many L^-1 stages as fit; returns the
+// stage count, 0 if nothing fits.  A chunk's MMAs wait for all of its tiles at once -- min(n_chunks, panel width) --
+// so the ring needs at least that many stages (and no more: the warpgroups release a chunk's tiles before either
+// waits for the next chunk's).
 static int pick_stages(FusedParams& p, int max_smem) {
-  for (int st = kMaxStagesB; st >= kMinStagesB; --st) {
-    p.stages_b = st;
-    if (fused_smem_bytes(p) <= (size_t)max_smem) return st;
+  for (int w = kPanelSB; w >= 2; w -= 2) {
+    p.panel_sb = w;
+    const int need = p.n_chunks < w ? p.n_chunks : w;
+    for (int st = kMaxStagesB; st >= need && st >= 1; --st) {
+      p.stages_b = st;
+      if (fused_smem_bytes(p) <= (size_t)max_smem) return st;
+    }
   }
-  p.stages_b = kMinStagesB;
+  p.panel_sb = 2;
+  p.stages_b = 2;
   return 0;
 }
 
@@ -1132,6 +1172,7 @@ bool fused_gate_supported(const bb_model* m, const bb_acq_spec* acq, int32_t S) 
   memset(&p, 0, sizeof(p));
   p.n_pad = m->n_pad;
   p.d_pad = m->d_pad;
+  p.n_chunks = m->n_chunks;
   int sms = 0, max_smem = 0;
   if (device_limits(&sms, &max_smem) != BB_OK) return false;
   return pick_stages(p, max_smem) > 0;

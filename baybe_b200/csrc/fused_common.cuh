@@ -9,15 +9,22 @@
 
 namespace bb {
 
-// Two consumer warpgroups (rows 0-63 and 64-127 of a 128-candidate tile) and one bulk-copy producer warp.
+// Two consumer warpgroups (rows 0-63 and 64-127 of a 128-candidate tile) and one producer warpgroup, one elected
+// thread of which issues the bulk copies.
 constexpr int kConsumerWGs = 2;
 constexpr int kConsumerThreads = kConsumerWGs * 128;  // 256
-constexpr int kFusedThreads = kConsumerThreads + 32;  // + producer warp
+constexpr int kFusedThreads = kConsumerThreads + 128;  // + producer warpgroup
 constexpr int kWarpProducer = kConsumerThreads / 32;  // 8
-// 64-column sub-blocks of V held in registers at once (a 64 x 128 fp32 panel, 64 registers per thread): nine warps
-// spread over the four SM sub-partitions put three warps on one of them, which caps a thread at 168 registers
-constexpr int kPanelSB = 2;
-constexpr int kMinStagesB = kPanelSB, kMaxStagesB = 8;
+// Register split (setmaxnreg): 384 threads launch at 168 registers each; the producer warpgroup gives most of its
+// share back so that a consumer thread can hold 240: 128 x 24 + 256 x 240 = 64,512 of the SM's 65,536.
+constexpr int kProducerRegs = 24, kConsumerRegs = 240;
+// 64-column sub-blocks of V held in registers at once: up to a 64 x 256 fp32 panel, 128 registers per consumer
+// thread.  A model with n_pad <= 256 runs one panel, so every K* chunk is formed once per tile.  A launch uses
+// kPanelSB or, where shared memory cannot hold the L^-1 tiles one chunk of such a panel needs, 2 (FusedParams).
+constexpr int kPanelSB = 4;
+constexpr int kMaxStagesB = 8;
+// k_kmat_wg (wide.cu): two consumer warpgroups and one bulk-copy producer warp
+constexpr int kWideThreads = kConsumerThreads + 32;
 constexpr uint32_t kABytes = 16384;      // one warpgroup's K* chunk: [hi 8 KB | lo 8 KB], 64 rows x 64 fp16, SW128
 constexpr uint32_t kStageBBytes = 16384; // one L^-1 tile: [hi 8 KB | lo 8 KB], 64 rows x 64 fp16, SW128
 constexpr int kMaxTasks = 16;
@@ -38,6 +45,7 @@ struct FusedParams {
   float y_mean, y_std, prior_scale, inv_r_scale2;
   int scaled;  // task kernel or output scale present
   int stages_b;  // L^-1 tiles in flight
+  int panel_sb;  // V sub-blocks per column panel (kPanelSB or 2), chosen with stages_b by pick_stages
   // tensor-core distances (tc = 1): augmented training image [sb (-2b) | Q1 | |b|^2 Q] as fp16 hi/mid/lo panels of
   // n_pad rows x 32 k (SW64); candidate rows become [sa a | |a|^2 P | P1], so the GEMM yields t / ts_g directly
   int tc;
@@ -75,6 +83,10 @@ struct StreamGate {
   int layout;  // kLayoutCodes4 / kLayoutCodes8 / BB_ROW_MAJOR_F32
 };
 
+// Trace events of k_fused, recorded by thread 0 of consumer warpgroup wg as 100 wg + id: tile start, end of the chunk
+// loop, end of the tile's epilogue, and the start (turn granted) and end (MMAs issued) of each MMA turn.
+constexpr int kEvTileStart = 0, kEvChunksDone = 1, kEvEpilogueDone = 2, kEvTurnBegin = 10, kEvTurnEnd = 11;
+
 // test-only: (event id, SM clock) pairs of CTA 0 for a few tiles, to reconstruct the pipeline timeline
 __device__ __forceinline__ void trace_ev(const FusedParams& p, int it, int ev) {
   if (p.trace != nullptr && blockIdx.x == 0 && it >= 6 && it < 9) {
@@ -89,6 +101,16 @@ __device__ __forceinline__ void trace_ev(const FusedParams& p, int it, int ev) {
 
 // the 256 consumer threads
 __device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Ping-pong of the two consumer warpgroups' MMA issue (named barriers 4 and 5 over both warpgroups): warpgroup wg
+// waits for its turn on barrier 4 + wg and hands the turn to the other one by arriving on the other's barrier.
+__device__ __forceinline__ void mma_turn_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(4 + wg) : "memory"); }
+__device__ __forceinline__ void mma_turn_pass(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(5 - wg) : "memory"); }
+
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 
 // Wait used by the single-lane helper warps: mbarrier.try_wait with a suspend-time hint parks the

@@ -138,7 +138,7 @@ __device__ __forceinline__ uint32_t wide_load_bits16(const WideParams& p, int64_
 }
 
 template <int FAMILY, bool BITS>
-__global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_wg(const WideParams p) {
+__global__ void __launch_bounds__(kWideThreads, 1) k_kmat_wg(const WideParams p) {
   constexpr int PA = BITS ? 1 : 3;
   constexpr int PB = BITS ? 2 : 3;  // W of the bit-linear form has <= 2 distinct values per column: hi+mid (2^-22) suffices
   constexpr uint32_t kStageA = PA * kWPanelA;
@@ -156,11 +156,11 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_kmat_wg(const WideParams p
     }
     fence_mbar_init();
   }
-  for (int e = tid; e < p.n_pad; e += kFusedThreads) {
+  for (int e = tid; e < p.n_pad; e += kWideThreads) {
     s.wnorm_s[e] = __ldg(p.wnorm + e);
     s.ttask[e] = __ldg(p.train_task + e);
   }
-  for (int e = tid; e < p.n_tasks * p.n_tasks; e += kFusedThreads) s.tcov[e] = __ldg(p.task_covar + e);
+  for (int e = tid; e < p.n_tasks * p.n_tasks; e += kWideThreads) s.tcov[e] = __ldg(p.task_covar + e);
   __syncthreads();
 
   if (warp < kWarpProducer) {
@@ -386,7 +386,7 @@ static int launch_kmat_one(WideParams& p, int sms, int max_smem, cudaStream_t st
   BB_CHECK_SUPPORTED(smem <= (size_t)max_smem, "wide kernel-matrix path: shared-memory budget exceeded (%zu bytes)", smem);
   BB_SMEM_OPTIN_ONCE((k_kmat_wg<FAMILY, BITS>));
   const int grid = p.num_items < sms ? p.num_items : sms;
-  k_kmat_wg<FAMILY, BITS><<<grid, kFusedThreads, smem, stream>>>(p);
+  k_kmat_wg<FAMILY, BITS><<<grid, kWideThreads, smem, stream>>>(p);
   BB_LAUNCH_CHECK();
   return BB_OK;
 }
