@@ -9,7 +9,7 @@ import ctypes as C
 from pathlib import Path
 
 LIB_PATH = Path(__file__).resolve().parent / "_C" / "libbaybe_b200.so"
-ABI_VERSION = 2
+ABI_VERSION = 3
 
 # enums (mirror include/baybe_b200.h)
 KERNEL_FAMILY = {"matern12": 0, "matern32": 1, "matern52": 2, "rbf": 3}
@@ -51,19 +51,16 @@ class Model(C.Structure):
         ("d_train_sq", C.c_void_p), ("d_alpha", C.c_void_p), ("d_train_task", C.c_void_p),
         ("d_task_covar", C.c_void_p), ("d_mean_const", C.c_void_p), ("d_rimg", C.c_void_p),
         ("d_linv", C.c_void_p), ("d_alpha64", C.c_void_p), ("d_xn64", C.c_void_p),
-        ("d_linv32", C.c_void_p), ("d_bimg", C.c_void_p),
+        ("d_linv32", C.c_void_p),
         ("dist_scale_a", C.c_float), ("dist_scale_b", C.c_float),
-        ("dist_k", C.c_int32), ("pad_", C.c_int32), ("d_rimg2", C.c_void_p),
         ("wide", C.c_int32), ("d_wide", C.c_int32), ("d_wimg", C.c_void_p),
         ("d_wimg_bits", C.c_void_p), ("d_wnorm_bits", C.c_void_p), ("d_wide_ws", C.c_void_p),
-        ("wide_ws_rows", C.c_int64), ("dist_scale_w", C.c_float), ("pad2_", C.c_int32),
-        ("d_rimg4", C.c_void_p), ("d_rimg2g", C.c_void_p),
+        ("wide_ws_rows", C.c_int64), ("dist_scale_w", C.c_float), ("pad_", C.c_int32),
         ("d_pend_img", C.c_void_p), ("d_pend_norm", C.c_void_p), ("d_pend_task", C.c_void_p),
         ("d_kpend_ws", C.c_void_p), ("dist_scale_p", C.c_float), ("dist_scale_wp", C.c_float),
-        ("d_mc_table", C.c_void_p), ("d_wide_vacc", C.c_void_p),
-        ("d_timg_l", C.c_void_p), ("d_timg_b", C.c_void_p), ("d_ts_alpha", C.c_void_p),
+        ("d_mc_table", C.c_void_p), ("d_timg_b", C.c_void_p), ("dist_k", C.c_int32),
         ("ts_sa", C.c_float), ("ts_aug_sq", C.c_float), ("ts_aug_one", C.c_float), ("ts_g", C.c_float),
-        ("ts_kscale", C.c_float), ("pad3_", C.c_int32),
+        ("ts_kscale", C.c_float),
     ]
 
 

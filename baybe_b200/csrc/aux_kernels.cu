@@ -33,51 +33,72 @@ struct AuxParams {
   float *mu, *var;
 };
 
+// Shared memory of k_kmat and k_cross: the assembly core's buffers, then each kernel's own.
 struct AuxSmem {
-  AsmSmem sm;
-  StageCtx sc;
-  float* extra;
+  float4 *xt4, *a_s;
+  float *tsq, *tcov, *cscale, *cshift;
+  int32_t *ttask, *cand_task;
+  float* ks;  // k_kmat: [128][kKsStride] staged output rows
+  float *cross_s, *psq;  // k_cross: [128][32] partial sums, [32] squared norms of the pending rows
+  float4* pxt4;          // k_cross: [dq][32] pending rows, pair-interleaved like the training rows
+  int32_t* ptask;        // k_cross: [32]
 };
 
-__device__ __forceinline__ AuxSmem aux_carve(uint8_t* base, const AuxParams& p, int tid,
-                                             int nthreads) {
-  AuxSmem r;
+static __host__ __device__ SmemCarver carve_asm(uint8_t* base, const AuxParams& p, AuxSmem& s) {
+  SmemCarver c{base};
+  s.xt4 = c.take<float4>((size_t)p.n_pad * p.d_pad * 4);
+  s.tsq = c.take<float>((size_t)p.n_pad * 4);
+  s.ttask = c.take<int32_t>((size_t)p.n_pad * 4);
+  s.a_s = c.take<float4>((size_t)kTileM * p.d_pad * 8);  // duplicated candidate values
+  s.tcov = c.take<float>(kMaxTasks * kMaxTasks * 4);
+  s.cand_task = c.take<int32_t>(kTileM * 4);
+  s.cscale = c.take<float>((size_t)p.d_pad * 4);
+  s.cshift = c.take<float>((size_t)p.d_pad * 4);
+  return c;
+}
+
+static __host__ __device__ size_t carve_kmat(uint8_t* base, const AuxParams& p, AuxSmem& s) {
+  SmemCarver c = carve_asm(base, p, s);
+  s.ks = c.take<float>((size_t)kTileM * kKsStride * 4);
+  return c.bytes;
+}
+
+static __host__ __device__ size_t carve_cross(uint8_t* base, const AuxParams& p, AuxSmem& s) {
+  SmemCarver c = carve_asm(base, p, s);
+  s.cross_s = c.take<float>(kTileM * 32 * 4);
+  s.pxt4 = c.take<float4>((size_t)32 * p.d_pad * 4);
+  s.psq = c.take<float>(32 * 4);
+  s.ptask = c.take<int32_t>(32 * 4);
+  return c.bytes;
+}
+
+// How the assembly core (sm) and the candidate staging (sc) see the shared buffers.
+struct AuxCore {
+  AsmSmem sm;
+  StageCtx sc;
+};
+
+// Loads the model data of the assembly core into shared memory.
+__device__ __forceinline__ AuxCore aux_setup(const AuxSmem& s, const AuxParams& p, int tid, int nthreads) {
   const int dq = p.d_pad >> 2;
-  uint8_t* cur = base;
-  float4* xt4 = reinterpret_cast<float4*>(cur);
-  cur += (size_t)p.n_pad * p.d_pad * 4;
-  float* tsq = reinterpret_cast<float*>(cur);
-  cur += p.n_pad * 4;
-  int32_t* ttask = reinterpret_cast<int32_t*>(cur);
-  cur += p.n_pad * 4;
-  float4* a_s = reinterpret_cast<float4*>(cur);
-  cur += (size_t)kTileM * p.d_pad * 8;  // duplicated candidate values
-  float* tcov = reinterpret_cast<float*>(cur);
-  cur += 256 * 4;
-  int32_t* cand_task = reinterpret_cast<int32_t*>(cur);
-  cur += kTileM * 4;
-  float* cscale_s = reinterpret_cast<float*>(cur);
-  cur += ((p.d_pad * 4 + 15) / 16) * 16;
-  float* cshift_s = reinterpret_cast<float*>(cur);
-  cur += ((p.d_pad * 4 + 15) / 16) * 16;
-  r.extra = reinterpret_cast<float*>(cur);
-  load_train_rows(xt4, p.train_m2, p.n_pad, dq, tid, nthreads);
+  load_train_rows(s.xt4, p.train_m2, p.n_pad, dq, tid, nthreads);
   for (int e = tid; e < p.d_pad; e += nthreads) {
-    cscale_s[e] = __ldg(p.cand_scale + e);
-    cshift_s[e] = __ldg(p.cand_shift + e);
+    s.cscale[e] = __ldg(p.cand_scale + e);
+    s.cshift[e] = __ldg(p.cand_shift + e);
   }
   for (int e = tid; e < p.n_pad; e += nthreads) {
-    tsq[e] = __ldg(p.train_sq + e);
-    ttask[e] = __ldg(p.train_task + e);
+    s.tsq[e] = __ldg(p.train_sq + e);
+    s.ttask[e] = __ldg(p.train_task + e);
   }
-  for (int e = tid; e < p.n_tasks * p.n_tasks; e += nthreads) tcov[e] = __ldg(p.task_covar + e);
-  for (int e = tid; e < kTileM; e += nthreads) cand_task[e] = 0;
-  r.sm.xt4 = xt4;
-  r.sm.tsq = tsq;
-  r.sm.ttask = ttask;
-  r.sm.tcov = tcov;
-  r.sm.a_s = a_s;
-  r.sm.cand_task = cand_task;
+  for (int e = tid; e < p.n_tasks * p.n_tasks; e += nthreads) s.tcov[e] = __ldg(p.task_covar + e);
+  for (int e = tid; e < kTileM; e += nthreads) s.cand_task[e] = 0;
+  AuxCore r;
+  r.sm.xt4 = s.xt4;
+  r.sm.tsq = s.tsq;
+  r.sm.ttask = s.ttask;
+  r.sm.tcov = s.tcov;
+  r.sm.a_s = s.a_s;
+  r.sm.cand_task = s.cand_task;
   r.sm.dq = dq;
   r.sm.np = p.n_pad;
   r.sm.T = p.n_tasks;
@@ -88,18 +109,13 @@ __device__ __forceinline__ AuxSmem aux_carve(uint8_t* base, const AuxParams& p, 
   r.sc.ldx = p.ldx;
   r.sc.d = p.d;
   r.sc.task_col = p.task_col;
-  r.sc.cscale = cscale_s;
-  r.sc.cshift = cshift_s;
+  r.sc.cscale = s.cscale;
+  r.sc.cshift = s.cshift;
   r.sc.groups = nthreads / kTileM;
   r.sc.gated = false;
   r.sc.code_table = nullptr;
   r.sc.code_table_ld = 0;
   return r;
-}
-
-static size_t aux_base_bytes(const AuxParams& p) {
-  return (size_t)p.n_pad * p.d_pad * 4 + (size_t)p.n_pad * 8 + (size_t)kTileM * p.d_pad * 8 +
-         256 * 4 + kTileM * 4 + 2 * (size_t)(((p.d_pad * 4 + 15) / 16) * 16);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -110,23 +126,27 @@ template <int FAMILY>
 __global__ void __launch_bounds__(kAuxThreads, 1) k_kmat(const AuxParams p) {
   extern __shared__ __align__(16) uint8_t smem_aux[];
   const int tid = threadIdx.x;
-  AuxSmem as = aux_carve(smem_aux, p, tid, kAuxThreads);
-  float* ks = as.extra;  // [128][kKsStride]
+  AuxSmem s;
+  carve_kmat(smem_aux, p, s);
+  const AuxCore core = aux_setup(s, p, tid, kAuxThreads);
+  const AsmSmem& sm = core.sm;
+  const StageCtx& sc = core.sc;
+  float* ks = s.ks;
   __syncthreads();
   const int mp = tid & 63, g = tid >> 6;
   const bool vec_ok = ((reinterpret_cast<uintptr_t>(p.kout) & 15) == 0) && ((p.ldk & 3) == 0);
   StageRegs regs;
-  if ((int)blockIdx.x < p.num_tiles) stage_prefetch(as.sc, as.sm.dq, (int64_t)blockIdx.x * kTileM, tid, regs);
+  if ((int)blockIdx.x < p.num_tiles) stage_prefetch(sc, sm.dq, (int64_t)blockIdx.x * kTileM, tid, regs);
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
     const int64_t row0 = (int64_t)tile * kTileM;
-    stage_commit(as.sc, as.sm.a_s, as.sm.cand_task, as.sm.T, as.sm.dq, row0, tid, regs);
+    stage_commit(sc, sm.a_s, sm.cand_task, sm.T, sm.dq, row0, tid, regs);
     __syncthreads();
     if (tile + (int)gridDim.x < p.num_tiles)
-      stage_prefetch(as.sc, as.sm.dq, (int64_t)(tile + gridDim.x) * kTileM, tid, regs);
-    const float an0 = cand_sqnorm(as.sm, mp), an1 = cand_sqnorm(as.sm, mp + 64);
+      stage_prefetch(sc, sm.dq, (int64_t)(tile + gridDim.x) * kTileM, tid, regs);
+    const float an0 = cand_sqnorm(sm, mp), an1 = cand_sqnorm(sm, mp + 64);
     for (int c = 0; c < p.n_chunks; ++c) {
       float k0[8], k1[8];
-      assemble_2x8<FAMILY>(as.sm, mp, mp + 64, an0, an1, c * kChunk + g * 8, k0, k1);
+      assemble_2x8<FAMILY>(sm, mp, mp + 64, an0, an1, c * kChunk + g * 8, k0, k1);
       float4* d0 = reinterpret_cast<float4*>(ks + mp * kKsStride + g * 8);
       float4* d1 = reinterpret_cast<float4*>(ks + (mp + 64) * kKsStride + g * 8);
       d0[0] = make_float4(k0[0], k0[1], k0[2], k0[3]);
@@ -165,12 +185,15 @@ template <int FAMILY>
 __global__ void __launch_bounds__(256, 1) k_cross(const AuxParams p) {
   extern __shared__ __align__(16) uint8_t smem_aux[];
   const int tid = threadIdx.x;
-  AuxSmem as = aux_carve(smem_aux, p, tid, 256);
-  const int dq = p.d_pad >> 2;
-  float* cross_s = as.extra;                               // [128][32]
-  float4* pxt4 = reinterpret_cast<float4*>(cross_s + kTileM * 32);  // [dq][32], pair-interleaved
-  float* psq = reinterpret_cast<float*>(pxt4 + 32 * dq);   // [32]
-  int32_t* ptask = reinterpret_cast<int32_t*>(psq + 32);   // [32]
+  AuxSmem s;
+  carve_cross(smem_aux, p, s);
+  const AuxCore core = aux_setup(s, p, tid, 256);
+  const AsmSmem& sm = core.sm;
+  const StageCtx& sc = core.sc;
+  float* cross_s = s.cross_s;
+  float4* pxt4 = s.pxt4;
+  float* psq = s.psq;
+  int32_t* ptask = s.ptask;
   // scaled pending rows, laid out like the training rows (-2 b, quad-major) + squared norms
   for (int e = tid; e < 32 * p.d_pad; e += 256) {
     int pp = e / p.d_pad, j = e - pp * p.d_pad;
@@ -198,12 +221,12 @@ __global__ void __launch_bounds__(256, 1) k_cross(const AuxParams p) {
     const int64_t row0 = (int64_t)tile * kTileM;
     {
       StageRegs regs;
-      stage_prefetch(as.sc, as.sm.dq, row0, tid, regs);
-      stage_commit(as.sc, as.sm.a_s, as.sm.cand_task, as.sm.T, as.sm.dq, row0, tid, regs);
+      stage_prefetch(sc, sm.dq, row0, tid, regs);
+      stage_commit(sc, sm.a_s, sm.cand_task, sm.T, sm.dq, row0, tid, regs);
     }
     for (int e = tid; e < kTileM * 32; e += 256) cross_s[e] = 0.f;
     __syncthreads();
-    const float an0 = cand_sqnorm(as.sm, mp), an1 = cand_sqnorm(as.sm, mp + 64);
+    const float an0 = cand_sqnorm(sm, mp), an1 = cand_sqnorm(sm, mp + 64);
     float acc0[BB_MAX_PENDING + 1], acc1[BB_MAX_PENDING + 1];
 #pragma unroll
     for (int pp = 0; pp <= BB_MAX_PENDING; ++pp) {
@@ -213,7 +236,7 @@ __global__ void __launch_bounds__(256, 1) k_cross(const AuxParams p) {
     const int octets = p.n_pad >> 3;
     for (int o = g; o < octets; o += 4) {
       float k0[8], k1[8];
-      assemble_2x8<FAMILY>(as.sm, mp, mp + 64, an0, an1, o * 8, k0, k1);
+      assemble_2x8<FAMILY>(sm, mp, mp + 64, an0, an1, o * 8, k0, k1);
 #pragma unroll
       for (int pp = 0; pp <= BB_MAX_PENDING; ++pp) {
         if (pp < p.P) {
@@ -228,7 +251,7 @@ __global__ void __launch_bounds__(256, 1) k_cross(const AuxParams p) {
     }
     // prior term k(x*, p): group g handles pending octet g (P <= 32)
     {
-      AsmSmem ps = as.sm;
+      AsmSmem ps = sm;
       ps.xt4 = pxt4;
       ps.np = 32;
       ps.tsq = psq;
@@ -273,27 +296,33 @@ __global__ void __launch_bounds__(256, 1) k_cross(const AuxParams p) {
 // test-only SIMT posterior: 32 candidates per CTA, direct-difference distances, fp32 FMA
 // contraction with the dense fp32 copy of L^-1.
 // ------------------------------------------------------------------------------------------
+struct SimtSmem {
+  float *ks, *xa, *red;
+  int* ct;
+};
+
+static __host__ __device__ size_t carve_simt(uint8_t* base, const AuxParams& p, SimtSmem& s) {
+  SmemCarver c{base};
+  s.ks = c.take<float>((size_t)32 * (p.n_pad + 1) * 4);  // [32][n_pad+1]
+  s.xa = c.take<float>((size_t)32 * p.d_pad * 4);        // [32][d_pad]
+  s.ct = c.take<int>(32 * 4);                            // [32]
+  s.red = c.take<float>(8 * 32 * 2 * 4);                 // [8][32][2]
+  return c.bytes;
+}
+
 template <int FAMILY>
 __global__ void __launch_bounds__(256, 1) k_simt(const AuxParams p) {
   extern __shared__ __align__(16) uint8_t smem_aux[];
   const int tid = threadIdx.x;
-  float* ks = reinterpret_cast<float*>(smem_aux);  // [32][n_pad+1]
-  float* xa = ks + 32 * (p.n_pad + 1);             // [32][d_pad]
-  int* ct = reinterpret_cast<int*>(xa + 32 * p.d_pad);  // [32]
-  float* red = reinterpret_cast<float*>(ct + 32);  // [8][32][2]
+  SimtSmem s;
+  carve_simt(smem_aux, p, s);
+  float *ks = s.ks, *xa = s.xa, *red = s.red;
+  int* ct = s.ct;
   const int64_t row0 = (int64_t)blockIdx.x * 32;
   for (int e = tid; e < 32 * p.d_pad; e += 256) {
     int r = e / p.d_pad, j = e - r * p.d_pad;
     int64_t row = row0 + r;
-    float xv = 0.f;
-    if (j < p.d && row < p.N) {
-      switch (p.layout) {
-        case BB_ROW_MAJOR_F32: xv = load_x<BB_ROW_MAJOR_F32>(p.x, row, j, p.ldx); break;
-        case BB_COL_MAJOR_F32: xv = load_x<BB_COL_MAJOR_F32>(p.x, row, j, p.ldx); break;
-        case BB_ROW_MAJOR_F64: xv = load_x<BB_ROW_MAJOR_F64>(p.x, row, j, p.ldx); break;
-        default: xv = load_x<BB_COL_MAJOR_F64>(p.x, row, j, p.ldx); break;
-      }
-    }
+    const float xv = (j < p.d && row < p.N) ? load_x_any(p.x, p.layout, row, j, p.ldx) : 0.f;
     xa[e] = (j < p.d) ? fmaf(xv, __ldg(p.cand_scale + j), __ldg(p.cand_shift + j)) : 0.f;
     if (j == p.task_col) ct[r] = min(max(__float2int_rn(xv), 0), p.n_tasks - 1);
   }
@@ -339,16 +368,13 @@ __global__ void __launch_bounds__(256, 1) k_simt(const AuxParams p) {
   }
 }
 
+// Candidate checks (check_candidates) and the model fields of AuxParams.  These kernels read the four float layouts
+// only: bit-packed rows are rejected as an invalid layout even for a wide-feature model.
 static int fill_params(AuxParams& p, const bb_model* m, const void* d_x, int32_t layout, int64_t N,
                        int64_t ldx) {
-  BB_CHECK_ARG(m && m->abi_version == BB_ABI_VERSION, "model struct missing or ABI mismatch");
-  BB_CHECK_ARG(d_x != nullptr || N == 0, "candidate pointer is null");
-  BB_CHECK_ARG(layout >= 0 && layout <= 3, "unknown candidate layout %d", layout);
-  BB_CHECK_ARG(N >= 0, "negative candidate count");
-  const bool col_major = (layout == BB_COL_MAJOR_F32 || layout == BB_COL_MAJOR_F64);
-  BB_CHECK_ARG(col_major ? ldx >= N : ldx >= m->d, "leading dimension %lld too small",
-               (long long)ldx);
-  BB_CHECK_SUPPORTED(m->n_tasks <= 16, "at most 16 tasks supported");
+  BB_CHECK_ARG(layout != BB_BITS_U8, "bit-packed candidates are not read by this entry point");
+  const int rc = check_candidates(m, d_x, layout, N, ldx);
+  if (rc != BB_OK) return rc;
   memset(&p, 0, sizeof(p));
   p.x = d_x;
   p.layout = layout;
@@ -368,7 +394,7 @@ static int fill_params(AuxParams& p, const bb_model* m, const void* d_x, int32_t
   p.n_chunks = m->n_chunks;
   p.task_col = m->task_col;
   p.n_tasks = m->n_tasks;
-  p.scaled = (m->task_col >= 0 || m->prior_scale != 1.0f) ? 1 : 0;
+  p.scaled = model_scaled(m) ? 1 : 0;
   p.y_std = m->y_std;
   p.y_mean = m->y_mean;
   p.alpha = m->d_alpha;
@@ -376,35 +402,6 @@ static int fill_params(AuxParams& p, const bb_model* m, const void* d_x, int32_t
   p.linv32 = m->d_linv32;
   return BB_OK;
 }
-
-#define BB_DISPATCH_FAMILY(KERNEL, family, grid, block, smem, stream, params)                   \
-  do {                                                                                          \
-    switch (family) {                                                                           \
-      case BB_KERNEL_MATERN12:                                                                  \
-        BB_CUDA(cudaFuncSetAttribute(KERNEL<BB_KERNEL_MATERN12>,                                \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem))); \
-        KERNEL<BB_KERNEL_MATERN12><<<grid, block, smem, stream>>>(params);                      \
-        break;                                                                                  \
-      case BB_KERNEL_MATERN32:                                                                  \
-        BB_CUDA(cudaFuncSetAttribute(KERNEL<BB_KERNEL_MATERN32>,                                \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem))); \
-        KERNEL<BB_KERNEL_MATERN32><<<grid, block, smem, stream>>>(params);                      \
-        break;                                                                                  \
-      case BB_KERNEL_MATERN52:                                                                  \
-        BB_CUDA(cudaFuncSetAttribute(KERNEL<BB_KERNEL_MATERN52>,                                \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem))); \
-        KERNEL<BB_KERNEL_MATERN52><<<grid, block, smem, stream>>>(params);                      \
-        break;                                                                                  \
-      default:                                                                                  \
-        BB_CUDA(cudaFuncSetAttribute(KERNEL<BB_KERNEL_RBF>,                                     \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem))); \
-        KERNEL<BB_KERNEL_RBF><<<grid, block, smem, stream>>>(params);                           \
-        break;                                                                                  \
-    }                                                                                           \
-    BB_LAUNCH_CHECK();                                                                          \
-  } while (0)
-
-static int device_limits(int& sms, int& max_smem) { return device_limits(&sms, &max_smem); }  // cached (common.cuh)
 
 int launch_cross(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx,
                  const float* d_pend_x, const float* d_pend_beta, int32_t P, float* d_cross,
@@ -420,13 +417,18 @@ int launch_cross(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
   p.P = P;
   p.cross = d_cross;
   int sms, max_smem;
-  rc = device_limits(sms, max_smem);
+  rc = device_limits(&sms, &max_smem);
   if (rc != BB_OK) return rc;
-  size_t smem = aux_base_bytes(p) + kTileM * 32 * 4 + 32 * p.d_pad * 4 + 32 * 8;
+  AuxSmem unused;
+  const size_t smem = carve_cross(nullptr, p, unused);
   BB_CHECK_SUPPORTED(smem <= (size_t)max_smem, "shared-memory budget exceeded (%zu bytes)", smem);
-  int grid = p.num_tiles < sms ? p.num_tiles : sms;
-  BB_DISPATCH_FAMILY(k_cross, m->family, grid, 256, smem, stream, p);
-  return BB_OK;
+  const int grid = p.num_tiles < sms ? p.num_tiles : sms;
+  return dispatch_family<true>(m->family, [&](auto fam) {
+    BB_SMEM_OPTIN_ONCE(k_cross<decltype(fam)::value>);
+    k_cross<decltype(fam)::value><<<grid, 256, smem, stream>>>(p);
+    BB_LAUNCH_CHECK();
+    return BB_OK;
+  });
 }
 
 }  // namespace bb
@@ -436,24 +438,14 @@ using namespace bb;
 extern "C" int bb_kernel_matrix(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
                                 int64_t ldx, float* d_k, int64_t ldk, void* stream_) {
   cudaStream_t stream = (cudaStream_t)stream_;
-  if (m && m->abi_version == BB_ABI_VERSION && m->wide) {  // K-chunked tensor-core path (wide.cu)
-    BB_CHECK_ARG(d_x != nullptr || N == 0, "candidate pointer is null");
-    BB_CHECK_ARG(layout >= 0 && layout <= BB_BITS_U8, "unknown candidate layout %d", layout);
-    BB_CHECK_ARG(N >= 0, "negative candidate count");
-    const bool cm = (layout == BB_COL_MAJOR_F32 || layout == BB_COL_MAJOR_F64);
-    BB_CHECK_ARG(layout == BB_BITS_U8 ? ldx >= (m->d + 7) / 8 : (cm ? ldx >= N : ldx >= m->d),
-                 "leading dimension %lld too small", (long long)ldx);
-    BB_CHECK_ARG(d_k != nullptr || N == 0, "bb_kernel_matrix: output pointer is null");
-    BB_CHECK_ARG(ldk >= m->n, "bb_kernel_matrix: ldk=%lld smaller than n=%d", (long long)ldk, m->n);
-    if (N == 0) return BB_OK;
-    return launch_kmat_wide(m, d_x, layout, N, ldx, d_k, ldk, N, m->n, stream);
-  }
+  const bool wide = m && m->abi_version == BB_ABI_VERSION && m->wide;  // K-chunked tensor-core path (wide.cu)
   AuxParams p;
-  int rc = fill_params(p, m, d_x, layout, N, ldx);
+  int rc = wide ? check_candidates(m, d_x, layout, N, ldx) : fill_params(p, m, d_x, layout, N, ldx);
   if (rc != BB_OK) return rc;
   BB_CHECK_ARG(d_k != nullptr || N == 0, "bb_kernel_matrix: output pointer is null");
   BB_CHECK_ARG(ldk >= m->n, "bb_kernel_matrix: ldk=%lld smaller than n=%d", (long long)ldk, m->n);
   if (N == 0) return BB_OK;
+  if (wide) return launch_kmat_wide(m, d_x, layout, N, ldx, d_k, ldk, N, m->n, stream);
   {  // tensor-core distances + TMA tensor stores (fused.cu: k_kmat_tma) where the model and the output allow
     bool handled = false;
     rc = try_kmat_tma(m, d_x, layout, N, ldx, d_k, ldk, stream, &handled);
@@ -462,15 +454,20 @@ extern "C" int bb_kernel_matrix(const bb_model* m, const void* d_x, int32_t layo
   p.kout = d_k;
   p.ldk = ldk;
   int sms, max_smem;
-  rc = device_limits(sms, max_smem);
+  rc = device_limits(&sms, &max_smem);
   if (rc != BB_OK) return rc;
-  size_t smem = aux_base_bytes(p) + (size_t)kTileM * kKsStride * 4;
+  AuxSmem unused;
+  const size_t smem = carve_kmat(nullptr, p, unused);
   BB_CHECK_SUPPORTED(smem <= (size_t)max_smem, "shared-memory budget exceeded (%zu bytes)", smem);
   // several waves of small tiles balance better than one persistent CTA per SM for this
   // store-bound kernel: 2 CTAs per SM worth of grid, grid-stride over the tiles.
-  int grid = p.num_tiles < 2 * sms ? p.num_tiles : 2 * sms;
-  BB_DISPATCH_FAMILY(k_kmat, m->family, grid, kAuxThreads, smem, stream, p);
-  return BB_OK;
+  const int grid = p.num_tiles < 2 * sms ? p.num_tiles : 2 * sms;
+  return dispatch_family<true>(m->family, [&](auto fam) {
+    BB_SMEM_OPTIN_ONCE(k_kmat<decltype(fam)::value>);
+    k_kmat<decltype(fam)::value><<<grid, kAuxThreads, smem, stream>>>(p);
+    BB_LAUNCH_CHECK();
+    return BB_OK;
+  });
 }
 
 extern "C" int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout,
@@ -484,8 +481,13 @@ extern "C" int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32
   BB_CHECK_ARG(d_mu && d_var, "bb_debug_posterior_simt: output pointers are null");
   p.mu = d_mu;
   p.var = d_var;
-  size_t smem = (size_t)32 * (p.n_pad + 1) * 4 + 32 * p.d_pad * 4 + 32 * 4 + 8 * 32 * 2 * 4;
-  int grid = (int)((N + 31) / 32);
-  BB_DISPATCH_FAMILY(k_simt, m->family, grid, 256, smem, stream, p);
-  return BB_OK;
+  SimtSmem unused;
+  const size_t smem = carve_simt(nullptr, p, unused);
+  const int grid = (int)((N + 31) / 32);
+  return dispatch_family<true>(m->family, [&](auto fam) {
+    BB_SMEM_OPTIN_ONCE(k_simt<decltype(fam)::value>);
+    k_simt<decltype(fam)::value><<<grid, 256, smem, stream>>>(p);
+    BB_LAUNCH_CHECK();
+    return BB_OK;
+  });
 }

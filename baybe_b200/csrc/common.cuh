@@ -1,7 +1,8 @@
-// common.cuh -- shared helpers: error plumbing, PTX wrappers for sm_90a (mbarrier, bulk copy
-// (TMA engine), warpgroup MMA), fp16 split, packed arg-max keys.
+// common.cuh -- shared helpers: error plumbing, candidate loads, shared-memory carving, PTX wrappers for sm_90a
+// (mbarrier, bulk copy (TMA engine), warpgroup MMA), fp16 split, packed arg-max keys.
 #pragma once
 
+#include <assert.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -107,6 +108,38 @@ __device__ __forceinline__ float load_x(const void* __restrict__ x, int64_t row,
     return (float)__ldg(reinterpret_cast<const double*>(x) + (int64_t)col * ld + row);
   }
 }
+
+// load_x with the layout known only at run time
+__device__ __forceinline__ float load_x_any(const void* __restrict__ x, int layout, int64_t row, int col, int64_t ld) {
+  switch (layout) {
+    case BB_ROW_MAJOR_F32: return load_x<BB_ROW_MAJOR_F32>(x, row, col, ld);
+    case BB_COL_MAJOR_F32: return load_x<BB_COL_MAJOR_F32>(x, row, col, ld);
+    case BB_ROW_MAJOR_F64: return load_x<BB_ROW_MAJOR_F64>(x, row, col, ld);
+    default: return load_x<BB_COL_MAJOR_F64>(x, row, col, ld);
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// Dynamic shared memory, carved in order: a buffer starts where the previous one ends and spans a whole multiple of
+// its alignment, so the buffers of the largest alignment go first (the base is 1024-byte aligned).  A kernel's carve
+// function runs on the host with base = null to size the launch, and in the kernel to place the buffers, so the
+// byte count and the pointers come from the same code.  The host run asserts that every buffer starts on its
+// alignment, so a carve that takes a more aligned buffer after a less aligned one fails at its first launch.  (The
+// kernels do not round the offset up themselves: that arithmetic raises k_fused's spills.)
+// ------------------------------------------------------------------------------------------
+struct SmemCarver {
+  uint8_t* base;
+  size_t bytes = 0;
+  template <class T>
+  __host__ __device__ __forceinline__ T* take(size_t n, size_t align = 16) {
+#ifndef __CUDA_ARCH__
+    assert(bytes % align == 0 && "carve the buffers of larger alignment first");
+#endif
+    uint8_t* p = base + bytes;  // plain pointer arithmetic: nvcc keeps seeing a shared-memory address
+    bytes += (n + align - 1) / align * align;
+    return reinterpret_cast<T*>(p);
+  }
+};
 
 // ------------------------------------------------------------------------------------------
 // kernel epilogues k(r^2) -- the scaled squared distance t already carries the family's

@@ -1,5 +1,7 @@
 // fused.cu -- the scoring kernel and its launcher: per tile of 128 candidates
-//   K* = k(X*, X)                       CUDA cores (fp32, GEMM-form distance + Matern/RBF epilogue)
+//   K* = k(X*, X)                       distances on the tensor cores (augmented fp16-split GEMM, K = 32 / 64) where
+//                                       the model has the augmented training image, else on the CUDA cores (fp32
+//                                       GEMM form); Matern/RBF epilogue on the CUDA cores
 //   mu~ = c + K* alpha                  CUDA cores (fp32, folded into the K* pass)
 //   V = K* L^-T                         warpgroup MMAs (wgmma), fp16 hi/lo split x3, fp32 accumulators in
 //                                       registers, lower-triangular structure of L^-1 skipped tile-wise
@@ -51,66 +53,40 @@ struct FusedSmem {
   volatile unsigned* ready_cache;
 };
 
-// stages_b = number of L^-1 tiles in flight; returns the byte count (base == nullptr: size only)
-static __host__ __device__ size_t carve_fused(uint8_t* base, const FusedParams& p, FusedSmem* s) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    const size_t o = off;
-    off += (bytes + 15) / 16 * 16;
-    return base + o;
-  };
-  uint8_t* ring_b = take((size_t)p.stages_b * kStageBBytes);  // first: 1024-byte aligned swizzled tiles
-  uint8_t* abuf = take(p.tc ? 0 : (size_t)kConsumerWGs * kABytes);
-  uint8_t* bt = take((size_t)3 * p.n_pad * p.tc * 2);  // 1024-byte aligned: swizzle atoms
-  uint8_t* a2 = take((size_t)kConsumerWGs * 3 * 64 * p.tc * 2);
-  uint8_t* an_x = take(p.tc ? 2 * kTileM * 4 : 0);
-  uint8_t* xt4 = take(p.tc ? 0 : (size_t)p.n_pad * p.d_pad * 4);
-  uint8_t* tsq = take((size_t)p.n_pad * 4);
-  uint8_t* alpha_s = take((size_t)p.n_pad * 4);
-  uint8_t* ttask = take((size_t)p.n_pad * 4);
-  uint8_t* a_s = take(p.tc ? 0 : (size_t)kTileM * p.d_pad * 8);  // duplicated candidate values
-  uint8_t* z_s = take(kMaxSamples * 4);
-  uint8_t* mean_part = take(4 * kTileM * 4);          // [4 octet groups][128]
-  uint8_t* var_part = take(kTileM * 4);
-  uint8_t* mc_part = take(1024 * 4);                  // qLogEI table + exact rows, or [2 groups][128][2]
-  uint8_t* tcov = take(kMaxTasks * kMaxTasks * 4);
-  uint8_t* meanc = take(kMaxTasks * 4);
-  uint8_t* cand_task = take(kTileM * 4);
-  uint8_t* cscale = take((size_t)p.d_pad * 4);
-  uint8_t* cshift = take((size_t)p.d_pad * 4);
-  uint8_t* bars = take(2 * kMaxStagesB * 8);
-  uint8_t* best = take(4 * 8);
-  uint8_t* misc = take(16);
-  if (s != nullptr) {
-    s->ring_b = ring_b;
-    s->abuf = abuf;
-    s->bt = bt;
-    s->a2 = a2;
-    s->an_x = reinterpret_cast<float*>(an_x);
-    s->xt4 = reinterpret_cast<float4*>(xt4);
-    s->tsq = reinterpret_cast<float*>(tsq);
-    s->alpha_s = reinterpret_cast<float*>(alpha_s);
-    s->ttask = reinterpret_cast<int32_t*>(ttask);
-    s->a_s = reinterpret_cast<float4*>(a_s);
-    s->z_s = reinterpret_cast<float*>(z_s);
-    s->mean_part = reinterpret_cast<float*>(mean_part);
-    s->var_part = reinterpret_cast<float*>(var_part);
-    s->mc_part = reinterpret_cast<float*>(mc_part);
-    s->tcov = reinterpret_cast<float*>(tcov);
-    s->meanc = reinterpret_cast<float*>(meanc);
-    s->cand_task = reinterpret_cast<int32_t*>(cand_task);
-    s->cscale_s = reinterpret_cast<float*>(cscale);
-    s->cshift_s = reinterpret_cast<float*>(cshift);
-    s->b_full = reinterpret_cast<uint64_t*>(bars);
-    s->b_empty = s->b_full + kMaxStagesB;
-    s->best_red = reinterpret_cast<long long*>(best);
-    s->zstat = reinterpret_cast<float*>(misc);  // mean z, mean |z - mean z|
-    s->ready_cache = reinterpret_cast<volatile unsigned*>(misc + 8);
-  }
-  return off;
+// stages_b = number of L^-1 tiles in flight; returns the byte count
+static __host__ __device__ size_t carve_fused(uint8_t* base, const FusedParams& p, FusedSmem& s) {
+  SmemCarver c{base};
+  s.ring_b = c.take<uint8_t>((size_t)p.stages_b * kStageBBytes, 1024);  // swizzled tiles first
+  s.abuf = c.take<uint8_t>(p.tc ? 0 : (size_t)kConsumerWGs * kABytes, 1024);
+  s.bt = c.take<uint8_t>((size_t)3 * p.n_pad * p.tc * 2, 1024);
+  s.a2 = c.take<uint8_t>((size_t)kConsumerWGs * 3 * 64 * p.tc * 2, 1024);
+  s.an_x = c.take<float>(p.tc ? 2 * kTileM * 4 : 0);
+  s.xt4 = c.take<float4>(p.tc ? 0 : (size_t)p.n_pad * p.d_pad * 4);
+  s.tsq = c.take<float>((size_t)p.n_pad * 4);
+  s.alpha_s = c.take<float>((size_t)p.n_pad * 4);
+  s.ttask = c.take<int32_t>((size_t)p.n_pad * 4);
+  s.a_s = c.take<float4>(p.tc ? 0 : (size_t)kTileM * p.d_pad * 8);  // duplicated candidate values
+  s.z_s = c.take<float>(kMaxSamples * 4);
+  s.mean_part = c.take<float>(4 * kTileM * 4);  // [4 octet groups][128]
+  s.var_part = c.take<float>(kTileM * 4);
+  s.mc_part = c.take<float>(1024 * 4);  // qLogEI table + exact rows, or [2 groups][128][2]
+  s.tcov = c.take<float>(kMaxTasks * kMaxTasks * 4);
+  s.meanc = c.take<float>(kMaxTasks * 4);
+  s.cand_task = c.take<int32_t>(kTileM * 4);
+  s.cscale_s = c.take<float>((size_t)p.d_pad * 4);
+  s.cshift_s = c.take<float>((size_t)p.d_pad * 4);
+  s.b_full = c.take<uint64_t>(2 * kMaxStagesB * 8);
+  s.b_empty = s.b_full + kMaxStagesB;
+  s.best_red = c.take<long long>(4 * 8);
+  s.zstat = c.take<float>(16);  // mean z, mean |z - mean z|, then the gated pass's row counts
+  s.ready_cache = reinterpret_cast<volatile unsigned*>(s.zstat + 2);
+  return c.bytes;
 }
 
-static size_t fused_smem_bytes(const FusedParams& p) { return carve_fused(nullptr, p, nullptr); }
+static size_t fused_smem_bytes(const FusedParams& p) {
+  FusedSmem unused;
+  return carve_fused(nullptr, p, unused);
+}
 
 // Position of L^-1 tile (chunk c, sub-block sb >= c) in the c-major image of C chunks.
 __host__ __device__ __forceinline__ size_t rimg_tile(int c, int sb, int C) {
@@ -250,7 +226,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
   constexpr int K2 = TC ? TCK : 32;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   FusedSmem s;
-  carve_fused(smem_raw, p, &s);
+  carve_fused(smem_raw, p, s);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int C = p.n_chunks;
   const int dq = p.d_pad >> 2;
@@ -373,15 +349,7 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
       if constexpr (PRE) {
         if (p.task_col >= 0 && tid < kTileM) {  // task id of each candidate row (mean constant, prior variance)
           const int64_t row = row0 + tid;
-          float tv = 0.f;
-          if (row < p.N) {
-            switch (p.layout) {
-              case BB_ROW_MAJOR_F32: tv = load_x<BB_ROW_MAJOR_F32>(p.x, row, p.task_col, p.ldx); break;
-              case BB_COL_MAJOR_F32: tv = load_x<BB_COL_MAJOR_F32>(p.x, row, p.task_col, p.ldx); break;
-              case BB_ROW_MAJOR_F64: tv = load_x<BB_ROW_MAJOR_F64>(p.x, row, p.task_col, p.ldx); break;
-              default: tv = load_x<BB_COL_MAJOR_F64>(p.x, row, p.task_col, p.ldx); break;
-            }
-          }
+          const float tv = row < p.N ? load_x_any(p.x, p.layout, row, p.task_col, p.ldx) : 0.f;
           s.cand_task[tid] = min(max(__float2int_rn(tv), 0), p.n_tasks - 1);
         }
         bar_compute();
@@ -719,34 +687,19 @@ struct KmatSmem {
   int32_t *cand_task, *ttask;
 };
 
-static __host__ __device__ size_t kmat_carve(uint8_t* base, const FusedParams& p, KmatSmem* s) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    const size_t o = off;
-    off += (bytes + 1023) / 1024 * 1024;  // swizzled tiles and TMA boxes: 1024-byte aligned
-    return base + o;
-  };
-  uint8_t* out = take((size_t)kConsumerWGs * 2 * 16384);
-  uint8_t* bt = take((size_t)3 * p.n_pad * p.tc * 2);
-  uint8_t* a2 = take((size_t)kConsumerWGs * 3 * 64 * p.tc * 2);
-  uint8_t* an_x = take(2 * kTileM * 4);
-  uint8_t* cs = take((size_t)p.d_pad * 4);
-  uint8_t* sh = take((size_t)p.d_pad * 4);
-  uint8_t* tc = take(kMaxTasks * kMaxTasks * 4);
-  uint8_t* ct = take(kTileM * 4);
-  uint8_t* tt = take((size_t)p.n_pad * 4);
-  if (s != nullptr) {
-    s->out = out;
-    s->bt = bt;
-    s->a2 = a2;
-    s->an_x = reinterpret_cast<float*>(an_x);
-    s->cscale = reinterpret_cast<float*>(cs);
-    s->cshift = reinterpret_cast<float*>(sh);
-    s->tcov = reinterpret_cast<float*>(tc);
-    s->cand_task = reinterpret_cast<int32_t*>(ct);
-    s->ttask = reinterpret_cast<int32_t*>(tt);
-  }
-  return off;
+// Every buffer on a 1024-byte boundary, as the swizzled tiles and TMA boxes need.
+static __host__ __device__ size_t kmat_carve(uint8_t* base, const FusedParams& p, KmatSmem& s) {
+  SmemCarver c{base};
+  s.out = c.take<uint8_t>((size_t)kConsumerWGs * 2 * 16384, 1024);
+  s.bt = c.take<uint8_t>((size_t)3 * p.n_pad * p.tc * 2, 1024);
+  s.a2 = c.take<uint8_t>((size_t)kConsumerWGs * 3 * 64 * p.tc * 2, 1024);
+  s.an_x = c.take<float>(2 * kTileM * 4, 1024);
+  s.cscale = c.take<float>((size_t)p.d_pad * 4, 1024);
+  s.cshift = c.take<float>((size_t)p.d_pad * 4, 1024);
+  s.tcov = c.take<float>(kMaxTasks * kMaxTasks * 4, 1024);
+  s.cand_task = c.take<int32_t>(kTileM * 4, 1024);
+  s.ttask = c.take<int32_t>((size_t)p.n_pad * 4, 1024);
+  return c.bytes;
 }
 
 template <int FAMILY, int K2>
@@ -754,7 +707,7 @@ __global__ void __launch_bounds__(kConsumerThreads, 1) k_kmat_tma(const FusedPar
                                                                   const __grid_constant__ CUtensorMap tm) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   KmatSmem s;
-  kmat_carve(smem_raw, p, &s);
+  kmat_carve(smem_raw, p, s);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, t = tid & 127;
   if (tid == 0 && (smem_u32(smem_raw) & 1023u) != 0u) __trap();
   {
@@ -844,14 +797,9 @@ static int launch_kmat_tma_one(const FusedParams& p, const CUtensorMap& tm, int 
   return BB_OK;
 }
 
-// bb_kernel_matrix front door of k_kmat_tma: *handled = false when the model or the output is outside its envelope
-// (no augmented training image, Matern-1/2, bit-packed rows, ldk not a multiple of 4 or d_k not 16-byte aligned).
-int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, float* d_k, int64_t ldk,
-                 cudaStream_t stream, bool* handled) {
-  *handled = false;
-  if (m->wide || m->d_timg_b == nullptr || (m->dist_k != 32 && m->dist_k != 64) || m->family == BB_KERNEL_MATERN12 ||
-      layout == BB_BITS_U8 || (ldk & 3) != 0 || (reinterpret_cast<uintptr_t>(d_k) & 15) != 0 || m->n_tasks > kMaxTasks)
-    return BB_OK;
+// FusedParams of a launch over candidates x: the candidate and model fields (acquisition and outputs: the caller's).
+// The tensor-core distance fields are set where the model has the augmented training image (p.tc = model_tc_k).
+static FusedParams fused_params(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx) {
   FusedParams p;
   memset(&p, 0, sizeof(p));
   p.x = d_x;
@@ -861,25 +809,49 @@ int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
   p.num_tiles = (int)((N + kTileM - 1) / kTileM);
   p.cand_scale = m->d_cand_scale;
   p.cand_shift = m->d_cand_shift;
+  p.train_m2 = m->d_train_m2;
+  p.train_sq = m->d_train_sq;
+  p.alpha = m->d_alpha;
   p.task_covar = m->d_task_covar;
+  p.mean_const = m->d_mean_const;
   p.train_task = m->d_train_task;
+  p.rimg = reinterpret_cast<const uint8_t*>(m->d_rimg);
   p.n_pad = m->n_pad;
   p.d = m->d;
   p.d_pad = m->d_pad;
   p.n_chunks = m->n_chunks;
   p.task_col = m->task_col;
   p.n_tasks = m->n_tasks;
-  p.scaled = (m->task_col >= 0 || m->prior_scale != 1.0f) ? 1 : 0;
-  p.tc = m->dist_k;
-  p.timg_b = reinterpret_cast<const uint8_t*>(m->d_timg_b);
-  p.ts_sa = m->ts_sa;
-  p.ts_aug_sq = m->ts_aug_sq;
-  p.ts_aug_one = m->ts_aug_one;
-  p.ts_g = m->ts_g;
+  p.y_mean = m->y_mean;
+  p.y_std = m->y_std;
+  p.inv_r_scale2 = 1.0f / (m->r_scale * m->r_scale);
+  p.scaled = model_scaled(m) ? 1 : 0;
+  p.tc = model_tc_k(m);
+  if (p.tc) {
+    p.timg_b = reinterpret_cast<const uint8_t*>(m->d_timg_b);
+    p.ts_sa = m->ts_sa;
+    p.ts_aug_sq = m->ts_aug_sq;
+    p.ts_aug_one = m->ts_aug_one;
+    p.ts_g = m->ts_g;
+    p.ts_kscale = m->ts_kscale;
+    p.inv_r_scale2 /= m->ts_kscale * m->ts_kscale;  // |V|^2 of ts_kscale K*
+  }
+  return p;
+}
+
+// bb_kernel_matrix front door of k_kmat_tma, after check_candidates: *handled = false when the model or the output is
+// outside its envelope (no tensor-core distances, ldk not a multiple of 4 or d_k not 16-byte aligned).
+int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, float* d_k, int64_t ldk,
+                 cudaStream_t stream, bool* handled) {
+  *handled = false;
+  if (model_tc_k(m) == 0 || layout == BB_BITS_U8 || (ldk & 3) != 0 || (reinterpret_cast<uintptr_t>(d_k) & 15) != 0)
+    return BB_OK;
+  const FusedParams p = fused_params(m, d_x, layout, N, ldx);
   int sms = 0, max_smem = 0;
   int rc = device_limits(&sms, &max_smem);
   if (rc != BB_OK) return rc;
-  const size_t smem = kmat_carve(nullptr, p, nullptr);
+  KmatSmem unused;
+  const size_t smem = kmat_carve(nullptr, p, unused);
   if (smem > (size_t)max_smem) return BB_OK;
   static EncodeTiledFn encode = nullptr;
   if (encode == nullptr) {
@@ -902,19 +874,11 @@ int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
     return BB_ERR_CUDA;
   }
   const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-  if (p.tc == 32) {
-    switch (m->family) {
-      case BB_KERNEL_MATERN32: rc = launch_kmat_tma_one<BB_KERNEL_MATERN32, 32>(p, tm, grid, smem, stream); break;
-      case BB_KERNEL_MATERN52: rc = launch_kmat_tma_one<BB_KERNEL_MATERN52, 32>(p, tm, grid, smem, stream); break;
-      default: rc = launch_kmat_tma_one<BB_KERNEL_RBF, 32>(p, tm, grid, smem, stream); break;
-    }
-  } else {
-    switch (m->family) {
-      case BB_KERNEL_MATERN32: rc = launch_kmat_tma_one<BB_KERNEL_MATERN32, 64>(p, tm, grid, smem, stream); break;
-      case BB_KERNEL_MATERN52: rc = launch_kmat_tma_one<BB_KERNEL_MATERN52, 64>(p, tm, grid, smem, stream); break;
-      default: rc = launch_kmat_tma_one<BB_KERNEL_RBF, 64>(p, tm, grid, smem, stream); break;
-    }
-  }
+  rc = dispatch_family<false>(m->family, [&](auto fam) {
+    constexpr int F = decltype(fam)::value;
+    return p.tc == 32 ? launch_kmat_tma_one<F, 32>(p, tm, grid, smem, stream)
+                      : launch_kmat_tma_one<F, 64>(p, tm, grid, smem, stream);
+  });
   if (rc == BB_OK) *handled = true;
   return rc;
 }
@@ -1037,20 +1001,11 @@ static thread_local int g_trace_cap = 0;
 int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx,
                  const bb_acq_spec* acq, const float* d_z, int32_t S, const uint8_t* d_keep,
                  float* d_mu, float* d_var, float* d_score, int64_t* d_best_key,
-                 int64_t index_offset, cudaStream_t stream, const WideCross* wc = nullptr,
-                 const StreamGate* gate = nullptr) {
-  BB_CHECK_ARG(m && m->abi_version == BB_ABI_VERSION, "model struct missing or ABI mismatch");
-  BB_CHECK_ARG(d_x != nullptr || N == 0, "candidate pointer is null");
-  BB_CHECK_ARG(layout >= 0 && layout <= BB_BITS_U8, "unknown candidate layout %d", layout);
-  BB_CHECK_ARG(N >= 0, "negative candidate count");
-  BB_CHECK_SUPPORTED(layout != BB_BITS_U8 || m->wide,
-                     "bit-packed candidates need a wide-feature model (n_pad*d_pad*4 > 56 KB)");
-  const bool col_major = (layout == BB_COL_MAJOR_F32 || layout == BB_COL_MAJOR_F64);
-  BB_CHECK_ARG((gate != nullptr && gate->layout >= kLayoutCodes4) ||  // code rows: ld in bytes, checked by the caller
-                   (layout == BB_BITS_U8 ? ldx >= (m->d + 7) / 8 : (col_major ? ldx >= N : ldx >= m->d)),
-               "leading dimension %lld too small", (long long)ldx);
+                 int64_t index_offset, cudaStream_t stream, const WideCross* wc, const StreamGate* gate) {
+  const bool code_rows = gate != nullptr && gate->layout >= kLayoutCodes4;
+  const int rc_x = check_candidates(m, d_x, layout, N, ldx, !code_rows);
+  if (rc_x != BB_OK) return rc_x;
   BB_CHECK_ARG(N + index_offset < 0xffffffffLL, "candidate index exceeds the 32-bit key range");
-  BB_CHECK_SUPPORTED(m->n_tasks <= kMaxTasks, "at most %d tasks supported", kMaxTasks);
   if (acq) {
     BB_CHECK_ARG(acq->kind >= BB_ACQ_QLOGEI && acq->kind <= BB_ACQ_PSTD, "unknown acquisition kind %d",
                  acq->kind);
@@ -1061,34 +1016,7 @@ int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
   }
   if (N == 0) return BB_OK;
 
-  FusedParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = d_x;
-  p.layout = layout;
-  p.N = N;
-  p.ldx = ldx;
-  p.num_tiles = (int)((N + kTileM - 1) / kTileM);
-  p.cand_scale = m->d_cand_scale;
-  p.cand_shift = m->d_cand_shift;
-  p.train_m2 = m->d_train_m2;
-  p.train_sq = m->d_train_sq;
-  p.alpha = m->d_alpha;
-  p.task_covar = m->d_task_covar;
-  p.mean_const = m->d_mean_const;
-  p.train_task = m->d_train_task;
-  p.rimg = reinterpret_cast<const uint8_t*>(m->d_rimg);
-  p.family = m->family;
-  p.n_pad = m->n_pad;
-  p.d = m->d;
-  p.d_pad = m->d_pad;
-  p.n_chunks = m->n_chunks;
-  p.task_col = m->task_col;
-  p.n_tasks = m->n_tasks;
-  p.y_mean = m->y_mean;
-  p.y_std = m->y_std;
-  p.prior_scale = m->prior_scale;
-  p.inv_r_scale2 = 1.0f / (m->r_scale * m->r_scale);
-  p.scaled = (m->task_col >= 0 || m->prior_scale != 1.0f) ? 1 : 0;
+  FusedParams p = fused_params(m, d_x, layout, N, ldx);
   p.has_acq = acq ? 1 : 0;
   if (acq) p.acq = *acq;
   p.z = d_z;
@@ -1107,17 +1035,6 @@ int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
     p.code_table = gate->code_table;
     p.code_table_ld = gate->code_table_ld;
     p.layout = gate->layout;
-  }
-  // tensor-core distances where the model carries the augmented training image
-  if (!m->wide && m->d_timg_b != nullptr && m->family != BB_KERNEL_MATERN12 && (m->dist_k == 32 || m->dist_k == 64)) {
-    p.tc = m->dist_k;
-    p.timg_b = reinterpret_cast<const uint8_t*>(m->d_timg_b);
-    p.ts_sa = m->ts_sa;
-    p.ts_aug_sq = m->ts_aug_sq;
-    p.ts_aug_one = m->ts_aug_one;
-    p.ts_g = m->ts_g;
-    p.ts_kscale = m->ts_kscale;
-    p.inv_r_scale2 /= m->ts_kscale * m->ts_kscale;  // |V|^2 of ts_kscale K*
   }
   int max_smem = 0, sms = 0;
   {
@@ -1141,32 +1058,19 @@ int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
   }
   const size_t smem = fused_smem_bytes(p);
   const bool dep = p.mc_table != nullptr;
-  if (p.tc == 32) {
-    switch (m->family) {
-      case BB_KERNEL_MATERN32: return launch_one<BB_KERNEL_MATERN32, false, 32>(p, grid, smem, stream, dep);
-      case BB_KERNEL_MATERN52: return launch_one<BB_KERNEL_MATERN52, false, 32>(p, grid, smem, stream, dep);
-      default: return launch_one<BB_KERNEL_RBF, false, 32>(p, grid, smem, stream, dep);
-    }
-  }
-  if (p.tc == 64) {
-    switch (m->family) {
-      case BB_KERNEL_MATERN32: return launch_one<BB_KERNEL_MATERN32, false, 64>(p, grid, smem, stream, dep);
-      case BB_KERNEL_MATERN52: return launch_one<BB_KERNEL_MATERN52, false, 64>(p, grid, smem, stream, dep);
-      default: return launch_one<BB_KERNEL_RBF, false, 64>(p, grid, smem, stream, dep);
-    }
-  }
-  switch (m->family) {
-    case BB_KERNEL_MATERN12: return launch_one<BB_KERNEL_MATERN12, false>(p, grid, smem, stream, dep);
-    case BB_KERNEL_MATERN32: return launch_one<BB_KERNEL_MATERN32, false>(p, grid, smem, stream, dep);
-    case BB_KERNEL_MATERN52: return launch_one<BB_KERNEL_MATERN52, false>(p, grid, smem, stream, dep);
-    default: return launch_one<BB_KERNEL_RBF, false>(p, grid, smem, stream, dep);
-  }
+  if (p.tc == 0)
+    return dispatch_family<true>(m->family, [&](auto fam) {
+      return launch_one<decltype(fam)::value, false>(p, grid, smem, stream, dep);
+    });
+  return dispatch_family<false>(m->family, [&](auto fam) {
+    constexpr int F = decltype(fam)::value;
+    return p.tc == 32 ? launch_one<F, false, 32>(p, grid, smem, stream, dep)
+                      : launch_one<F, false, 64>(p, grid, smem, stream, dep);
+  });
 }
 
 // Shape test of the single-launch gated pass: k_fused over non-wide models.
-bool fused_gate_supported(const bb_model* m, const bb_acq_spec* acq, int32_t S) {
-  (void)acq;
-  (void)S;
+bool fused_gate_supported(const bb_model* m) {
   if (m == nullptr || m->wide || m->n_tasks > kMaxTasks) return false;
   FusedParams p;
   memset(&p, 0, sizeof(p));
@@ -1197,12 +1101,6 @@ extern "C" int bb_score_fused(const bb_model* m, const bb_acq_spec* a, const voi
   BB_CHECK_ARG(a != nullptr, "bb_score_fused: acquisition spec is null");
   return launch_fused(m, d_x, layout, N, ldx, a, d_z, S, d_keep, nullptr, nullptr, d_score,
                       d_best_key, index_offset, (cudaStream_t)stream);
-}
-
-namespace bb {
-int launch_cross(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx,
-                 const float* d_pend_x, const float* d_pend_beta, int32_t P, float* d_cross,
-                 cudaStream_t stream);
 }
 
 extern "C" int bb_posterior(const bb_model* m, const void* d_x, int32_t layout, int64_t N,

@@ -1,8 +1,11 @@
-// fused_common.cuh -- parameters and helpers shared by the scoring kernels
-//   fused.cu  k_fused    distances on CUDA cores, V = K* L^-T on warpgroup MMAs (wgmma), q = 1 acquisition and
-//                        arg-max; its PRE variant reads a K* block instead (wide-feature path)
+// fused_common.cuh -- parameters and helpers shared by the scoring kernels, and the host side every launcher uses
+// (candidate checks, model-derived choices, family dispatch, the launchers' prototypes)
+//   fused.cu  k_fused    distances on the tensor cores or the CUDA cores, V = K* L^-T on warpgroup MMAs (wgmma),
+//                        q = 1 acquisition and arg-max; its PRE variant reads a K* block instead (wide-feature path)
 //   wide.cu   k_kmat_wg  K-looped wgmma distance GEMM for wide / bit-packed feature spaces and n_pad > 512
 #pragma once
+
+#include <type_traits>
 
 #include "acq_math.cuh"
 #include "common.cuh"
@@ -35,20 +38,23 @@ struct FusedParams {
   const void* x;
   int layout;
   int64_t N, ldx;
-  int num_tiles;
-  // model
+  // model.  The order of the 4-byte scalars from num_tiles to panel_sb is not arbitrary: it places each at the 8-byte
+  // parity it had when ptxas allocated the fewest spills for the K = 64 tensor-core k_fused (ptxas pairs adjacent
+  // parameter words into 64-bit loads); other orders spill more.
   const float *cand_scale, *cand_shift, *train_m2, *train_sq, *alpha, *task_covar, *mean_const;
   const int32_t* train_task;
   const uint8_t* rimg;  // fp16 hi/lo image of L^-1: tiles (chunk c, sub-block s >= c), c-major
-  int family;
+  int num_tiles;        // 128-row candidate tiles
   int n_pad, d, d_pad, n_chunks, task_col, n_tasks;
-  float y_mean, y_std, prior_scale, inv_r_scale2;
+  float y_mean, y_std;
+  // tensor-core distances (tc = K extent 32 / 64, 0: none): augmented training image [sb (-2b) | Q1 | |b|^2 Q] as
+  // fp16 hi/mid/lo panels of n_pad rows x tc k; candidate rows become [sa a | |a|^2 P | P1], so the GEMM yields
+  // t / ts_g directly
+  int tc;
+  float inv_r_scale2;
   int scaled;  // task kernel or output scale present
   int stages_b;  // L^-1 tiles in flight
   int panel_sb;  // V sub-blocks per column panel (kPanelSB or 2), chosen with stages_b by pick_stages
-  // tensor-core distances (tc = 1): augmented training image [sb (-2b) | Q1 | |b|^2 Q] as fp16 hi/mid/lo panels of
-  // n_pad rows x 32 k (SW64); candidate rows become [sa a | |a|^2 P | P1], so the GEMM yields t / ts_g directly
-  int tc;
   const uint8_t* timg_b;
   float ts_sa, ts_aug_sq, ts_aug_one, ts_g;
   float ts_kscale;  // power of two applied to K* before the fp16 hi/lo split (fp16 range and resolution)
@@ -153,11 +159,56 @@ __device__ __forceinline__ bool elect_one() {
       : "=r"(pred));
   return pred != 0;
 }
-int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, float* d_k, int64_t ldk,
-                 cudaStream_t stream, bool* handled);
-int launch_pend_images(const bb_model* m, int32_t layout, const float* d_pend_x, int32_t P, cudaStream_t stream);
-int launch_cross_wide(const bb_model* m, const void* d_x, int32_t layout, int64_t nb, int64_t ldx,
-                      const float* d_pend_beta, int32_t P, float* d_cross_blk, cudaStream_t stream);
+
+// ------------------------------------------------------------------------------------------
+// host side shared by every launcher
+// ------------------------------------------------------------------------------------------
+// Checks of a candidate matrix, made by every entry point that reads one before any CUDA call.  check_ld = false
+// skips the leading-dimension check (level-coded rows of the gated host pass: ld in bytes, checked by the caller).
+inline int check_candidates(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx,
+                            bool check_ld = true) {
+  BB_CHECK_ARG(m && m->abi_version == BB_ABI_VERSION, "model struct missing or ABI mismatch");
+  BB_CHECK_ARG(d_x != nullptr || N == 0, "candidate pointer is null");
+  BB_CHECK_ARG(layout >= 0 && layout <= BB_BITS_U8, "unknown candidate layout %d", layout);
+  BB_CHECK_ARG(N >= 0, "negative candidate count");
+  BB_CHECK_SUPPORTED(layout != BB_BITS_U8 || m->wide,
+                     "bit-packed candidates need a wide-feature model (n_pad*d_pad*4 > 56 KB)");
+  const bool col_major = (layout == BB_COL_MAJOR_F32 || layout == BB_COL_MAJOR_F64);
+  BB_CHECK_ARG(!check_ld || (layout == BB_BITS_U8 ? ldx >= (m->d + 7) / 8 : (col_major ? ldx >= N : ldx >= m->d)),
+               "leading dimension %lld too small", (long long)ldx);
+  BB_CHECK_SUPPORTED(m->n_tasks <= kMaxTasks, "at most %d tasks supported", kMaxTasks);
+  return BB_OK;
+}
+
+// K* is multiplied by the task covariance (task kernel or output scale present)
+inline bool model_scaled(const bb_model* m) { return m->task_col >= 0 || m->prior_scale != 1.0f; }
+
+// K extent (32 or 64) of the tensor-core distance GEMM over the augmented training image, 0 where the distances run
+// on the CUDA cores.  Matern-1/2 has no such kernel: GEMM-form distances are singular at r = 0.
+inline int model_tc_k(const bb_model* m) {
+  const bool tc = !m->wide && m->d_timg_b != nullptr && m->family != BB_KERNEL_MATERN12 &&
+                  (m->dist_k == 32 || m->dist_k == 64);
+  return tc ? m->dist_k : 0;
+}
+
+// Calls f(std::integral_constant<int, FAMILY>()) for a runtime kernel family and returns its status.  With
+// kMatern12 = false, Matern-1/2 is rejected instead of instantiated (the tensor-core distance kernels).
+template <bool kMatern12, class F>
+int dispatch_family(int family, F&& f) {
+  switch (family) {
+    case BB_KERNEL_MATERN12:
+      if constexpr (kMatern12) {
+        return f(std::integral_constant<int, BB_KERNEL_MATERN12>());
+      } else {
+        set_error("Matern-1/2 has no tensor-core distance kernel");
+        return BB_ERR_UNSUPPORTED;
+      }
+    case BB_KERNEL_MATERN32: return f(std::integral_constant<int, BB_KERNEL_MATERN32>());
+    case BB_KERNEL_MATERN52: return f(std::integral_constant<int, BB_KERNEL_MATERN52>());
+    default: return f(std::integral_constant<int, BB_KERNEL_RBF>());
+  }
+}
+
 // pending-point request threaded through launch_fused on the wide path (null members: none)
 struct WideCross {
   const float* pend_x;
@@ -165,9 +216,25 @@ struct WideCross {
   int32_t P;
   float* cross;
 };
+
+// fused.cu
+int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, const bb_acq_spec* acq,
+                 const float* d_z, int32_t S, const uint8_t* d_keep, float* d_mu, float* d_var, float* d_score,
+                 int64_t* d_best_key, int64_t index_offset, cudaStream_t stream, const WideCross* wc = nullptr,
+                 const StreamGate* gate = nullptr);
+// k_kmat_tma; *handled = false when the model or the output is outside its envelope
+int try_kmat_tma(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, float* d_k, int64_t ldk,
+                 cudaStream_t stream, bool* handled);
 // true when the single-launch gated pass can run this model
-bool fused_gate_supported(const bb_model* m, const bb_acq_spec* acq, int32_t S);
+bool fused_gate_supported(const bb_model* m);
+// aux_kernels.cu
+int launch_cross(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, const float* d_pend_x,
+                 const float* d_pend_beta, int32_t P, float* d_cross, cudaStream_t stream);
+// wide.cu
 int launch_kmat_wide(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx,
                      float* d_out, int64_t ldk, int64_t out_rows, int out_cols, cudaStream_t stream);
+int launch_pend_images(const bb_model* m, int32_t layout, const float* d_pend_x, int32_t P, cudaStream_t stream);
+int launch_cross_wide(const bb_model* m, const void* d_x, int32_t layout, int64_t nb, int64_t ldx,
+                      const float* d_pend_beta, int32_t P, float* d_cross_blk, cudaStream_t stream);
 
 }  // namespace bb

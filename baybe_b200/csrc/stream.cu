@@ -11,16 +11,6 @@
 
 #include "fused_common.cuh"
 
-namespace bb {
-int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, int64_t ldx, const bb_acq_spec* acq,
-                 const float* d_z, int32_t S, const uint8_t* d_keep, float* d_mu, float* d_var, float* d_score,
-                 int64_t* d_best_key, int64_t index_offset, cudaStream_t stream, const WideCross* wc,
-                 const StreamGate* gate);
-}
-extern "C" int bb_decode_codes(const uint8_t* d_codes, int32_t bits, int64_t N, int32_t d, int64_t ld_bytes,
-                               const float* d_table, int32_t table_ld, float* d_out, int64_t ldo, void* stream);
-extern "C" int bb_best_init(int64_t* d_best_key, void* stream);
-
 using namespace bb;
 
 extern "C" int bb_score_fused_host(const bb_model* m, const bb_acq_spec* a, const void* h_x, int32_t host_format,
@@ -139,7 +129,7 @@ extern "C" int bb_score_fused_overlapped(const bb_model* m, const bb_acq_spec* a
     BB_CHECK_ARG(ld >= d, "bb_score_fused_overlapped: leading dimension smaller than d");
   }
   BB_CHECK_ARG((int64_t)(row_bytes * (size_t)N) <= stage_bytes, "bb_score_fused_overlapped: staging buffer too small");
-  BB_CHECK_SUPPORTED(fused_gate_supported(m, a, S), "bb_score_fused_overlapped: shape outside the headline kernel's envelope");
+  BB_CHECK_SUPPORTED(fused_gate_supported(m), "bb_score_fused_overlapped: shape outside the headline kernel's envelope");
   static WriteValue32Fn write32 = nullptr;
   if (write32 == nullptr) {
     void* fn = nullptr;

@@ -59,29 +59,17 @@ struct WideSmem {
 };
 
 template <bool BITS>
-__host__ __device__ inline size_t wide_carve(uint8_t* base, const WideParams& p, WideSmem* s) {
+__host__ __device__ inline size_t wide_carve(uint8_t* base, const WideParams& p, WideSmem& s) {
   constexpr uint32_t kStage = (BITS ? 1 : 3) * kWPanelA + (BITS ? 2 : 3) * kWPanelB;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    size_t o = off;
-    off += (bytes + 15) / 16 * 16;
-    return o;
-  };
-  const size_t o_ring = take((size_t)p.stages * kStage);
-  const size_t o_wn = take((size_t)p.n_pad * 4), o_tt = take((size_t)p.n_pad * 4);
-  const size_t o_an = take(2 * kWTileM * 8), o_tc = take(kMaxTasks * kMaxTasks * 4);
-  const size_t o_bar = take(16 * 8);
-  if (s) {
-    s->ring = base + o_ring;
-    s->wnorm_s = reinterpret_cast<float*>(base + o_wn);
-    s->ttask = reinterpret_cast<int32_t*>(base + o_tt);
-    s->an_part = reinterpret_cast<double*>(base + o_an);
-    s->tcov = reinterpret_cast<float*>(base + o_tc);
-    uint64_t* b = reinterpret_cast<uint64_t*>(base + o_bar);
-    s->full = b;       // [<=4]
-    s->empty = b + 4;  // [<=4]
-  }
-  return off;
+  SmemCarver c{base};
+  s.ring = c.take<uint8_t>((size_t)p.stages * kStage, 1024);  // swizzled panels
+  s.wnorm_s = c.take<float>((size_t)p.n_pad * 4);
+  s.ttask = c.take<int32_t>((size_t)p.n_pad * 4);
+  s.an_part = c.take<double>(2 * kWTileM * 8);
+  s.tcov = c.take<float>(kMaxTasks * kMaxTasks * 4);
+  s.full = c.take<uint64_t>(16 * 8);  // [<=4]
+  s.empty = s.full + 4;               // [<=4]
+  return c.bytes;
 }
 
 // 16 consecutive features k0..k0+15 of one candidate row as fp32 (0 beyond d / beyond N).
@@ -145,7 +133,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_kmat_wg(const WideParams p)
   constexpr uint32_t kStage = kStageA + PB * kWPanelB;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   WideSmem s;
-  wide_carve<BITS>(smem_raw, p, &s);
+  wide_carve<BITS>(smem_raw, p, s);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   if (tid == 0 && (smem_u32(smem_raw) & 1023u) != 0u) __trap();
 
@@ -312,13 +300,7 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_kmat_wg(const WideParams p)
         const float an_r = (float)(s.an_part[rl] + s.an_part[kWTileM + rl]);
         int ct = 0;
         if (p.scaled && p.task_col >= 0 && grow < p.N) {
-          float tv;
-          switch (p.layout) {
-            case BB_ROW_MAJOR_F32: tv = load_x<BB_ROW_MAJOR_F32>(p.x, grow, p.task_col, p.ldx); break;
-            case BB_COL_MAJOR_F32: tv = load_x<BB_COL_MAJOR_F32>(p.x, grow, p.task_col, p.ldx); break;
-            case BB_ROW_MAJOR_F64: tv = load_x<BB_ROW_MAJOR_F64>(p.x, grow, p.task_col, p.ldx); break;
-            default: tv = load_x<BB_COL_MAJOR_F64>(p.x, grow, p.task_col, p.ldx); break;
-          }
+          const float tv = load_x_any(p.x, p.layout, grow, p.task_col, p.ldx);
           ct = min(max(__float2int_rn(tv), 0), p.n_tasks - 1);
         }
         const float* tcrow = s.tcov + ct * p.n_tasks;
@@ -382,19 +364,14 @@ __global__ void __launch_bounds__(kWideThreads, 1) k_kmat_wg(const WideParams p)
 template <int FAMILY, bool BITS>
 static int launch_kmat_one(WideParams& p, int sms, int max_smem, cudaStream_t stream) {
   p.stages = 4;
-  const size_t smem = wide_carve<BITS>(nullptr, p, nullptr);
+  WideSmem unused;
+  const size_t smem = wide_carve<BITS>(nullptr, p, unused);
   BB_CHECK_SUPPORTED(smem <= (size_t)max_smem, "wide kernel-matrix path: shared-memory budget exceeded (%zu bytes)", smem);
   BB_SMEM_OPTIN_ONCE((k_kmat_wg<FAMILY, BITS>));
   const int grid = p.num_items < sms ? p.num_items : sms;
   k_kmat_wg<FAMILY, BITS><<<grid, kWideThreads, smem, stream>>>(p);
   BB_LAUNCH_CHECK();
   return BB_OK;
-}
-
-template <int FAMILY>
-static int launch_kmat_family(WideParams& p, bool bits, int sms, int max_smem, cudaStream_t stream) {
-  return bits ? launch_kmat_one<FAMILY, true>(p, sms, max_smem, stream)
-              : launch_kmat_one<FAMILY, false>(p, sms, max_smem, stream);
 }
 
 // Column set of a K(X*, .) launch: the training rows (model images) or the pending points (scratch images).
@@ -431,7 +408,7 @@ static int launch_kmat_cols(const bb_model* m, const WideColumns& c, const void*
   p.task_covar = m->d_task_covar;
   p.task_col = m->task_col;
   p.n_tasks = m->n_tasks;
-  p.scaled = (m->task_col >= 0 || m->prior_scale != 1.0f) ? 1 : 0;
+  p.scaled = model_scaled(m) ? 1 : 0;
   p.out = d_out;
   p.ldk = ldk;
   p.out_rows = out_rows;
@@ -444,11 +421,10 @@ static int launch_kmat_cols(const bb_model* m, const WideColumns& c, const void*
     const int rc_lim = device_limits(&sms, &max_smem);
     if (rc_lim != BB_OK) return rc_lim;
   }
-  switch (m->family) {
-    case BB_KERNEL_MATERN32: return launch_kmat_family<BB_KERNEL_MATERN32>(p, bits, sms, max_smem, stream);
-    case BB_KERNEL_MATERN52: return launch_kmat_family<BB_KERNEL_MATERN52>(p, bits, sms, max_smem, stream);
-    default: return launch_kmat_family<BB_KERNEL_RBF>(p, bits, sms, max_smem, stream);
-  }
+  return dispatch_family<false>(m->family, [&](auto fam) {
+    constexpr int F = decltype(fam)::value;
+    return bits ? launch_kmat_one<F, true>(p, sms, max_smem, stream) : launch_kmat_one<F, false>(p, sms, max_smem, stream);
+  });
 }
 
 static int wide_checks(const bb_model* m, int32_t layout) {
@@ -590,7 +566,7 @@ int launch_cross_wide(const bb_model* m, const void* d_x, int32_t layout, int64_
   int rc = launch_kmat_cols(m, c, d_x, layout, nb, ldx, m->d_kpend_ws, 64, rows_pad, 64, stream);
   if (rc != BB_OK) return rc;
   const size_t smem = (size_t)P * m->n_pad * sizeof(float);
-  BB_CUDA(cudaFuncSetAttribute(k_cross_pre, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  BB_SMEM_OPTIN_ONCE(k_cross_pre);
   int sms = 0, max_smem = 0;
   rc = device_limits(&sms, &max_smem);
   if (rc != BB_OK) return rc;

@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define BB_ABI_VERSION 2
+#define BB_ABI_VERSION 3
 
 typedef enum bb_status {
   BB_OK = 0,
@@ -77,7 +77,7 @@ typedef enum bb_acq_kind {
 
 #define BB_MAX_PENDING 31 /* max pending points in a joint (q>1) evaluation */
 #define BB_MAX_TRAIN 1024 /* max training points of this build (gpytorch switches away from exact Cholesky
-                             above 800); n > 512 always takes the wide-feature path (two V column panels) */
+                             above 800); n > 512 always takes the wide-feature path (K* block + K*-reading kernel) */
 
 /*
  * Description of a fitted GP, i.e. what botorch.models.SingleTaskGP holds after
@@ -109,9 +109,9 @@ typedef struct bb_model_desc {
  * bb_model_build; the pointers point INTO the caller-owned blob.
  *
  * Concurrency: the caches are read-only after the build, but the blob also holds per-call SCRATCH -- the K* block
- * and pending-point images of the wide-feature path, the per-call qLogEI table (d_mc_table), the |V|^2 partial of
- * two-panel models.  Calls that use one bb_model must therefore be ordered on ONE stream (or externally
- * serialised); two streams need two models (two blobs built from the same bb_model_desc).
+ * and pending-point images of the wide-feature path and the per-call qLogEI table (d_mc_table).  Calls that use one
+ * bb_model must therefore be ordered on ONE stream (or externally serialised); two streams need two models (two
+ * blobs built from the same bb_model_desc).
  */
 typedef struct bb_model {
   int32_t abi_version;
@@ -138,12 +138,8 @@ typedef struct bb_model {
   const double* d_alpha64;   /* [n]                                                       */
   const double* d_xn64;      /* [n*d] normalised training inputs, float64                 */
   const float* d_linv32;     /* [n_pad*n_pad] row-major L^-1, fp32 (zero padded)          */
-  const void* d_bimg;        /* unused (NULL); kept for the ABI                             */
   float dist_scale_a;        /* power-of-two scales folded into the fp16 images of the      */
   float dist_scale_b;        /* candidate rows (a) and training rows (b)                    */
-  int32_t dist_k;            /* K extent of d_timg_b: 32 (d <= 30), 64 (d <= 62), 0 = none */
-  int32_t pad_;
-  const void* d_rimg2;       /* unused (NULL); kept for the ABI                                 */
   /* wide-feature path (n_pad*d_pad*4 > 56 KB, e.g. fingerprint spaces): K-chunked operand images of
    * the tensor-core distance GEMM and a K* workspace (whole waves, <= 40 MB up to n_pad = 640), all inside the blob */
   int32_t wide;              /* 1: scoring runs k_kmat_wg + the K*-reading posterior kernel     */
@@ -154,9 +150,7 @@ typedef struct bb_model {
   float* d_wide_ws;          /* [wide_ws_rows * n_pad] fp32 K* block                            */
   int64_t wide_ws_rows;
   float dist_scale_w;        /* power-of-two scale folded into d_wimg_bits                      */
-  int32_t pad2_;
-  const void* d_rimg4;       /* unused (NULL); kept for the ABI                                 */
-  const void* d_rimg2g;      /* unused (NULL); kept for the ABI                                 */
+  int32_t pad_;
   /* wide path, pending points (sequential greedy): scratch images of <=31 pending rows as extra K columns */
   void* d_pend_img;          /* [64 rows] K-chunked split image, rebuilt per bb_posterior call          */
   float* d_pend_norm;        /* [64]                                                                    */
@@ -165,18 +159,15 @@ typedef struct bb_model {
   float dist_scale_p;        /* power-of-two scales of the pending images (float form / bit-linear form) */
   float dist_scale_wp;
   float* d_mc_table;         /* [1024] per-call qLogEI table of the K*-reading kernel (acq_math.cuh)             */
-  float* d_wide_vacc;        /* unused (NULL); kept for the ABI                                                 */
   /* tensor-core distances (n_pad <= 256, d <= 62; NULL otherwise): augmented training image
    * and the power-of-two scales folded into it */
-  const void* d_timg_l;      /* unused (NULL); kept for the ABI                                                    */
   const void* d_timg_b;      /* training rows [-2b | q | |b|^2 q'] as hi/mid/lo panels of dist_k k (SW64 / SW128)   */
-  const float* d_ts_alpha;   /* unused (NULL); kept for the ABI                                                    */
+  int32_t dist_k;            /* K extent of d_timg_b: 32 (d <= 30), 64 (d <= 62), 0 = none                        */
   float ts_sa;               /* candidate rows are multiplied by ts_sa                                             */
   float ts_aug_sq;           /* K column dist_k - 2 of the candidate tile = |a|^2 * ts_aug_sq                      */
   float ts_aug_one;          /* K column dist_k - 1 of the candidate tile = ts_aug_one                             */
   float ts_g;                /* accumulator * ts_g = scaled squared distance                                       */
   float ts_kscale;           /* K* is multiplied by ts_kscale before the fp16 hi/lo split                          */
-  int32_t pad3_;
 } bb_model;
 
 /* Acquisition context built by BotorchAcquisitionFunctionBuilder.build

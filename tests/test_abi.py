@@ -97,6 +97,87 @@ def test_round2_entry_points_validate_their_arguments_before_any_cuda_call(lib):
     assert rc == _lib.BB_ERR_INVALID and b"rank 3" in lib.bb_last_error()
 
 
+def _fake_model(wide: bool, n_tasks: int):
+    """A bb_model filled by hand: plausible shapes, fake non-null device pointers (never dereferenced)."""
+    import ctypes as C
+
+    from baybe_b200 import _lib
+
+    m = _lib.Model()
+    m.abi_version = _lib.ABI_VERSION
+    m.n = m.n_pad = 64
+    m.n_chunks = 1
+    m.d = m.d_pad = 2048 if wide else 20
+    m.family = _lib.KERNEL_FAMILY["rbf"]
+    m.task_col = -1
+    m.n_tasks = n_tasks
+    m.y_std = m.prior_scale = m.r_scale = 1.0
+    m.wide = int(wide)
+    m.d_wide = m.d if wide else 0
+    for name, ctype in _lib.Model._fields_:
+        if name.startswith("d_") and ctype is C.c_void_p:
+            setattr(m, name, 1 << 20)
+    return m
+
+
+def _call_entry(lib, entry: str, m, layout: int, ldx: int) -> int:
+    import ctypes as C
+
+    from baybe_b200 import _lib
+
+    n = 1000
+    x = out = C.c_void_p(1 << 20)
+    if entry == "bb_score_fused":
+        a = _lib.AcqSpec(kind=_lib.ACQ_KIND["UCB"], beta=2.0, obj_scale=1.0)
+        return lib.bb_score_fused(C.byref(m), C.byref(a), x, layout, n, ldx, None, None, 0, out, out, 0, None)
+    if entry == "bb_posterior":
+        return lib.bb_posterior(C.byref(m), x, layout, n, ldx, out, out, None, None, None, 0, None)
+    if entry == "bb_kernel_matrix":
+        return lib.bb_kernel_matrix(C.byref(m), x, layout, n, ldx, out, m.n, None)
+    return lib.bb_debug_posterior_simt(C.byref(m), x, layout, n, ldx, out, out, None)
+
+
+_ENTRIES = ["bb_score_fused", "bb_posterior", "bb_kernel_matrix", "bb_debug_posterior_simt"]
+# (entry point, wide model) -> status for bit-packed rows: the scoring kernels read them from wide models only, the
+# CUDA-core kernels behind bb_debug_posterior_simt and the non-wide bb_kernel_matrix never
+_BITS_STATUS = {("bb_score_fused", False): "unsupported", ("bb_posterior", False): "unsupported",
+                ("bb_kernel_matrix", False): "invalid", ("bb_debug_posterior_simt", False): "invalid",
+                ("bb_debug_posterior_simt", True): "invalid"}
+_BAD_CANDIDATES = (
+    [(e, w, "17 tasks", "unsupported") for e in _ENTRIES for w in (False, True)]
+    + [(e, w, "layout 5", "invalid") for e in _ENTRIES for w in (False, True)]
+    + [(e, w, "bit-packed rows", s) for (e, w), s in _BITS_STATUS.items()]
+    + [(e, w, "ldx too small", "invalid") for e in _ENTRIES for w in (False, True)]
+)
+
+
+@pytest.mark.parametrize("entry, wide, case, status", _BAD_CANDIDATES,
+                         ids=[f"{e}-{'wide' if w else 'resident'}-{c}" for e, w, c, _ in _BAD_CANDIDATES])
+def test_entry_points_reject_bad_candidates_before_any_cuda_call(lib, entry, wide, case, status):
+    import torch
+
+    from baybe_b200 import _lib
+
+    if torch.cuda.is_available():
+        pytest.skip("CUDA present: the fake device pointers must never reach a GPU")
+    m = _fake_model(wide, n_tasks=17 if case == "17 tasks" else 1)
+    layout, ldx = _lib.LAYOUT["row_f32"], m.d
+    if case == "layout 5":
+        layout = 5
+    elif case == "bit-packed rows":
+        layout, ldx = _lib.LAYOUT["bits_u8"], m.d // 8
+    elif case == "ldx too small":
+        ldx = m.d - 1
+    rc = _call_entry(lib, entry, m, layout, ldx)
+    msg = lib.bb_last_error()
+    assert rc == {"invalid": _lib.BB_ERR_INVALID, "unsupported": _lib.BB_ERR_UNSUPPORTED}[status], msg
+    if case == "17 tasks":
+        assert b"at most 16 tasks" in msg
+    else:
+        assert {"layout 5": b"layout 5", "bit-packed rows": b"bit-packed", "ldx too small": b"leading dimension"}[case] \
+            in msg
+
+
 def test_product_has_no_cpu_fallback():
     import torch
 
