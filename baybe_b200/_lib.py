@@ -18,8 +18,12 @@ HOST_FORMAT = {"rows_f32": 0, "rows_f64": 1, "codes4": 2, "codes8": 3}
 ACQ_KIND = {
     "qLogEI": 0, "qEI": 1, "qUCB": 2, "qSR": 3, "qPI": 4,
     "UCB": 5, "EI": 6, "LogEI": 7, "PI": 8, "PM": 9, "PSTD": 10,
+    "qEHVI": 11, "qLogEHVI": 12,
 }
-MC_KINDS = ("qLogEI", "qEI", "qUCB", "qSR", "qPI")
+MC_KINDS = ("qLogEI", "qEI", "qUCB", "qSR", "qPI", "qEHVI", "qLogEHVI")
+HVI_KINDS = ("qEHVI", "qLogEHVI")  # Pareto objectives: bb_hvi_score (baybe_b200/multiobjective.py)
+HVI_MAX_TARGETS = 4
+HVI_MAX_CELLS = 1024
 NEI_KINDS = ("qNEI",)  # evaluated by baybe_b200/hybrid.py (conditional form + bb_nei_reduce), not by the fused kernels
 MAX_PENDING = 31
 MAX_TRAIN = 1024
@@ -115,7 +119,9 @@ _SIGNATURES = {
     "bb_score_fused_overlapped": (C.c_int, [C.POINTER(Model), C.POINTER(AcqSpec), _vp, _i32, _i64, _i64, _vp, _i32, _vp,
                                             _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _i64, _vp, _vp]),
     "bb_nei_reduce": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _i64, _vp, _vp]),
-    "bb_decode_codes": (C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
+    "bb_hvi_score": (C.c_int, [C.POINTER(AcqSpec), _i32, C.POINTER(C.c_float), C.POINTER(C.c_float), _i64, _vp, _vp,
+                               _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp]),
+    "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),
     "bb_debug_posterior_simt": (C.c_int, [C.POINTER(Model), _vp, _i32, _i64, _i64, _vp, _vp, _vp]),

@@ -20,6 +20,7 @@ __all__ = [
     "UpperConfidenceBound", "qUpperConfidenceBound", "convert_acqf",
     "PM", "PSTD", "qSR", "EI", "qEI", "LogEI", "qLogEI", "PI", "qPI", "UCB", "qUCB",
     "qNoisyExpectedImprovement", "qNEI",
+    "qExpectedHypervolumeImprovement", "qEHVI", "qLogExpectedHypervolumeImprovement", "qLogEHVI",
 ]
 
 
@@ -186,12 +187,95 @@ class qNoisyExpectedImprovement(AcquisitionFunction):
     prune_baseline: bool = field(default=True, validator=instance_of(bool))
 
 
+def _reference_point(v):
+    if v is None:
+        return None
+    if isinstance(v, (int, float)):
+        return float(v)
+    return tuple(float(x) for x in v)
+
+
+@define(frozen=True)
+class _ExpectedHypervolumeImprovement(AcquisitionFunction):
+    """acquisition/acqfs.py:342-418: Pareto objectives of 2 to 4 targets, scored by ``bb_hvi_score``
+    (``baybe_b200.multiobjective``).  ``reference_point``: None (default factor 0.1), a factor, or coordinates in
+    the oriented objective space; ``alpha``: None or 0.0 (exact partitioning)."""
+
+    supports_multi_output: ClassVar[bool] = True
+    reference_point: float | tuple[float, ...] | None = field(default=None, converter=_reference_point)
+    alpha: float | None = field(default=None, converter=lambda v: None if v is None else float(v))
+
+    @staticmethod
+    def compute_ref_point(array, maximize=None, factor: float = 0.1):
+        from baybe_b200.multiobjective import compute_ref_point
+
+        return compute_ref_point(array, maximize, factor)
+
+    def to_engine(self, surrogate, searchspace, objective, measurements, pending_experiments=None) -> AcqConfig:
+        raise IncompatibleAcquisitionFunctionError(
+            f"'{type(self).__name__}' needs a multi-output objective; it is evaluated by "
+            "baybe_b200.multiobjective.HviScorer (see scorer())")
+
+    def scorer(self, surrogate, searchspace, objective, measurements):
+        """Fit the per-target surrogates (a ``CompositeSurrogate``, surrogates/composite.py:96) and set up the
+        reference point and the partitioning of the posterior-mean front."""
+        from baybe_b200.multiobjective import _error, build_hvi_scorer
+
+        if not getattr(objective, "is_multi_output", False):
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
+        kind = getattr(getattr(searchspace, "type", None), "name", "DISCRETE")
+        if kind != "DISCRETE":
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
+        surrogate.fit(searchspace, objective, measurements)
+        gps = [s.device_gp for s in surrogate._surrogates_flat]
+        return build_hvi_scorer(self, gps, searchspace, objective, measurements)
+
+    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
+                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
+        import numpy as np
+
+        from baybe_b200._lib import MAX_PENDING
+        from baybe_b200.engine import DEFAULT_MC_SAMPLES
+        from baybe_b200.recommenders import _draw_sampler_seed
+
+        scorer = self.scorer(surrogate, searchspace, objective, measurements)
+        rows = searchspace.transform(candidates, allow_extra=True).to_numpy(dtype="float64")
+        pend = None
+        if pending_experiments is not None and len(pending_experiments) > 0:
+            pend = searchspace.transform(pending_experiments, allow_extra=True).to_numpy(dtype="float64")
+        seed = _draw_sampler_seed()
+        if jointly:  # candidate first, then the rest of the batch and the pending points
+            rest = rows[1:] if pend is None else np.concatenate([rows[1:], pend], axis=0)
+            if len(rest) > MAX_PENDING:
+                raise NotImplementedError(f"joint evaluation supports at most {MAX_PENDING + 1} points")
+            return float(scorer.scores(rows[:1], rest if len(rest) else None, seed, DEFAULT_MC_SAMPLES)[0])
+        return pd.Series(scorer.scores(rows, pend, seed, DEFAULT_MC_SAMPLES), index=candidates.index)
+
+
+@define(frozen=True)
+class qExpectedHypervolumeImprovement(_ExpectedHypervolumeImprovement):
+    """acquisition/acqfs.py:421-434."""
+
+    abbreviation: ClassVar[str] = "qEHVI"
+
+
+@define(frozen=True)
+class qLogExpectedHypervolumeImprovement(_ExpectedHypervolumeImprovement):
+    """acquisition/acqfs.py:437-451; tau_relu = 1e-6 and tau_max = 1e-2 as in ``AcqConfig``."""
+
+    abbreviation: ClassVar[str] = "qLogEHVI"
+
+
 qNEI = qNoisyExpectedImprovement
+qEHVI, qLogEHVI = qExpectedHypervolumeImprovement, qLogExpectedHypervolumeImprovement
 PM, PSTD, qSR = PosteriorMean, PosteriorStandardDeviation, qSimpleRegret
 EI, qEI, LogEI, qLogEI = ExpectedImprovement, qExpectedImprovement, LogExpectedImprovement, qLogExpectedImprovement
 PI, qPI, UCB, qUCB = ProbabilityOfImprovement, qProbabilityOfImprovement, UpperConfidenceBound, qUpperConfidenceBound
 
-_BY_NAME = {c.__name__: c for c in (PM, PSTD, qSR, EI, qEI, LogEI, qLogEI, PI, qPI, UCB, qUCB, qNEI)}
+_BY_NAME = {c.__name__: c for c in (PM, PSTD, qSR, EI, qEI, LogEI, qLogEI, PI, qPI, UCB, qUCB, qNEI, qEHVI,
+                                    qLogEHVI)}
 _BY_NAME.update({c.abbreviation: c for c in list(_BY_NAME.values())})
 
 

@@ -37,6 +37,7 @@ from baybe.exceptions import (IncompatibilityError, IncompatibleAcquisitionFunct
 from baybe.recommenders.pure.bayesian.base import BayesianRecommender
 from baybe.searchspace import SearchSpaceType
 
+from baybe_b200 import _lib
 from baybe_b200 import acquisition as _acq
 from baybe_b200.engine import DEFAULT_MC_SAMPLES, sobol_normal_samples
 from baybe_b200.recommenders import _draw_sampler_seed, recommend_discrete_positions
@@ -66,11 +67,12 @@ class EngineAcquisitionFunction:
     """The acquisition callable BayBE hands around (``recommender._botorch_acqf``): ``acqf(X)`` with ``X`` of shape
     ``[b, q, d]`` (un-scaled comp-rep) returns ``[b]`` joint values of ``[X_b ; X_pending]``."""
 
-    def __init__(self, surrogate: GaussianProcessSurrogate, cfg, n_mc_samples: int, X_pending=None):
+    def __init__(self, surrogate: GaussianProcessSurrogate, cfg, n_mc_samples: int, X_pending=None, hvi=None):
         self.model = surrogate
         self.cfg = cfg
         self.n_mc_samples = n_mc_samples
         self.X_pending = X_pending
+        self.hvi = hvi  # multi-output objectives: the baybe_b200.multiobjective.HviScorer
         self.seed = _draw_sampler_seed()  # botorch samplers draw their seed once, at construction
 
     def set_X_pending(self, X_pending=None) -> None:
@@ -80,8 +82,16 @@ class EngineAcquisitionFunction:
         if X.dim() == 2:
             X = X.unsqueeze(0)
         b, q, d = X.shape
-        gp = self.model.device_gp
         pend = None if self.X_pending is None else torch.as_tensor(self.X_pending).reshape(-1, d)
+        if self.hvi is not None:
+            if q == 1 and (pend is None or len(pend) == 0):
+                return torch.from_numpy(self.hvi.scores(X[:, 0, :], None, self.seed, self.n_mc_samples))
+            out = torch.empty(b, dtype=torch.float64)
+            for i in range(b):
+                rest = X[i, 1:, :] if pend is None else torch.cat([X[i, 1:, :], pend.to(X)], dim=0)
+                out[i] = float(self.hvi.scores(X[i, :1, :], rest.cpu().numpy(), self.seed, self.n_mc_samples)[0])
+            return out
+        gp = self.model.device_gp
         if q == 1 and (pend is None or len(pend) == 0):
             z = sobol_normal_samples(self.n_mc_samples, 1, self.seed)[:, 0] if self.cfg.is_mc else None
             scores, _ = gp.score(self.cfg, X[:, 0, :], z)
@@ -113,6 +123,8 @@ class B200BotorchRecommender(BayesianRecommender):
     """As ``BotorchRecommender.max_n_subsets`` (botorch/core.py:101-105)."""
 
     _context = field(default=None, init=False, eq=False, repr=False)
+    _hvi = field(default=None, init=False, eq=False, repr=False)
+    """Multi-output objectives: the ``HviScorer`` set up by ``_setup_botorch_acqf``."""
     _last_acq_values: list = field(factory=list, init=False, eq=False, repr=False)
 
     # ---- multi-target objectives (SURVEY.md 8f-4, surrogates/composite.py:59-181) ------------------------------
@@ -121,8 +133,8 @@ class B200BotorchRecommender(BayesianRecommender):
         (``bayesian/base.py:35-39``); the engine surrogate is a duck-typed ``SurrogateProtocol``, so the same
         replication is done here -- with BayBE's OWN ``CompositeSurrogate``, which only needs ``fit`` and
         ``posterior_stats`` of its members.  ``Campaign.posterior_stats`` / ``get_surrogate`` then work for Pareto and
-        desirability objectives; recommending still needs a multi-output acquisition function (not implemented:
-        ``_setup_botorch_acqf`` raises ``IncompatibleAcquisitionFunctionError``)."""
+        desirability objectives; Pareto objectives recommend with qEHVI / qLogEHVI (``baybe_b200.multiobjective``),
+        every other multi-output acquisition function raises ``IncompatibleAcquisitionFunctionError``."""
         if objective.is_multi_output and isinstance(self._surrogate_model, GaussianProcessSurrogate):
             from baybe.surrogates.composite import CompositeSurrogate
 
@@ -133,20 +145,27 @@ class B200BotorchRecommender(BayesianRecommender):
     def _setup_botorch_acqf(self, searchspace, objective, measurements, pending_experiments=None) -> None:
         self._objective = objective
         acqf = self._get_acquisition_function(objective)
+        self._hvi = None
         if objective.is_multi_output:
-            raise IncompatibleAcquisitionFunctionError(
-                "recommending for multi-output objectives needs a multi-output acquisition function (qLogNEHVI, "
-                "bayesian/base.py:73), which the B200 engine does not implement; the per-target surrogates are "
-                "available through Campaign.get_surrogate / posterior_stats")
+            if getattr(type(acqf), "abbreviation", None) not in _lib.HVI_KINDS:
+                raise IncompatibleAcquisitionFunctionError(
+                    f"recommending for multi-output objectives on the B200 engine needs "
+                    f"qExpectedHypervolumeImprovement (qEHVI) or qLogExpectedHypervolumeImprovement (qLogEHVI); "
+                    f"'{type(acqf).__name__}' is not implemented (the default for multi-output objectives is "
+                    f"qLogNEHVI, bayesian/base.py:73)")
         surrogate = self.get_surrogate(searchspace, objective, measurements)
-        cfg = mirror_acquisition_function(acqf).to_engine(surrogate, searchspace, objective, measurements,
-                                                          pending_experiments)
+        spec = mirror_acquisition_function(acqf)
+        if objective.is_multi_output:
+            self._hvi = spec.scorer(surrogate, searchspace, objective, measurements)
+            cfg = self._hvi.cfg
+        else:
+            cfg = spec.to_engine(surrogate, searchspace, objective, measurements, pending_experiments)
         self._context = (cfg, searchspace, pending_experiments)
         pend = None
         if pending_experiments is not None and len(pending_experiments) > 0:
             pend = torch.from_numpy(searchspace.transform(pending_experiments, allow_extra=True)
                                     .to_numpy(dtype=np.float64))
-        self._botorch_acqf = EngineAcquisitionFunction(surrogate, cfg, self.n_mc_samples, pend)
+        self._botorch_acqf = EngineAcquisitionFunction(surrogate, cfg, self.n_mc_samples, pend, hvi=self._hvi)
 
     # ---- the PureRecommender hook (exact reference signature) ------------------------------------------------
     def _recommend_discrete(self, subspace_discrete, candidates_exp: pd.DataFrame, batch_size: int) -> pd.Index:
@@ -190,9 +209,9 @@ class B200BotorchRecommender(BayesianRecommender):
 
     def _recommend_discrete_without_subsets(self, subspace_discrete, candidates_exp, batch_size) -> pd.Index:
         cfg, searchspace, pending = self._context
-        return recommend_discrete_positions(self._surrogate_model.device_gp, cfg, subspace_discrete, candidates_exp,
-                                            batch_size, searchspace, pending, self.n_mc_samples,
-                                            self._last_acq_values)
+        gp = self._hvi if self._hvi is not None else self._surrogate_model.device_gp
+        return recommend_discrete_positions(gp, cfg, subspace_discrete, candidates_exp, batch_size, searchspace,
+                                            pending, self.n_mc_samples, self._last_acq_values)
 
     def _recommend_discrete_with_subsets(self, subspace_discrete, candidates_exp, batch_size) -> pd.Index:
         """``recommend_discrete_with_subsets`` (botorch/discrete.py:21-75): optimise inside every feasible subset,

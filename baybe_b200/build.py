@@ -18,7 +18,7 @@ OUT_DIR = PKG / "_C"
 LIB_PATH = OUT_DIR / "libbaybe_b200.so"
 STAMP = OUT_DIR / "build.stamp"
 
-SOURCES = ["model.cu", "fused.cu", "wide.cu", "aux_kernels.cu", "acq.cu", "peer.cu", "stream.cu"]
+SOURCES = ["model.cu", "fused.cu", "wide.cu", "aux_kernels.cu", "acq.cu", "mo.cu", "peer.cu", "stream.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",

@@ -89,9 +89,7 @@ struct JointParams {
 
 __device__ __forceinline__ float log_fatplus_f(float x, float tau) {
   // log( tau * (softplus(t) + 0.1/(1+t^2)) ), t = x/tau
-  const float t = x / tau;
-  const float sp = fmaxf(t, 0.f) + ((fabsf(t) < 30.f) ? softplus_tail(fabsf(t)) : 0.f);
-  return logf(tau) + logf(sp + 0.1f / fmaf(t, t, 1.0f));
+  return logf(tau) + log_fatplus_t(x / tau);
 }
 
 __global__ void __launch_bounds__(256) k_acq_joint(const JointParams p) {

@@ -19,6 +19,12 @@ __device__ __forceinline__ float softplus_tail(float abs_t) {
   return log1pf(e);
 }
 
+// log(fatplus(x, tau) / tau) = log(softplus(t) + 0.1/(1+t^2)) at t = x/tau (botorch fatplus, alpha = 0.1).
+__device__ __forceinline__ float log_fatplus_t(float t) {
+  const float sp = fmaxf(t, 0.f) + ((fabsf(t) < 30.f) ? softplus_tail(fabsf(t)) : 0.f);
+  return logf(sp + 0.1f / fmaf(t, t, 1.0f));
+}
+
 // One Monte-Carlo sample contributes to two running sums; t = c0 + c1 * z_s with
 //   qLogEI: t = (o_s - best_f)/tau_relu ; s0 += softplus(t) ; s1 += 1/(1+t^2)
 //   qEI   : t = o_s - best_f            ; s0 += relu(t)

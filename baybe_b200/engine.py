@@ -608,6 +608,45 @@ def _(x, keep, z, handle, kind, params, index_offset, want_scores):
             x.new_empty(1, dtype=torch.int64))
 
 
+@torch.library.custom_op("baybe_b200::hvi_score", mutates_args=())
+def _op_hvi_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | None, linv: torch.Tensor | None,
+                  w: torch.Tensor | None, z: torch.Tensor, lower: torch.Tensor, upper: torch.Tensor,
+                  n_cells: torch.Tensor, keep: torch.Tensor | None, kind: int, params: list[float],
+                  obj_scale: list[float], obj_shift: list[float], index_offset: int,
+                  want_scores: bool) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_hvi_score``: mu/var [M, N]; with P pending points cross [M, N, P], linv [M, P, P] (L_PP^-1), w [M, S, P];
+    z [S, M(1+P)]; cells lower/upper [n_dec, C, M] float32 with counts n_cells [n_dec] int32."""
+    acq = AcqConfig.from_params(kind, params).to_c()
+    M, N = mu.shape
+    P = 0 if cross is None else cross.shape[2]
+    S = z.shape[0]
+    if z.dim() != 2 or z.shape[1] != M * (1 + P):
+        raise ValueError(f"base samples must be (S, {M * (1 + P)})")
+    if lower.shape != upper.shape or lower.dim() != 3 or lower.shape[2] != M or n_cells.numel() != lower.shape[0] \
+            or n_cells.dtype != torch.int32 or lower.shape[0] != (1 if P == 0 else S):
+        raise ValueError("cells must be lower/upper [n_dec, C, M] with n_cells [n_dec] (n_dec = 1 or S)")
+    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
+        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
+    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
+    key = torch.empty(1, dtype=torch.int64, device=mu.device)
+    fa = (C.c_float * M)(*obj_scale)
+    fb = (C.c_float * M)(*obj_shift)
+    lib = _lib.load()
+    with torch.cuda.device(mu.device):
+        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        _lib.check(lib.bb_hvi_score(C.byref(acq), M, fa, fb, N, _ptr(mu), _ptr(var), P, _ptr(cross), _ptr(linv),
+                                    _ptr(w), _ptr(z), S, _ptr(lower), _ptr(upper), _ptr(n_cells), lower.shape[1],
+                                    _ptr(keep), _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
+                                    _stream_ptr()), "bb_hvi_score")
+    return score, key
+
+
+@_op_hvi_score.register_fake
+def _(mu, var, cross, linv, w, z, lower, upper, n_cells, keep, kind, params, obj_scale, obj_shift, index_offset,
+      want_scores):
+    return (mu.new_empty(mu.shape[1] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
+
+
 @torch.library.custom_op("baybe_b200::argmax", mutates_args=())
 def _op_argmax(score: torch.Tensor, keep: torch.Tensor | None, index_offset: int) -> torch.Tensor:
     key = torch.empty(1, dtype=torch.int64, device=score.device)

@@ -166,14 +166,20 @@ def greedy_select(gp: DeviceGP, cfg: AcqConfig, x_shard: torch.Tensor, d: int, q
                   offset: int = 0, keep_init: torch.Tensor | None = None) -> tuple[list[int], list[float]]:
     """Sequential greedy selection of q rows (global positions) -- ``optimize_acqf_discrete`` with
     ``unique=True``.  `x_shard` holds this rank's rows [offset, offset+len) on the device; the features of each
-    round's winner are fetched from the rank that owns it (``_winner_row``)."""
+    round's winner are fetched from the rank that owns it (``_winner_row``).  A `gp` with a ``round_best`` method
+    (``baybe_b200.multiobjective.HviScorer``) scores a round itself and maps the winner's key value to the
+    reported acquisition value."""
     chosen: list[int] = []
     values: list[float] = []
     keep = (torch.ones(x_shard.shape[0], dtype=torch.uint8, device=x_shard.device)
             if keep_init is None else keep_init.to(device=x_shard.device, dtype=torch.uint8).clone())
     pend = np.zeros((0, d)) if base_pending is None else np.asarray(base_pending, dtype=np.float64).reshape(-1, d)
+    round_best = getattr(gp, "round_best", None)
     for r in range(q):
-        if len(pend) == 0:
+        report = None
+        if round_best is not None:
+            key, report = round_best(x_shard, pend, keep, offset, seed, n_samples)
+        elif len(pend) == 0:
             z = sobol_normal_samples(n_samples, 1, seed)[:, 0] if cfg.is_mc else None
             _, key = gp.score(cfg, x_shard, z, keep=keep, index_offset=offset, want_scores=False)
         else:
@@ -185,7 +191,7 @@ def greedy_select(gp: DeviceGP, cfg: AcqConfig, x_shard: torch.Tensor, d: int, q
         if idx < 0:
             raise NotEnoughPointsLeftError("no eligible candidate left to recommend")
         chosen.append(idx)
-        values.append(val)
+        values.append(val if report is None else report(val))
         if offset <= idx < offset + x_shard.shape[0]:
             keep[idx - offset] = 0
         if r + 1 < q:

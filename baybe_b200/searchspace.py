@@ -202,7 +202,12 @@ def objective_affine(objective) -> tuple[float, float, str]:
     targets = getattr(objective, "targets", None)
     if targets is None or len(targets) != 1:
         raise NotImplementedError("only single-target objectives are supported by the B200 engine")
-    t = targets[0]
+    a, b = target_affine(targets[0])
+    return a, b, targets[0].name
+
+
+def target_affine(t) -> tuple[float, float]:
+    """(a, b) of one target oriented for maximisation, o = a*y + b (Identity/Affine transformations only)."""
     a, b = 1.0, 0.0
     tr = getattr(t, "transformation", None)
     if tr is not None:
@@ -214,4 +219,4 @@ def objective_affine(objective) -> tuple[float, float, str]:
                 f"target transformation {name} is not affine; fall back to the reference path")
     if getattr(t, "minimize", False):
         a, b = -a, -b
-    return a, b, t.name
+    return a, b

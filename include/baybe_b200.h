@@ -72,7 +72,9 @@ typedef enum bb_acq_kind {
   BB_ACQ_LOGEI = 7,  /* LogExpectedImprovement    acqfs.py:213 */
   BB_ACQ_PI = 8,     /* ProbabilityOfImprovement  acqfs.py:249 */
   BB_ACQ_PM = 9,     /* PosteriorMean             acqfs.py:162 */
-  BB_ACQ_PSTD = 10   /* PosteriorStandardDeviation acqfs.py:169 */
+  BB_ACQ_PSTD = 10,  /* PosteriorStandardDeviation acqfs.py:169 */
+  BB_ACQ_QEHVI = 11,   /* qExpectedHypervolumeImprovement    acqfs.py:430 (bb_hvi_score only) */
+  BB_ACQ_QLOGEHVI = 12 /* qLogExpectedHypervolumeImprovement acqfs.py:448 (bb_hvi_score only) */
 } bb_acq_kind;
 
 #define BB_MAX_PENDING 31 /* max pending points in a joint (q>1) evaluation */
@@ -342,6 +344,29 @@ int bb_score_fused_overlapped(const bb_model* m, const bb_acq_spec* a, const voi
 int bb_nei_reduce(const float* d_out, int64_t ld, int32_t S, int32_t m, const float* d_mu, const float* d_var,
                   const float* d_zx, const float* d_g, float obj_scale, float obj_shift, int64_t N, float* d_score,
                   void* stream);
+
+/* ---- hypervolume improvement of one new point per candidate for a Pareto objective of M targets
+ * (qExpectedHypervolumeImprovement / qLogExpectedHypervolumeImprovement, baybe/acquisition/acqfs.py:430-465; reference
+ * point and partitioning from acquisition/_builder.py:286-317, both built on the host by baybe_b200/multiobjective.py).
+ * Kind BB_ACQ_QEHVI or BB_ACQ_QLOGEHVI (a->tau_relu / a->tau_max smooth the latter); a->obj_scale / obj_shift are not
+ * used: obj_scale[M] / obj_shift[M] (HOST arrays) orient each target, o_m = obj_scale[m] * y_m + obj_shift[m].
+ *   d_mu / d_var [M][N]: marginal posterior of every candidate per target (bb_posterior, one model per target).
+ *   n_pending = P in [0, BB_MAX_PENDING].  With P > 0: d_cross [M][N][P] (bb_posterior's cross covariance),
+ *     d_linv [M][P][P] = L_PP^-1 (row-major, lower triangular) and d_w [M][S][P] = L_PP^-T z_P of each target (pending Cholesky L_PP L_PP^T = K_PP).
+ *   d_z [S][M(1+P)]: base samples; column m(1+P)+j is pending point j of target m, column m(1+P)+P the candidate.
+ *   Cells: d_lower / d_upper [n_dec][cell_stride][M], d_n_cells [n_dec] (entries above cell_stride are clamped);
+ *     n_dec = 1 (one decomposition of the front F, shared by all samples) for P = 0, else S (F u P_s per sample).
+ *     An upper bound of +inf leaves that side open.  cell_stride <= BB_HVI_MAX_CELLS.
+ * Writes the improvement of x over the cells (the pending points' own improvement is the caller's candidate-
+ * independent term) to d_score (nullable), and folds d_keep (nullable) and index_offset into *d_best_key like
+ * bb_argmax (initialise with bb_best_init).  S <= 1024; 2 <= M <= BB_HVI_MAX_TARGETS. */
+#define BB_HVI_MAX_TARGETS 4
+#define BB_HVI_MAX_CELLS 1024
+int bb_hvi_score(const bb_acq_spec* a, int32_t n_targets, const float* obj_scale, const float* obj_shift, int64_t N,
+                 const float* d_mu, const float* d_var, int32_t n_pending, const float* d_cross, const float* d_linv,
+                 const float* d_w, const float* d_z, int32_t S, const float* d_lower, const float* d_upper,
+                 const int32_t* d_n_cells, int32_t cell_stride, const uint8_t* d_keep, float* d_score,
+                 int64_t* d_best_key, int64_t index_offset, void* stream);
 
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
