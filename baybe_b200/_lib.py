@@ -76,6 +76,21 @@ class AcqSpec(C.Structure):
     ]
 
 
+OBJ_MAX_TARGETS, OBJ_MAX_OPS, OBJ_MAX_STACK = 8, 32, 4
+OBJ_OP = {"AFFINE": 0, "CONST": 1, "CLAMP": 2, "TWO_SIDED": 3, "BELL": 4, "LOG": 5, "EXP": 6, "POW_INT": 7,
+          "SIGMOID": 8, "DUP_INPUT": 9, "ADD": 10, "MUL": 11}
+OBJ_SCALARIZER = {"NONE": 0, "MEAN": 1, "GEOM_MEAN": 2}
+
+
+class ObjInstr(C.Structure):
+    _fields_ = [("op", C.c_int32), ("arg", C.c_float * 3)]
+
+
+class Objective(C.Structure):
+    _fields_ = [("n_targets", C.c_int32), ("scalarizer", C.c_int32), ("n_ops", C.c_int32 * OBJ_MAX_TARGETS),
+                ("weight", C.c_float * OBJ_MAX_TARGETS), ("prog", (ObjInstr * OBJ_MAX_OPS) * OBJ_MAX_TARGETS)]
+
+
 class Best(C.Structure):
     _fields_ = [("val", C.c_float), ("pad_", C.c_int32), ("idx", C.c_int64)]
 
@@ -121,6 +136,8 @@ _SIGNATURES = {
     "bb_nei_reduce": (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _i64, _vp, _vp]),
     "bb_hvi_score": (C.c_int, [C.POINTER(AcqSpec), _i32, C.POINTER(C.c_float), C.POINTER(C.c_float), _i64, _vp, _vp,
                                _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp]),
+    "bb_objective_score": (C.c_int, [C.POINTER(AcqSpec), C.POINTER(Objective), _i64, _vp, _vp, _i32, _vp, _vp, _vp,
+                                     _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),

@@ -58,12 +58,17 @@ class AcquisitionFunction:
                   pending_experiments: pd.DataFrame | None = None) -> AcqConfig:
         """Counterpart of ``to_botorch`` (acquisition/base.py:61-84): resolve the context
         (objective orientation, best_f) into the engine's acquisition config."""
+        from baybe_b200.objectives import uses_objective_scorer
         from baybe_b200.searchspace import objective_affine
 
         if pending_experiments is not None and not self.supports_pending_experiments:
             raise IncompatibleAcquisitionFunctionError(
                 f"The chosen acquisition function of type '{type(self).__name__}' "
                 f"does not support pending experiments.")
+        if uses_objective_scorer(objective):
+            raise IncompatibleAcquisitionFunctionError(
+                f"'{type(objective).__name__}' is not affine in its targets; it is evaluated by "
+                "baybe_b200.objectives.ObjectiveScorer (see scorer())")
         a, b, _ = objective_affine(objective)
         cfg = AcqConfig(kind=self.abbreviation, obj_scale=a, obj_shift=b, **self._engine_kwargs())
         if self.abbreviation in ("qLogEI", "qEI", "qPI", "EI", "LogEI", "PI"):
@@ -78,8 +83,16 @@ class AcquisitionFunction:
         import torch
 
         from baybe_b200.engine import DEFAULT_MC_SAMPLES
+        from baybe_b200.objectives import uses_objective_scorer
         from baybe_b200.recommenders import _draw_sampler_seed, _scores_for
 
+        if uses_objective_scorer(objective):
+            if pending_experiments is not None and not self.supports_pending_experiments:
+                raise IncompatibleAcquisitionFunctionError(
+                    f"The chosen acquisition function of type '{type(self).__name__}' "
+                    f"does not support pending experiments.")
+            scorer = self.scorer(surrogate, searchspace, objective, measurements)
+            return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
         surrogate.fit(searchspace, objective, measurements)
         cfg = self.to_engine(surrogate, searchspace, objective, measurements, pending_experiments)
         comp = searchspace.transform(candidates, allow_extra=True)
@@ -109,6 +122,48 @@ class AcquisitionFunction:
             return float(surrogate.device_gp.score_joint(cfg, x[:1], rest, z)[0])
         scores = _scores_for(surrogate.device_gp, cfg, x, pend, seed, DEFAULT_MC_SAMPLES)
         return pd.Series(scores.double().cpu().numpy(), index=candidates.index)
+
+    def scorer(self, surrogate, searchspace, objective, measurements):
+        """Objectives that are not affine in their targets (desirability, non-affine single targets): fit the
+        surrogate -- one model per target through a ``CompositeSurrogate`` for desirability -- and set up best_f
+        and the compiled objective (``baybe_b200.objectives``)."""
+        from baybe_b200.objectives import build_objective_scorer
+
+        kind = getattr(getattr(searchspace, "type", None), "name", "DISCRETE")
+        if kind != "DISCRETE":
+            raise IncompatibleAcquisitionFunctionError(
+                f"'{type(objective).__name__}' with a non-affine objective is served on discrete search spaces only "
+                f"by the B200 engine (got {kind})")
+        surrogate.fit(searchspace, objective, measurements)
+        flat = getattr(surrogate, "_surrogates_flat", None)
+        gps = [s.device_gp for s in flat] if flat is not None else [surrogate.device_gp]
+        return build_objective_scorer(self, gps, searchspace, objective, measurements)
+
+
+def _evaluate_with_scorer(acqf, scorer, candidates: pd.DataFrame, searchspace, pending_experiments, jointly: bool):
+    """``evaluate`` through a scorer that runs its own rounds (``HviScorer``, ``ObjectiveScorer``): one value per
+    candidate, or the joint value of the batch [candidates; pending] with the first candidate scored against the
+    rest."""
+    import numpy as np
+
+    from baybe_b200._lib import MAX_PENDING
+    from baybe_b200.engine import DEFAULT_MC_SAMPLES
+    from baybe_b200.recommenders import _draw_sampler_seed
+
+    rows = searchspace.transform(candidates, allow_extra=True).to_numpy(dtype="float64")
+    pend = None
+    if pending_experiments is not None and len(pending_experiments) > 0:
+        pend = searchspace.transform(pending_experiments, allow_extra=True).to_numpy(dtype="float64")
+    seed = _draw_sampler_seed()
+    if jointly:  # candidate first, then the rest of the batch and the pending points
+        rest = rows[1:] if pend is None else np.concatenate([rows[1:], pend], axis=0)
+        if len(rest) and not scorer.cfg.is_mc:
+            raise IncompatibleAcquisitionFunctionError(
+                f"'{type(acqf).__name__}' is analytic and cannot value a batch of {len(rows)} points jointly.")
+        if len(rest) > MAX_PENDING:
+            raise NotImplementedError(f"joint evaluation supports at most {MAX_PENDING + 1} points")
+        return float(scorer.scores(rows[:1], rest if len(rest) else None, seed, DEFAULT_MC_SAMPLES)[0])
+    return pd.Series(scorer.scores(rows, pend, seed, DEFAULT_MC_SAMPLES), index=candidates.index)
 
 
 @define(frozen=True)
@@ -234,24 +289,8 @@ class _ExpectedHypervolumeImprovement(AcquisitionFunction):
 
     def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
                  pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
-        import numpy as np
-
-        from baybe_b200._lib import MAX_PENDING
-        from baybe_b200.engine import DEFAULT_MC_SAMPLES
-        from baybe_b200.recommenders import _draw_sampler_seed
-
         scorer = self.scorer(surrogate, searchspace, objective, measurements)
-        rows = searchspace.transform(candidates, allow_extra=True).to_numpy(dtype="float64")
-        pend = None
-        if pending_experiments is not None and len(pending_experiments) > 0:
-            pend = searchspace.transform(pending_experiments, allow_extra=True).to_numpy(dtype="float64")
-        seed = _draw_sampler_seed()
-        if jointly:  # candidate first, then the rest of the batch and the pending points
-            rest = rows[1:] if pend is None else np.concatenate([rows[1:], pend], axis=0)
-            if len(rest) > MAX_PENDING:
-                raise NotImplementedError(f"joint evaluation supports at most {MAX_PENDING + 1} points")
-            return float(scorer.scores(rows[:1], rest if len(rest) else None, seed, DEFAULT_MC_SAMPLES)[0])
-        return pd.Series(scorer.scores(rows, pend, seed, DEFAULT_MC_SAMPLES), index=candidates.index)
+        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
 
 
 @define(frozen=True)

@@ -67,12 +67,14 @@ class EngineAcquisitionFunction:
     """The acquisition callable BayBE hands around (``recommender._botorch_acqf``): ``acqf(X)`` with ``X`` of shape
     ``[b, q, d]`` (un-scaled comp-rep) returns ``[b]`` joint values of ``[X_b ; X_pending]``."""
 
-    def __init__(self, surrogate: GaussianProcessSurrogate, cfg, n_mc_samples: int, X_pending=None, hvi=None):
+    def __init__(self, surrogate: GaussianProcessSurrogate, cfg, n_mc_samples: int, X_pending=None, scorer=None):
         self.model = surrogate
         self.cfg = cfg
         self.n_mc_samples = n_mc_samples
         self.X_pending = X_pending
-        self.hvi = hvi  # multi-output objectives: the baybe_b200.multiobjective.HviScorer
+        # objectives the fused path does not serve: baybe_b200.multiobjective.HviScorer (Pareto) or
+        # baybe_b200.objectives.ObjectiveScorer (desirability, non-affine single targets)
+        self.scorer = scorer
         self.seed = _draw_sampler_seed()  # botorch samplers draw their seed once, at construction
 
     def set_X_pending(self, X_pending=None) -> None:
@@ -83,13 +85,15 @@ class EngineAcquisitionFunction:
             X = X.unsqueeze(0)
         b, q, d = X.shape
         pend = None if self.X_pending is None else torch.as_tensor(self.X_pending).reshape(-1, d)
-        if self.hvi is not None:
+        if self.scorer is not None:
             if q == 1 and (pend is None or len(pend) == 0):
-                return torch.from_numpy(self.hvi.scores(X[:, 0, :], None, self.seed, self.n_mc_samples))
+                return torch.from_numpy(self.scorer.scores(X[:, 0, :], None, self.seed, self.n_mc_samples))
+            if not self.scorer.cfg.is_mc:
+                raise IncompatibleAcquisitionFunctionError("analytic acquisition functions value single points only")
             out = torch.empty(b, dtype=torch.float64)
             for i in range(b):
                 rest = X[i, 1:, :] if pend is None else torch.cat([X[i, 1:, :], pend.to(X)], dim=0)
-                out[i] = float(self.hvi.scores(X[i, :1, :], rest.cpu().numpy(), self.seed, self.n_mc_samples)[0])
+                out[i] = float(self.scorer.scores(X[i, :1, :], rest.cpu().numpy(), self.seed, self.n_mc_samples)[0])
             return out
         gp = self.model.device_gp
         if q == 1 and (pend is None or len(pend) == 0):
@@ -123,8 +127,9 @@ class B200BotorchRecommender(BayesianRecommender):
     """As ``BotorchRecommender.max_n_subsets`` (botorch/core.py:101-105)."""
 
     _context = field(default=None, init=False, eq=False, repr=False)
-    _hvi = field(default=None, init=False, eq=False, repr=False)
-    """Multi-output objectives: the ``HviScorer`` set up by ``_setup_botorch_acqf``."""
+    _scorer = field(default=None, init=False, eq=False, repr=False)
+    """Objectives the fused path does not serve: the ``HviScorer`` (Pareto) or ``ObjectiveScorer`` (desirability,
+    non-affine single targets) set up by ``_setup_botorch_acqf``."""
     _last_acq_values: list = field(factory=list, init=False, eq=False, repr=False)
 
     # ---- multi-target objectives (SURVEY.md 8f-4, surrogates/composite.py:59-181) ------------------------------
@@ -132,10 +137,12 @@ class B200BotorchRecommender(BayesianRecommender):
         """The reference replicates single-output ``Surrogate`` subclasses per modelled quantity
         (``bayesian/base.py:35-39``); the engine surrogate is a duck-typed ``SurrogateProtocol``, so the same
         replication is done here -- with BayBE's OWN ``CompositeSurrogate``, which only needs ``fit`` and
-        ``posterior_stats`` of its members.  ``Campaign.posterior_stats`` / ``get_surrogate`` then work for Pareto and
-        desirability objectives; Pareto objectives recommend with qEHVI / qLogEHVI (``baybe_b200.multiobjective``),
-        every other multi-output acquisition function raises ``IncompatibleAcquisitionFunctionError``."""
-        if objective.is_multi_output and isinstance(self._surrogate_model, GaussianProcessSurrogate):
+        ``posterior_stats`` of its members.  This happens whenever the objective models more than one quantity
+        (``Objective._is_multi_model``: Pareto objectives and desirability objectives that are not applied as a
+        pre-transformation).  Pareto objectives recommend with qEHVI / qLogEHVI (``baybe_b200.multiobjective``),
+        desirability objectives with ``baybe_b200.objectives``."""
+        multi_model = getattr(objective, "_is_multi_model", objective.is_multi_output)
+        if multi_model and isinstance(self._surrogate_model, GaussianProcessSurrogate):
             from baybe.surrogates.composite import CompositeSurrogate
 
             self._surrogate_model = CompositeSurrogate.from_replication(self._surrogate_model)
@@ -144,8 +151,10 @@ class B200BotorchRecommender(BayesianRecommender):
     # ---- acquisition set-up: the engine config takes the place of the botorch acquisition function ----------
     def _setup_botorch_acqf(self, searchspace, objective, measurements, pending_experiments=None) -> None:
         self._objective = objective
+        from baybe_b200.objectives import uses_objective_scorer
+
         acqf = self._get_acquisition_function(objective)
-        self._hvi = None
+        self._scorer = None
         if objective.is_multi_output:
             if getattr(type(acqf), "abbreviation", None) not in _lib.HVI_KINDS:
                 raise IncompatibleAcquisitionFunctionError(
@@ -155,9 +164,13 @@ class B200BotorchRecommender(BayesianRecommender):
                     f"qLogNEHVI, bayesian/base.py:73)")
         surrogate = self.get_surrogate(searchspace, objective, measurements)
         spec = mirror_acquisition_function(acqf)
-        if objective.is_multi_output:
-            self._hvi = spec.scorer(surrogate, searchspace, objective, measurements)
-            cfg = self._hvi.cfg
+        if objective.is_multi_output or uses_objective_scorer(objective):
+            if pending_experiments is not None and not spec.supports_pending_experiments:
+                raise IncompatibleAcquisitionFunctionError(
+                    f"The chosen acquisition function of type '{type(spec).__name__}' "
+                    f"does not support pending experiments.")
+            self._scorer = spec.scorer(surrogate, searchspace, objective, measurements)
+            cfg = self._scorer.cfg
         else:
             cfg = spec.to_engine(surrogate, searchspace, objective, measurements, pending_experiments)
         self._context = (cfg, searchspace, pending_experiments)
@@ -165,7 +178,7 @@ class B200BotorchRecommender(BayesianRecommender):
         if pending_experiments is not None and len(pending_experiments) > 0:
             pend = torch.from_numpy(searchspace.transform(pending_experiments, allow_extra=True)
                                     .to_numpy(dtype=np.float64))
-        self._botorch_acqf = EngineAcquisitionFunction(surrogate, cfg, self.n_mc_samples, pend, hvi=self._hvi)
+        self._botorch_acqf = EngineAcquisitionFunction(surrogate, cfg, self.n_mc_samples, pend, scorer=self._scorer)
 
     # ---- the PureRecommender hook (exact reference signature) ------------------------------------------------
     def _recommend_discrete(self, subspace_discrete, candidates_exp: pd.DataFrame, batch_size: int) -> pd.Index:
@@ -209,7 +222,7 @@ class B200BotorchRecommender(BayesianRecommender):
 
     def _recommend_discrete_without_subsets(self, subspace_discrete, candidates_exp, batch_size) -> pd.Index:
         cfg, searchspace, pending = self._context
-        gp = self._hvi if self._hvi is not None else self._surrogate_model.device_gp
+        gp = self._scorer if self._scorer is not None else self._surrogate_model.device_gp
         return recommend_discrete_positions(gp, cfg, subspace_discrete, candidates_exp, batch_size, searchspace,
                                             pending, self.n_mc_samples, self._last_acq_values)
 

@@ -209,14 +209,7 @@ __global__ void __launch_bounds__(256) k_acq_joint(const JointParams p) {
         red = fmaxf(red, val);
       }
       if (a.kind == BB_ACQ_QLOGEI) {
-        // fatmax over the q points: M + tau * log sum (1 + (M - li)/(2 tau))^-2
-        float ssum = 0.f;
-        const float inv = 1.0f / (2.0f * a.tau_max);
-        for (int k = 0; k < Q; ++k) {
-          const float w = fmaf(red - li_arr[k], inv, 1.0f);
-          ssum += 1.0f / (w * w);
-        }
-        const float li = red + a.tau_max * logf(ssum);
+        const float li = fatmax_q(li_arr, Q, red, a.tau_max);  // fatmax over the q points
         if (li > run_max) {
           run_sum = run_sum * __expf(run_max - li) + 1.0f;
           run_max = li;

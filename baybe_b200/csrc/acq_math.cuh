@@ -25,6 +25,52 @@ __device__ __forceinline__ float log_fatplus_t(float t) {
   return logf(sp + 0.1f / fmaf(t, t, 1.0f));
 }
 
+// ---- conditional moments of a candidate given P pending points (one warp per candidate) ----------------------------
+// |L^-1 c|^2 with lane j holding c_j (0 for j >= P) and forming (L^-1 c)_j; linv: L_PP^-1 row-major [P][P], lower
+// triangular.  A sum of squares: no cancellation against var for nearly collinear pending points.  Every lane
+// takes part in the shuffles; the result is in every lane.
+__device__ __forceinline__ float pending_r2_warp(float c, const float* linv, int P, int lane) {
+  float acc = 0.f;
+  for (int k = 0; k < P; ++k) {
+    const float ck = __shfl_sync(0xffffffffu, c, k);
+    if (lane < P && k <= lane) acc = fmaf(linv[lane * P + k], ck, acc);
+  }
+  float r2 = acc * acc;
+  for (int o = 16; o > 0; o >>= 1) r2 += __shfl_xor_sync(0xffffffffu, r2, o);
+  return r2;
+}
+
+// c . w_s (lane j holds c_j; wr: the P entries of w_s = L_PP^-T z_{s,P} of this lane's sample).  Every lane takes
+// part in the shuffles.
+__device__ __forceinline__ float pending_cw_warp(float c, const float* wr, int P) {
+  float dm = 0.f;
+  for (int j = 0; j < P; ++j) dm = fmaf(__shfl_sync(0xffffffffu, c, j), __ldg(wr + j), dm);
+  return dm;
+}
+
+// botorch fatmax over the q values l[0..q) of one sample whose hard maximum is mx:
+// mx + tau * log sum_k (1 + (mx - l_k)/(2 tau))^-2
+__device__ __forceinline__ float fatmax_q(const float* l, int q, float mx, float tau_max) {
+  float ssum = 0.f;
+  const float inv = 1.0f / (2.0f * tau_max);
+  for (int k = 0; k < q; ++k) {
+    const float w = fmaf(mx - l[k], inv, 1.0f);
+    ssum += 1.0f / (w * w);
+  }
+  return mx + tau_max * logf(ssum);
+}
+
+// online logsumexp: (mx, sum) holds log sum_k exp(v_k) = mx + log(sum); -inf / NaN values are skipped
+__device__ __forceinline__ void lse_push(float v, float& mx, float& sum) {
+  if (!(v > -INFINITY)) return;
+  if (v > mx) {
+    sum = sum * __expf(mx - v) + 1.0f;
+    mx = v;
+  } else {
+    sum += __expf(v - mx);
+  }
+}
+
 // One Monte-Carlo sample contributes to two running sums; t = c0 + c1 * z_s with
 //   qLogEI: t = (o_s - best_f)/tau_relu ; s0 += softplus(t) ; s1 += 1/(1+t^2)
 //   qEI   : t = o_s - best_f            ; s0 += relu(t)

@@ -44,16 +44,6 @@ __device__ __forceinline__ float fatmin_f(float y, float u, float half_inv_tau, 
   return fminf(y, u) - tau * __logf(1.0f + 1.0f / (w * w));
 }
 
-__device__ __forceinline__ void lse_push(float v, float& mx, float& sum) {
-  if (!(v > -INFINITY)) return;
-  if (v > mx) {
-    sum = sum * __expf(mx - v) + 1.0f;
-    mx = v;
-  } else {
-    sum += __expf(v - mx);
-  }
-}
-
 constexpr int kHviThreads = 256;
 
 template <int M, bool LOG>
@@ -92,15 +82,8 @@ __global__ void __launch_bounds__(kHviThreads) k_hvi(const HviParams p) {
       float r2 = 0.f;
       cm[m] = 0.f;
       if (P > 0) {
-        // |r|^2 = |L^-1 c|^2: lane j holds c_j and forms (L^-1 c)_j (L^-1 lower triangular)
         cm[m] = (lane < P) ? __ldg(p.cross + ((size_t)m * p.N + i) * P + lane) : 0.f;
-        float acc = 0.f;
-        for (int k = 0; k < P; ++k) {
-          const float ck = __shfl_sync(0xffffffffu, cm[m], k);
-          if (lane < P && k <= lane) acc = fmaf(linv[(m * P + lane) * P + k], ck, acc);
-        }
-        r2 = acc * acc;
-        for (int o = 16; o > 0; o >>= 1) r2 += __shfl_xor_sync(0xffffffffu, r2, o);
+        r2 = pending_r2_warp(cm[m], linv + m * P * P, P, lane);
       }
       sd[m] = sqrtf(fmaxf(v - r2, 0.f));
     }
@@ -112,10 +95,7 @@ __global__ void __launch_bounds__(kHviThreads) k_hvi(const HviParams p) {
 #pragma unroll
       for (int m = 0; m < M; ++m) {
         float dm = 0.f;
-        if (P > 0) {  // every lane takes part in the shuffles
-          const float* wr = p.w + ((size_t)m * S + (valid ? s : 0)) * P;
-          for (int j = 0; j < P; ++j) dm = fmaf(__shfl_sync(0xffffffffu, cm[m], j), __ldg(wr + j), dm);
-        }
+        if (P > 0) dm = pending_cw_warp(cm[m], p.w + ((size_t)m * S + (valid ? s : 0)) * P, P);
         const float zz = valid ? zc[s * M + m] : 0.f;
         y[m] = fmaf(p.a[m], mu[m] + dm + sd[m] * zz, p.b[m]);
       }

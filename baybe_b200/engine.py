@@ -647,6 +647,66 @@ def _(mu, var, cross, linv, w, z, lower, upper, n_cells, keep, kind, params, obj
     return (mu.new_empty(mu.shape[1] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
 
 
+def objective_struct(n_targets: int, scalarizer: int, programs, weights) -> _lib.Objective:
+    """``bb_objective`` from per-target programs [(opcode, (arg0, arg1, arg2)), ...] (baybe_b200/objectives.py)."""
+    obj = _lib.Objective()
+    obj.n_targets, obj.scalarizer = int(n_targets), int(scalarizer)
+    if len(programs) > _lib.OBJ_MAX_TARGETS:
+        raise ValueError(f"at most {_lib.OBJ_MAX_TARGETS} target programs")
+    for m, prog in enumerate(programs):
+        if len(prog) > _lib.OBJ_MAX_OPS:
+            raise ValueError(f"at most {_lib.OBJ_MAX_OPS} ops per target")
+        obj.n_ops[m] = len(prog)
+        obj.weight[m] = float(weights[m])
+        for i, (op, args) in enumerate(prog):
+            obj.prog[m][i].op = int(op)
+            for k, v in enumerate(args):
+                obj.prog[m][i].arg[k] = float(v)
+    return obj
+
+
+@torch.library.custom_op("baybe_b200::objective_score", mutates_args=())
+def _op_objective_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | None, linv: torch.Tensor | None,
+                        w: torch.Tensor | None, pend_terms: torch.Tensor | None, z: torch.Tensor | None,
+                        keep: torch.Tensor | None, kind: int, params: list[float], scalarizer: int,
+                        ops: list[int], args: list[float], n_ops: list[int], weights: list[float], index_offset: int,
+                        want_scores: bool) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_objective_score``: mu/var [M, N]; with P pending points cross [M, N, P], linv [M, P, P], w [M, S, P] and
+    pend_terms [S, P]; z [S, M(1+P)] (None for analytic kinds).  The programs come flattened: target m owns n_ops[m]
+    consecutive entries of ops (opcodes) and of args (three floats each)."""
+    acq = AcqConfig.from_params(kind, params).to_c()
+    M, N = mu.shape
+    P = 0 if cross is None else cross.shape[2]
+    S = 0 if z is None else z.shape[0]
+    if z is not None and (z.dim() != 2 or z.shape[1] != M * (1 + P)):
+        raise ValueError(f"base samples must be (S, {M * (1 + P)})")
+    if P and (pend_terms is None or tuple(pend_terms.shape) != (S, P)):
+        raise ValueError(f"pending terms must be (S, P) = ({S}, {P})")
+    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
+        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
+    progs, k = [], 0
+    for n in n_ops:
+        progs.append([(ops[k + i], args[3 * (k + i): 3 * (k + i) + 3]) for i in range(n)])
+        k += n
+    obj = objective_struct(M, scalarizer, progs, weights)
+    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
+    key = torch.empty(1, dtype=torch.int64, device=mu.device)
+    lib = _lib.load()
+    with torch.cuda.device(mu.device):
+        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        _lib.check(lib.bb_objective_score(C.byref(acq), C.byref(obj), N, _ptr(mu), _ptr(var), P, _ptr(cross),
+                                          _ptr(linv), _ptr(w), _ptr(pend_terms), _ptr(z), S, _ptr(keep),
+                                          _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
+                                          _stream_ptr()), "bb_objective_score")
+    return score, key
+
+
+@_op_objective_score.register_fake
+def _(mu, var, cross, linv, w, pend_terms, z, keep, kind, params, scalarizer, ops, args, n_ops, weights, index_offset,
+      want_scores):
+    return (mu.new_empty(mu.shape[1] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
+
+
 @torch.library.custom_op("baybe_b200::argmax", mutates_args=())
 def _op_argmax(score: torch.Tensor, keep: torch.Tensor | None, index_offset: int) -> torch.Tensor:
     key = torch.empty(1, dtype=torch.int64, device=score.device)

@@ -173,20 +173,11 @@ class HviScorer:
     def _pending_parts(self, pend: np.ndarray, z: torch.Tensor):
         """Per target: cross-covariance inputs, L_PP^-1 and L^-T z_P; per sample: decomposition of F u P_s and
         the exact improvement of P_s over F.  z: (S, M(1+P)) float64."""
-        P, M, S = len(pend), self.M, z.shape[0]
-        Q = P + 1
-        stats, linv, w = [], np.zeros((M, P, P)), np.zeros((M, S, P))
-        ps = np.zeros((S, P, M))
-        for m, gp in enumerate(self.gps):
-            px, beta, pmu, pcov = gp.pending_stats(pend)
-            stats.append((px, beta))
-            K = pcov.double().cpu().numpy()
-            L = _psd_cholesky(K)
-            Linv = np.linalg.inv(L)
-            linv[m] = Linv
-            zp = z[:, m * Q: m * Q + P].numpy()
-            w[m] = zp @ Linv  # rows: (L^-T z_s)^T
-            ps[:, :, m] = self.a[m] * (pmu.double().cpu().numpy()[None, :] + zp @ L.T) + self.b[m]
+        from baybe_b200.objectives import pending_conditioning
+
+        S = z.shape[0]
+        stats, linv, w, ys = pending_conditioning(self.gps, pend, z)
+        ps = self.a * ys + self.b
         decomps, gain = [], np.zeros(S)
         for s in range(S):
             lo, hi, hv = box_decomposition(np.concatenate([self.front, ps[s]], axis=0), self.ref)

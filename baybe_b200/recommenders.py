@@ -167,7 +167,7 @@ def greedy_select(gp: DeviceGP, cfg: AcqConfig, x_shard: torch.Tensor, d: int, q
     """Sequential greedy selection of q rows (global positions) -- ``optimize_acqf_discrete`` with
     ``unique=True``.  `x_shard` holds this rank's rows [offset, offset+len) on the device; the features of each
     round's winner are fetched from the rank that owns it (``_winner_row``).  A `gp` with a ``round_best`` method
-    (``baybe_b200.multiobjective.HviScorer``) scores a round itself and maps the winner's key value to the
+    (``baybe_b200.multiobjective.HviScorer``, ``baybe_b200.objectives.ObjectiveScorer``) scores a round itself and maps the winner's key value to the
     reported acquisition value."""
     chosen: list[int] = []
     values: list[float] = []
@@ -279,6 +279,7 @@ class B200Recommender:
 
     _objective = field(init=False, default=None, eq=False, repr=False)
     _context = field(init=False, default=None, eq=False, repr=False)
+    _scorer = field(init=False, default=None, eq=False, repr=False)
     _last_acq_values: list = field(init=False, factory=list, eq=False, repr=False)
 
     def _get_acquisition_function(self, objective) -> AcquisitionFunction:
@@ -304,9 +305,20 @@ class B200Recommender:
             raise IncompatibleAcquisitionFunctionError(
                 f"The '{type(self).__name__}' only works with Monte Carlo acquisition functions "
                 f"for batch sizes > 1.")
+        from baybe_b200.objectives import uses_objective_scorer
+
         self._objective = objective
         surrogate = self.get_surrogate(searchspace, objective, measurements)
-        cfg = acqf.to_engine(surrogate, searchspace, objective, measurements, pending_experiments)
+        self._scorer = None
+        if uses_objective_scorer(objective):  # a single target with a non-affine transformation
+            if pending_experiments is not None and not acqf.supports_pending_experiments:
+                raise IncompatibleAcquisitionFunctionError(
+                    f"The chosen acquisition function of type '{type(acqf).__name__}' "
+                    f"does not support pending experiments.")
+            self._scorer = acqf.scorer(surrogate, searchspace, objective, measurements)
+            cfg = self._scorer.cfg
+        else:
+            cfg = acqf.to_engine(surrogate, searchspace, objective, measurements, pending_experiments)
         subspace = searchspace.discrete
         candidates_exp, _ = subspace.get_candidates()
         if len(candidates_exp) < batch_size:
@@ -322,7 +334,8 @@ class B200Recommender:
         botorch/core.py:156-184); the recommendation context (acquisition config, search space, pending
         experiments) was stored by ``recommend`` the way the reference stores ``_botorch_acqf``."""
         cfg, searchspace, pending_experiments = self._context
-        return recommend_discrete_positions(self.surrogate_model.device_gp, cfg, subspace_discrete, candidates_exp,
+        gp = self._scorer if self._scorer is not None else self.surrogate_model.device_gp
+        return recommend_discrete_positions(gp, cfg, subspace_discrete, candidates_exp,
                                             batch_size, searchspace, pending_experiments, self.n_mc_samples,
                                             self._last_acq_values)
 

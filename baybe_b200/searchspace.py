@@ -198,7 +198,10 @@ def objective_affine(objective) -> tuple[float, float, str]:
 
     Accepts this module's SingleTargetObjective or a real BayBE one whose target carries an
     Identity/Affine transformation (objectives/single.py:77-91); anything else is rejected like
-    the reference rejects non-affine chains for analytic acquisition functions."""
+    the reference rejects non-affine chains for analytic acquisition functions.  A desirability objective applied as a
+    pre-transformation models its "Desirability" column with an identity objective (desirability.py:163-185, 224-225)."""
+    if type(objective).__name__ == "DesirabilityObjective" and getattr(objective, "as_pre_transformation", False):
+        return 1.0, 0.0, "Desirability"
     targets = getattr(objective, "targets", None)
     if targets is None or len(targets) != 1:
         raise NotImplementedError("only single-target objectives are supported by the B200 engine")

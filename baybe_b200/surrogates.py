@@ -222,6 +222,32 @@ def default_preset_name(searchspace) -> str:
     return "CHEN" if has_substance else "BAYBE"
 
 
+def _training_target(objective, measurements: pd.DataFrame) -> tuple[str, np.ndarray]:
+    """(modelled column, raw training values) of a single-model objective.  A single target is fitted on its raw
+    column whatever its transformation (``Objective._pre_transform`` passes it through, objectives/base.py:161-177;
+    the transformation belongs to the acquisition objective).  A desirability objective applied as a
+    pre-transformation is fitted on its "Desirability" column: the full desirability of every measured row
+    (desirability.py:322-345), computed by the float64 evaluator of ``baybe_b200.objectives``."""
+    from baybe_b200.objectives import compile_objective, evaluate_objective, is_desirability
+
+    if is_desirability(objective):
+        if not getattr(objective, "as_pre_transformation", False):
+            raise NotImplementedError("a desirability objective models one quantity per target: fit it through "
+                                      "BayBE's CompositeSurrogate (B200BotorchRecommender.get_surrogate does)")
+        comp = compile_objective(objective)
+        raw = measurements[list(comp.names)]
+        if raw.isna().any().any():
+            raise ValueError("partial measurements are not supported with as_pre_transformation=True")
+        return "Desirability", evaluate_objective(comp, raw.to_numpy(dtype=np.float64))
+    targets = getattr(objective, "targets", None)
+    if targets is None or len(targets) != 1:
+        _, _, name = objective_affine(objective)  # raises the usual message
+    name = targets[0].name
+    if measurements[name].isna().any():
+        raise ValueError("partial measurements are not supported (handle_missing_values)")
+    return name, measurements[name].to_numpy(dtype=np.float64)
+
+
 @define
 class GaussianProcessSurrogate:
     """GP surrogate whose posterior runs on the B200 engine."""
@@ -260,12 +286,9 @@ class GaussianProcessSurrogate:
             return
         if getattr(objective, "is_multi_output", False):
             raise NotImplementedError("multi-output objectives are outside the B200 engine's scope")
-        _, _, target = objective_affine(objective)
-        if measurements[target].isna().any():
-            raise ValueError("partial measurements are not supported (handle_missing_values)")
+        target, train_y = _training_target(objective, measurements)
         comp = searchspace.transform(measurements, allow_extra=True)
         train_x = comp.to_numpy(dtype=np.float64)
-        train_y = measurements[target].to_numpy(dtype=np.float64)
         bounds = np.asarray(searchspace.scaling_bounds.to_numpy(copy=True), dtype=np.float64)
         d = train_x.shape[1]
         task_col = searchspace.task_idx

@@ -368,6 +368,67 @@ int bb_hvi_score(const bb_acq_spec* a, int32_t n_targets, const float* obj_scale
                  const int32_t* d_n_cells, int32_t cell_stride, const uint8_t* d_keep, float* d_score,
                  int64_t* d_best_key, int64_t index_offset, void* stream);
 
+/* ---- Monte-Carlo (and, for affine MEAN desirability, analytic) acquisition values of an objective that is not
+ * affine in the modelled targets: DesirabilityObjective (baybe/objectives/desirability.py:229-264, weighted MEAN or
+ * geometric mean of per-target transformations) and single targets with a non-affine transformation
+ * (objectives/base.py:130-150), applied to posterior samples as the reference's MC acquisition functions do
+ * (acquisition/_builder.py:211-254, ChainedMCObjective).  Each target m carries a postfix program over its sample
+ * y_m (transformations/basic.py, composite.py; compiled on the host by baybe_b200/objectives.py), evaluated on an
+ * evaluation stack of at most BB_OBJ_MAX_STACK entries whose top starts as y_m; t_m = the single entry left.
+ * Then o = t_0 (NONE), sum_m w_m t_m (MEAN) or exp(sum_m w_m log(t_m + 2^-52)) (GEOM_MEAN), w normalised. */
+#define BB_OBJ_MAX_TARGETS 8
+#define BB_OBJ_MAX_OPS 32
+#define BB_OBJ_MAX_STACK 4
+typedef enum bb_obj_opcode {
+  BB_OBJ_AFFINE = 0,    /* top = top * arg0 + arg1                                      (AffineTransformation)  */
+  BB_OBJ_CONST = 1,     /* top = arg0                                                                         */
+  BB_OBJ_CLAMP = 2,     /* top = clamp(top, arg0, arg1), +-inf leaves a side open, NaN stays (Clamping)      */
+  BB_OBJ_TWO_SIDED = 3, /* d = top - arg2; top = d < 0 ? d * arg0 : d * arg1, a zero slope gives 0 (TwoSidedAffine) */
+  BB_OBJ_BELL = 4,      /* top = exp(-((top - arg0) / arg1)^2 / 2)                         (BellTransformation) */
+  BB_OBJ_LOG = 5,       /* top = log(top)                                           (LogarithmicTransformation) */
+  BB_OBJ_EXP = 6,       /* top = exp(top)                                           (ExponentialTransformation) */
+  BB_OBJ_POW_INT = 7,   /* top = top^arg0, arg0 integral                                  (PowerTransformation) */
+  BB_OBJ_SIGMOID = 8,   /* top = 1 / (1 + exp(arg1 * (top - arg0)))                     (SigmoidTransformation) */
+  BB_OBJ_DUP_INPUT = 9, /* push y_m (the second branch of an Additive / Multiplicative transformation)         */
+  BB_OBJ_ADD = 10,      /* pop b, pop a, push a + b                                     (AdditiveTransformation) */
+  BB_OBJ_MUL = 11       /* pop b, pop a, push a * b                               (MultiplicativeTransformation) */
+} bb_obj_opcode;
+typedef enum bb_obj_scalarizer {
+  BB_OBJ_SCALAR_NONE = 0,     /* single target                                                               */
+  BB_OBJ_SCALAR_MEAN = 1,     /* Scalarizer.MEAN      (LinearMCObjective(normalized_weights))                */
+  BB_OBJ_SCALAR_GEOM_MEAN = 2 /* Scalarizer.GEOM_MEAN (_geometric_mean, desirability.py:41-70)              */
+} bb_obj_scalarizer;
+typedef struct bb_obj_instr {
+  int32_t op; /* bb_obj_opcode */
+  float arg[3];
+} bb_obj_instr;
+typedef struct bb_objective {
+  int32_t n_targets;                          /* M in [1, BB_OBJ_MAX_TARGETS]                           */
+  int32_t scalarizer;                         /* bb_obj_scalarizer                                      */
+  int32_t n_ops[BB_OBJ_MAX_TARGETS];          /* program length per target (0: identity)                */
+  float weight[BB_OBJ_MAX_TARGETS];           /* normalised weights (MEAN / GEOM_MEAN)                  */
+  bb_obj_instr prog[BB_OBJ_MAX_TARGETS][BB_OBJ_MAX_OPS];
+} bb_objective;
+
+/* Kinds: BB_ACQ_QLOGEI / QEI / QPI / QSR / QUCB over the samples o_s of the objective; EI / LOGEI / PI / UCB / PM / PSTD
+ * only for MEAN scalarisation with every program a single AFFINE op (or empty) and no pending point: the moments
+ * sum_m w_m (a_m mu_m + b_m) and sum_m (w_m a_m)^2 var_m (desirability.py:266-320) go to the analytic formulas.
+ *   d_mu / d_var [M][N]: marginal posterior of every candidate per target (bb_posterior, one model per target).
+ *   d_z [S][M(1+P)]: base samples; column m(1+P)+j is pending point j of target m, column m(1+P)+P the candidate.
+ *   n_pending = P in [0, BB_MAX_PENDING].  With P > 0: d_cross [M][N][P], d_linv [M][P][P] = L_PP^-1 and
+ *     d_w [M][S][P] = L_PP^-T z_P per target (as bb_hvi_score): y_m = mu_m + c_m . w_{m,s} +
+ *     sqrt(max(var_m - |L_m^-1 c_m|^2, 0)) z_{s, m(1+P)+P}; d_pend_terms [S][P]: the per-sample term of every pending
+ *     point (qLogEI: log fatplus(o - best_f) with tau_relu; qEI: relu(o - best_f); qPI: sigmoid((o - best_f)/tau_pi);
+ *     qSR: o; qUCB: m + sqrt(beta pi / 2) |o - m| with m the sample mean of that point's o).  The candidate's term
+ *     joins them by max (qLogEI: fatmax with tau_max), like bb_acq_score_joint.
+ * Writes the value of every candidate to d_score (nullable) and folds d_keep (nullable) and index_offset into
+ * *d_best_key like bb_argmax (initialise with bb_best_init).  S in [1, 1024].  The objective is passed to the
+ * kernel by value (no device copy): concurrent calls on different streams do not share state. */
+int bb_objective_score(const bb_acq_spec* a, const bb_objective* obj, int64_t N, const float* d_mu, const float* d_var,
+                       int32_t n_pending, const float* d_cross, const float* d_linv, const float* d_w,
+                       const float* d_pend_terms, const float* d_z, int32_t S, const uint8_t* d_keep, float* d_score,
+                       int64_t* d_best_key, int64_t index_offset, void* stream);
+
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
 int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
