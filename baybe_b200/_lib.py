@@ -24,7 +24,9 @@ MC_KINDS = ("qLogEI", "qEI", "qUCB", "qSR", "qPI", "qEHVI", "qLogEHVI")
 HVI_KINDS = ("qEHVI", "qLogEHVI")  # Pareto objectives: bb_hvi_score (baybe_b200/multiobjective.py)
 HVI_MAX_TARGETS = 4
 HVI_MAX_CELLS = 1024
-NEI_KINDS = ("qNEI",)  # evaluated by baybe_b200/hybrid.py (conditional form + bb_nei_reduce), not by the fused kernels
+# never by the fused kernels: hybrid spaces (qNEI only) by baybe_b200/hybrid.py (conditional form + bb_nei_reduce),
+# discrete spaces by baybe_b200/noisy.py (bb_nei_score)
+NEI_KINDS = ("qNEI", "qLogNEI")
 MAX_PENDING = 31
 MAX_TRAIN = 1024
 
@@ -138,6 +140,9 @@ _SIGNATURES = {
                                _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp]),
     "bb_objective_score": (C.c_int, [C.POINTER(AcqSpec), C.POINTER(Objective), _i64, _vp, _vp, _i32, _vp, _vp, _vp,
                                      _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp]),
+    "bb_joint_posterior": (C.c_int, [C.POINTER(Model), _vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "bb_nei_score": (C.c_int, [_i32, C.c_float, C.c_float, C.c_float, C.c_float, _i64, _vp, _vp, _i32, _vp, _vp, _vp,
+                               _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),

@@ -19,7 +19,7 @@ __all__ = [
     "qLogExpectedImprovement", "ProbabilityOfImprovement", "qProbabilityOfImprovement",
     "UpperConfidenceBound", "qUpperConfidenceBound", "convert_acqf",
     "PM", "PSTD", "qSR", "EI", "qEI", "LogEI", "qLogEI", "PI", "qPI", "UCB", "qUCB",
-    "qNoisyExpectedImprovement", "qNEI",
+    "qNoisyExpectedImprovement", "qNEI", "qLogNoisyExpectedImprovement", "qLogNEI",
     "qExpectedHypervolumeImprovement", "qEHVI", "qLogExpectedHypervolumeImprovement", "qLogEHVI",
 ]
 
@@ -155,6 +155,8 @@ def _evaluate_with_scorer(acqf, scorer, candidates: pd.DataFrame, searchspace, p
     if pending_experiments is not None and len(pending_experiments) > 0:
         pend = searchspace.transform(pending_experiments, allow_extra=True).to_numpy(dtype="float64")
     seed = _draw_sampler_seed()
+    if jointly and hasattr(scorer, "joint_value"):  # the scorer tells batch points from pending points itself
+        return scorer.joint_value(rows, pend, seed, DEFAULT_MC_SAMPLES)
     if jointly:  # candidate first, then the rest of the batch and the pending points
         rest = rows[1:] if pend is None else np.concatenate([rows[1:], pend], axis=0)
         if len(rest) and not scorer.cfg.is_mc:
@@ -233,13 +235,54 @@ class qUpperConfidenceBound(AcquisitionFunction):
         return {"beta": self.beta}
 
 
+def _space_kind(searchspace) -> str:
+    return getattr(getattr(searchspace, "type", None), "name", "DISCRETE")
+
+
 @define(frozen=True)
-class qNoisyExpectedImprovement(AcquisitionFunction):
-    """acquisition/acqfs.py:227-232.  Evaluated by ``baybe_b200.hybrid`` (hybrid search spaces); ``prune_baseline``
-    is accepted for compatibility: the engine keeps every baseline point (its cost is one GEMM column each)."""
+class _NoisyExpectedImprovement(AcquisitionFunction):
+    """The noisy-EI family on discrete search spaces: ``baybe_b200.noisy.NeiScorer`` (``bb_nei_score``) with the
+    measured rows as baseline, pruned to the points that are the best of at least one joint posterior sample
+    (``prune_baseline=True``, the default) or kept whole (``prune_baseline=False``, at most 31 points together with
+    the pending points)."""
+
+    prune_baseline: bool = field(default=True, validator=instance_of(bool))
+
+    def scorer(self, surrogate, searchspace, objective, measurements):
+        """Check the objective, fit the surrogate, then set up the baseline and its pruning
+        (``baybe_b200.noisy.build_nei_scorer``)."""
+        from baybe_b200.noisy import build_nei_scorer
+
+        kind = _space_kind(searchspace)
+        if kind != "DISCRETE":
+            raise IncompatibleAcquisitionFunctionError(
+                f"'{type(self).__name__}' is scored by baybe_b200.noisy on discrete search spaces only (got {kind})")
+        return build_nei_scorer(self, surrogate, searchspace, objective, measurements)
+
+    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
+                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
+        if _space_kind(searchspace) != "DISCRETE":
+            return super().evaluate(candidates, surrogate, searchspace, objective, measurements, pending_experiments,
+                                    jointly=jointly)
+        scorer = self.scorer(surrogate, searchspace, objective, measurements)
+        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
+
+
+@define(frozen=True)
+class qNoisyExpectedImprovement(_NoisyExpectedImprovement):
+    """acquisition/acqfs.py:226-232.  Discrete search spaces: ``baybe_b200.noisy``; hybrid search spaces:
+    ``baybe_b200.hybrid``, which keeps every baseline point (its cost is one GEMM column each) and ignores
+    ``prune_baseline``."""
 
     abbreviation: ClassVar[str] = "qNEI"
-    prune_baseline: bool = field(default=True, validator=instance_of(bool))
+
+
+@define(frozen=True)
+class qLogNoisyExpectedImprovement(_NoisyExpectedImprovement):
+    """acquisition/acqfs.py:235-243; discrete search spaces only, tau_relu = 1e-6 and tau_max = 1e-2 as in
+    ``AcqConfig``."""
+
+    abbreviation: ClassVar[str] = "qLogNEI"
 
 
 def _reference_point(v):
@@ -307,14 +350,14 @@ class qLogExpectedHypervolumeImprovement(_ExpectedHypervolumeImprovement):
     abbreviation: ClassVar[str] = "qLogEHVI"
 
 
-qNEI = qNoisyExpectedImprovement
+qNEI, qLogNEI = qNoisyExpectedImprovement, qLogNoisyExpectedImprovement
 qEHVI, qLogEHVI = qExpectedHypervolumeImprovement, qLogExpectedHypervolumeImprovement
 PM, PSTD, qSR = PosteriorMean, PosteriorStandardDeviation, qSimpleRegret
 EI, qEI, LogEI, qLogEI = ExpectedImprovement, qExpectedImprovement, LogExpectedImprovement, qLogExpectedImprovement
 PI, qPI, UCB, qUCB = ProbabilityOfImprovement, qProbabilityOfImprovement, UpperConfidenceBound, qUpperConfidenceBound
 
-_BY_NAME = {c.__name__: c for c in (PM, PSTD, qSR, EI, qEI, LogEI, qLogEI, PI, qPI, UCB, qUCB, qNEI, qEHVI,
-                                    qLogEHVI)}
+_BY_NAME = {c.__name__: c for c in (PM, PSTD, qSR, EI, qEI, LogEI, qLogEI, PI, qPI, UCB, qUCB, qNEI, qLogNEI,
+                                    qEHVI, qLogEHVI)}
 _BY_NAME.update({c.abbreviation: c for c in list(_BY_NAME.values())})
 
 

@@ -72,8 +72,9 @@ class EngineAcquisitionFunction:
         self.cfg = cfg
         self.n_mc_samples = n_mc_samples
         self.X_pending = X_pending
-        # objectives the fused path does not serve: baybe_b200.multiobjective.HviScorer (Pareto) or
-        # baybe_b200.objectives.ObjectiveScorer (desirability, non-affine single targets)
+        # what the fused path does not serve: baybe_b200.multiobjective.HviScorer (Pareto),
+        # baybe_b200.objectives.ObjectiveScorer (desirability, non-affine single targets) or
+        # baybe_b200.noisy.NeiScorer (qNEI / qLogNEI on discrete spaces)
         self.scorer = scorer
         self.seed = _draw_sampler_seed()  # botorch samplers draw their seed once, at construction
 
@@ -91,6 +92,11 @@ class EngineAcquisitionFunction:
             if not self.scorer.cfg.is_mc:
                 raise IncompatibleAcquisitionFunctionError("analytic acquisition functions value single points only")
             out = torch.empty(b, dtype=torch.float64)
+            if hasattr(self.scorer, "joint_value"):  # batch points and pending points play different roles
+                pn = None if pend is None or len(pend) == 0 else pend.cpu().numpy()
+                for i in range(b):
+                    out[i] = self.scorer.joint_value(X[i].cpu().numpy(), pn, self.seed, self.n_mc_samples)
+                return out
             for i in range(b):
                 rest = X[i, 1:, :] if pend is None else torch.cat([X[i, 1:, :], pend.to(X)], dim=0)
                 out[i] = float(self.scorer.scores(X[i, :1, :], rest.cpu().numpy(), self.seed, self.n_mc_samples)[0])
@@ -129,7 +135,8 @@ class B200BotorchRecommender(BayesianRecommender):
     _context = field(default=None, init=False, eq=False, repr=False)
     _scorer = field(default=None, init=False, eq=False, repr=False)
     """Objectives the fused path does not serve: the ``HviScorer`` (Pareto) or ``ObjectiveScorer`` (desirability,
-    non-affine single targets) set up by ``_setup_botorch_acqf``."""
+    non-affine single targets) set up by ``_setup_botorch_acqf``; on discrete spaces also the ``NeiScorer`` of qNEI /
+    qLogNEI (its ``n_dropped``: baseline winners left out by the last evaluation)."""
     _last_acq_values: list = field(factory=list, init=False, eq=False, repr=False)
 
     # ---- multi-target objectives (SURVEY.md 8f-4, surrogates/composite.py:59-181) ------------------------------
@@ -164,7 +171,8 @@ class B200BotorchRecommender(BayesianRecommender):
                     f"qLogNEHVI, bayesian/base.py:73)")
         surrogate = self.get_surrogate(searchspace, objective, measurements)
         spec = mirror_acquisition_function(acqf)
-        if objective.is_multi_output or uses_objective_scorer(objective):
+        discrete_nei = spec.abbreviation in _lib.NEI_KINDS and searchspace.type is SearchSpaceType.DISCRETE
+        if objective.is_multi_output or uses_objective_scorer(objective) or discrete_nei:
             if pending_experiments is not None and not spec.supports_pending_experiments:
                 raise IncompatibleAcquisitionFunctionError(
                     f"The chosen acquisition function of type '{type(spec).__name__}' "

@@ -40,11 +40,12 @@ __device__ __forceinline__ float pending_r2_warp(float c, const float* linv, int
   return r2;
 }
 
-// c . w_s (lane j holds c_j; wr: the P entries of w_s = L_PP^-T z_{s,P} of this lane's sample).  Every lane takes
-// part in the shuffles.
-__device__ __forceinline__ float pending_cw_warp(float c, const float* wr, int P) {
+// c . w_s (lane j holds c_j; wr: entry 0 of w_s = L_PP^-T z_{s,P} of this lane's sample, entry j at wr[j * stride]:
+// stride 1 for a [S][P] layout, S for a sample-minor [P][S] layout whose loads coalesce across the warp).  Every lane
+// takes part in the shuffles.
+__device__ __forceinline__ float pending_cw_warp(float c, const float* wr, int P, int stride = 1) {
   float dm = 0.f;
-  for (int j = 0; j < P; ++j) dm = fmaf(__shfl_sync(0xffffffffu, c, j), __ldg(wr + j), dm);
+  for (int j = 0; j < P; ++j) dm = fmaf(__shfl_sync(0xffffffffu, c, j), __ldg(wr + (size_t)j * stride), dm);
   return dm;
 }
 
@@ -68,6 +69,20 @@ __device__ __forceinline__ void lse_push(float v, float& mx, float& sum) {
     mx = v;
   } else {
     sum += __expf(v - mx);
+  }
+}
+
+// warp-wide merge of per-lane online logsumexp states; result in every lane
+__device__ __forceinline__ void lse_warp_combine(float& mx, float& sum) {
+  for (int o = 16; o > 0; o >>= 1) {
+    const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+    const float os = __shfl_xor_sync(0xffffffffu, sum, o);
+    const float nm = fmaxf(mx, om);
+    float acc = 0.f;
+    if (mx > -INFINITY) acc += sum * __expf(mx - nm);
+    if (om > -INFINITY) acc += os * __expf(om - nm);
+    mx = nm;
+    sum = acc;
   }
 }
 

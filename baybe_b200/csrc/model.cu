@@ -454,7 +454,8 @@ __global__ void k_pending_w(const float* __restrict__ pend_x, int P, int n, int 
                             const float* __restrict__ cand_norm /* [2*d]: lo, inv_range */,
                             const double* __restrict__ Linv, const double* __restrict__ alpha64,
                             const float* __restrict__ mean_const, float y_mean, float y_std,
-                            float* __restrict__ beta_out, float* __restrict__ mu_out,
+                            float* __restrict__ beta_out /* nullable */, float* __restrict__ mu_out /* nullable */,
+                            double* __restrict__ mu64_out /* nullable */,
                             double* __restrict__ pn_out /* [P*d] normalised pending */,
                             double* __restrict__ w_out /* [P*n] */) {
   extern __shared__ double sh[];
@@ -485,7 +486,8 @@ __global__ void k_pending_w(const float* __restrict__ pend_x, int P, int n, int 
     if (tid < s) red[tid] += red[tid + s];
     __syncthreads();
   }
-  if (tid == 0) mu_out[p] = y_mean + y_std * (float)((double)mean_const[tp] + red[0]);
+  if (tid == 0 && mu_out) mu_out[p] = y_mean + y_std * (float)((double)mean_const[tp] + red[0]);
+  if (tid == 0 && mu64_out) mu64_out[p] = (double)y_mean + (double)y_std * ((double)mean_const[tp] + red[0]);
   for (int j = tid; j < n; j += blockDim.x) {
     double s = 0.0;
     for (int i = 0; i <= j; ++i) s += Linv[(size_t)j * n + i] * kx[i];
@@ -493,6 +495,7 @@ __global__ void k_pending_w(const float* __restrict__ pend_x, int P, int n, int 
     w_out[(size_t)p * n + j] = s;
   }
   __syncthreads();
+  if (beta_out == nullptr) return;
   for (int i = tid; i < n_pad; i += blockDim.x) {
     double s = 0.0;
     if (i < n)
@@ -501,12 +504,13 @@ __global__ void k_pending_w(const float* __restrict__ pend_x, int P, int n, int 
   }
 }
 
-// cov[p][q] = (k(p,q) - w_p . w_q) * y_std^2, float64
+// cov[p][q] = (k(p,q) - w_p . w_q) * y_std^2, float64; row p per blockIdx.x, columns q over blockIdx.y * 32 + lane.
+// Written as fp32 to cov and / or as float64 to cov64 (both nullable).
 __global__ void k_pending_cov(const double* __restrict__ pn, const double* __restrict__ w, int P,
                               int n, int d, int T, int family, int task_col,
                               const double* __restrict__ aux, float y_std,
-                              float* __restrict__ cov) {
-  int p = blockIdx.x, q = threadIdx.x;
+                              float* __restrict__ cov, double* __restrict__ cov64) {
+  int p = blockIdx.x, q = blockIdx.y * blockDim.x + threadIdx.x;
   if (q >= P) return;
   const double* tcov = aux;
   const double* inv_ls = aux + T * T;
@@ -516,7 +520,9 @@ __global__ void k_pending_cov(const double* __restrict__ pn, const double* __res
   k *= tcov[tp * T + tq];
   double s = 0.0;
   for (int j = 0; j < n; ++j) s += w[(size_t)p * n + j] * w[(size_t)q * n + j];
-  cov[p * P + q] = (float)((k - s) * (double)y_std * (double)y_std);
+  const double c = (k - s) * (double)y_std * (double)y_std;
+  if (cov) cov[p * P + q] = (float)c;
+  if (cov64) cov64[(size_t)p * P + q] = c;
 }
 
 }  // namespace bb
@@ -882,10 +888,38 @@ extern "C" int bb_pending_stats(const bb_model* m, const float* d_pend_x, int32_
                                        m->task_col, m->d_xn64, m->d_train_task,
                                        (const double*)(B + L.tcov64), (const float*)(B + L.cnorm),
                                        m->d_linv, m->d_alpha64, m->d_mean_const, m->y_mean,
-                                       m->y_std, d_pend_beta, d_pend_mu, pn, w64);
+                                       m->y_std, d_pend_beta, d_pend_mu, nullptr, pn, w64);
   BB_LAUNCH_CHECK();
   k_pending_cov<<<P, 32, 0, stream>>>(pn, w64, P, m->n, m->d, m->n_tasks, m->family, m->task_col,
-                                      (const double*)(B + L.tcov64), m->y_std, d_pend_cov);
+                                      (const double*)(B + L.tcov64), m->y_std, d_pend_cov, nullptr);
+  BB_LAUNCH_CHECK();
+  return BB_OK;
+}
+
+extern "C" int bb_joint_posterior(const bb_model* m, const float* d_x, int32_t R, double* d_mu, double* d_cov,
+                                  float* d_beta, double* d_ws, size_t ws_doubles, void* stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  BB_CHECK_ARG(m != nullptr, "bb_joint_posterior: null model");
+  BB_CHECK_ARG(m->abi_version == BB_ABI_VERSION, "bb_joint_posterior: ABI mismatch");
+  BB_CHECK_ARG(R >= 1 && R <= m->n_pad, "bb_joint_posterior: R=%d outside [1,n_pad=%d]", R, m->n_pad);
+  BB_CHECK_ARG(d_x && d_mu && d_cov && d_ws, "bb_joint_posterior: null argument");
+  const size_t need = (size_t)R * ((size_t)m->n_pad + (size_t)m->d);
+  if (ws_doubles < need) {
+    set_error("bb_joint_posterior: workspace of %zu doubles, need %zu", ws_doubles, need);
+    return BB_ERR_WORKSPACE;
+  }
+  BlobLayout L = make_layout(m->n, m->d, m->n_tasks);
+  uint8_t* B = (uint8_t*)m->d_blob;
+  double* w64 = d_ws;                           // [R][n] L^-1 k(X, x_r)
+  double* pn = d_ws + (size_t)R * m->n_pad;     // [R][d] normalised rows
+  size_t shm = sizeof(double) * (m->d + 2 * m->n);
+  k_pending_w<<<R, 256, shm, stream>>>(d_x, R, m->n, m->n_pad, m->d, m->n_tasks, m->family, m->task_col, m->d_xn64,
+                                       m->d_train_task, (const double*)(B + L.tcov64), (const float*)(B + L.cnorm),
+                                       m->d_linv, m->d_alpha64, m->d_mean_const, m->y_mean, m->y_std, d_beta,
+                                       nullptr, d_mu, pn, w64);
+  BB_LAUNCH_CHECK();
+  k_pending_cov<<<dim3(R, (R + 31) / 32), 32, 0, stream>>>(pn, w64, R, m->n, m->d, m->n_tasks, m->family, m->task_col,
+                                                          (const double*)(B + L.tcov64), m->y_std, nullptr, d_cov);
   BB_LAUNCH_CHECK();
   return BB_OK;
 }

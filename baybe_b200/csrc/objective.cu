@@ -86,20 +86,6 @@ __device__ __forceinline__ float run_program(const bb_obj_instr* prog, int n, fl
   return x;
 }
 
-// warp-wide merge of per-lane online logsumexp states; result in every lane
-__device__ __forceinline__ void lse_warp_combine(float& mx, float& sum) {
-  for (int o = 16; o > 0; o >>= 1) {
-    const float om = __shfl_xor_sync(0xffffffffu, mx, o);
-    const float os = __shfl_xor_sync(0xffffffffu, sum, o);
-    const float nm = fmaxf(mx, om);
-    float acc = 0.f;
-    if (mx > -INFINITY) acc += sum * __expf(mx - nm);
-    if (om > -INFINITY) acc += os * __expf(om - nm);
-    mx = nm;
-    sum = acc;
-  }
-}
-
 __global__ void __launch_bounds__(kObjThreads) k_objective(const __grid_constant__ ObjParams p) {
   extern __shared__ __align__(16) float smem_o[];
   const int M = p.obj.n_targets, P = p.P, S = p.S, Q = P + 1;

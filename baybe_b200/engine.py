@@ -86,7 +86,8 @@ class AcqConfig:
 
     def to_c(self) -> _lib.AcqSpec:
         if self.kind in _lib.NEI_KINDS:
-            raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.hybrid.NeiScorer, not by the fused kernels")
+            raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.noisy.NeiScorer (discrete spaces) or "
+                                      "baybe_b200.hybrid.NeiScorer (hybrid spaces), not by the fused kernels")
         return _lib.AcqSpec(
             _lib.ACQ_KIND[self.kind], int(self.maximize), self.best_f, self.beta, self.obj_scale,
             self.obj_shift, self.tau_relu, self.tau_max, self.tau_pi,
@@ -645,6 +646,73 @@ def _op_hvi_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | Non
 def _(mu, var, cross, linv, w, z, lower, upper, n_cells, keep, kind, params, obj_scale, obj_shift, index_offset,
       want_scores):
     return (mu.new_empty(mu.shape[1] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
+
+
+@torch.library.custom_op("baybe_b200::joint_posterior", mutates_args=())
+def _op_joint_posterior(x: torch.Tensor, handle: int, with_beta: bool) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """``bb_joint_posterior``: float64 mean [R] and covariance [R, R] of R raw fp32 rows [R, d]; with `with_beta`
+    also beta = K^-1 k(X, rows) [R, n_pad] fp32 (the input ``posterior_cross`` takes for them), else a [0, n_pad]
+    tensor."""
+    gp = _gp(handle)
+    R = x.shape[0]
+    if x.dim() != 2 or x.shape[1] != gp.d or x.dtype != torch.float32 or not x.is_contiguous():
+        raise ValueError(f"rows must be a contiguous float32 (R, {gp.d}) tensor")
+    mu = torch.empty(R, dtype=torch.float64, device=x.device)
+    cov = torch.empty((R, R), dtype=torch.float64, device=x.device)
+    beta = torch.empty((R if with_beta else 0, gp.model.n_pad), dtype=torch.float32, device=x.device)
+    ws = torch.empty(max(R, 1) * (gp.model.n_pad + gp.d), dtype=torch.float64, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().bb_joint_posterior(C.byref(gp.model), _ptr(x), R, _ptr(mu), _ptr(cov),
+                                                  _ptr(beta) if with_beta else None, _ptr(ws), ws.numel(),
+                                                  _stream_ptr()), "bb_joint_posterior")
+    return mu, cov, beta
+
+
+@_op_joint_posterior.register_fake
+def _(x, handle, with_beta):
+    R = x.shape[0]
+    return (x.new_empty(R, dtype=torch.float64), x.new_empty((R, R), dtype=torch.float64),
+            x.new_empty((R if with_beta else 0, _gp(handle).model.n_pad), dtype=torch.float32))
+
+
+@torch.library.custom_op("baybe_b200::nei_score", mutates_args=())
+def _op_nei_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | None, linv: torch.Tensor | None,
+                  w: torch.Tensor | None, z: torch.Tensor, g: torch.Tensor, batch_terms: torch.Tensor | None,
+                  keep: torch.Tensor | None, log_nei: bool, params: list[float], index_offset: int,
+                  want_scores: bool) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_nei_score``: mu/var [N]; with |C| conditioning points cross [N, |C|], linv [|C|, |C|] (L_C^-1) and
+    w [|C|, S] (sample-minor); z [S, 1 + |C|]; g [S]; batch_terms [S, Q] for the other Q points of a q-batch.
+    params = [obj_scale, obj_shift, tau_relu, tau_max]."""
+    N = mu.shape[0]
+    Cn = 0 if cross is None else cross.shape[1]
+    S = z.shape[0]
+    if z.dim() != 2 or z.shape[1] != Cn + 1:
+        raise ValueError(f"base samples must be (S, {Cn + 1})")
+    if g.numel() != S:
+        raise ValueError(f"incumbents must be (S,) = ({S},)")
+    if Cn and (linv is None or tuple(linv.shape) != (Cn, Cn) or w is None or tuple(w.shape) != (Cn, S)):
+        raise ValueError(f"conditioning needs linv ({Cn}, {Cn}) and w ({Cn}, {S})")
+    Q = 0 if batch_terms is None else batch_terms.shape[1]
+    if Q and tuple(batch_terms.shape) != (S, Q):
+        raise ValueError(f"batch terms must be (S, Q) = ({S}, {Q})")
+    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
+        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
+    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
+    key = torch.empty(1, dtype=torch.int64, device=mu.device)
+    a, b, tau_relu, tau_max = (float(v) for v in params)
+    lib = _lib.load()
+    with torch.cuda.device(mu.device):
+        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        _lib.check(lib.bb_nei_score(int(log_nei), a, b, tau_relu, tau_max, N, _ptr(mu), _ptr(var), Cn, _ptr(cross),
+                                    _ptr(linv), _ptr(w), _ptr(z), S, _ptr(g), Q, _ptr(batch_terms), _ptr(keep),
+                                    _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
+                                    _stream_ptr()), "bb_nei_score")
+    return score, key
+
+
+@_op_nei_score.register_fake
+def _(mu, var, cross, linv, w, z, g, batch_terms, keep, log_nei, params, index_offset, want_scores):
+    return (mu.new_empty(mu.shape[0] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
 
 
 def objective_struct(n_targets: int, scalarizer: int, programs, weights) -> _lib.Objective:

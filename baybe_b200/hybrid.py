@@ -238,7 +238,7 @@ def recommend_hybrid(gp: DeviceGP, acq: AcqConfig, disc_comp: np.ndarray, cont_b
 
     ``disc_comp``: (n_configs, d_disc) comp-rep rows of the discrete subspace (it comes first in BayBE's hybrid
     comp-rep, hybrid.py:45-46); ``cont_bounds``: (2, d_cont)."""
-    if acq.kind not in _lib.NEI_KINDS:
+    if acq.kind != "qNEI":
         raise NotImplementedError("the device hybrid recommender evaluates the noisy-EI family (qNEI)")
     search = search or HybridSearch()
     dev = gp.device

@@ -30,6 +30,7 @@ from attrs.converters import optional
 
 from baybe_b200.acquisition import (AcquisitionFunction, IncompatibleAcquisitionFunctionError,
                                     convert_acqf, qLogExpectedImprovement)
+from baybe_b200._lib import NEI_KINDS
 from baybe_b200.bits import pack_bits
 from baybe_b200.engine import DEFAULT_MC_SAMPLES, AcqConfig, DeviceGP, sobol_normal_samples, unpack_best
 from baybe_b200.surrogates import GaussianProcessSurrogate
@@ -167,8 +168,8 @@ def greedy_select(gp: DeviceGP, cfg: AcqConfig, x_shard: torch.Tensor, d: int, q
     """Sequential greedy selection of q rows (global positions) -- ``optimize_acqf_discrete`` with
     ``unique=True``.  `x_shard` holds this rank's rows [offset, offset+len) on the device; the features of each
     round's winner are fetched from the rank that owns it (``_winner_row``).  A `gp` with a ``round_best`` method
-    (``baybe_b200.multiobjective.HviScorer``, ``baybe_b200.objectives.ObjectiveScorer``) scores a round itself and maps the winner's key value to the
-    reported acquisition value."""
+    (``baybe_b200.multiobjective.HviScorer``, ``baybe_b200.objectives.ObjectiveScorer``, ``baybe_b200.noisy.NeiScorer``)
+    scores a round itself and maps the winner's key value to the reported acquisition value."""
     chosen: list[int] = []
     values: list[float] = []
     keep = (torch.ones(x_shard.shape[0], dtype=torch.uint8, device=x_shard.device)
@@ -310,7 +311,8 @@ class B200Recommender:
         self._objective = objective
         surrogate = self.get_surrogate(searchspace, objective, measurements)
         self._scorer = None
-        if uses_objective_scorer(objective):  # a single target with a non-affine transformation
+        # a single target with a non-affine transformation, or the noisy-EI family
+        if uses_objective_scorer(objective) or acqf.abbreviation in NEI_KINDS:
             if pending_experiments is not None and not acqf.supports_pending_experiments:
                 raise IncompatibleAcquisitionFunctionError(
                     f"The chosen acquisition function of type '{type(acqf).__name__}' "

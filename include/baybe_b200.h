@@ -241,6 +241,16 @@ int bb_posterior(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
 int bb_pending_stats(const bb_model* m, const float* d_pend_x, int32_t n_pending,
                      float* d_pend_beta, float* d_pend_mu, float* d_pend_cov, void* stream);
 
+/* ---- joint posterior of R raw rows (fp32 row-major raw comp-rep, 1 <= R <= n_pad), float64 throughout: mean d_mu [R]
+ * and full covariance d_cov [R][R] of the latent function in original units -- what the reference samples from when
+ * it prunes the noisy-EI baseline (botorch prune_inferior_points on the measured rows, acquisition/_builder.py:
+ * 319-324).  d_beta (nullable): [R][n_pad] fp32 beta = K^-1 k(X, x_r), as bb_pending_stats gives it, so that the
+ * same rows can condition bb_posterior's cross covariance without a second pass.  The caller owns the float64
+ * workspace d_ws of ws_doubles >= R * (n_pad + d) entries.  Unlike forming the covariance in fp32 from
+ * bb_kernel_matrix, this does not cancel at noise-level variances. */
+int bb_joint_posterior(const bb_model* m, const float* d_x, int32_t R, double* d_mu, double* d_cov, float* d_beta,
+                       double* d_ws, size_t ws_doubles, void* stream);
+
 /* ---- K6: acquisition value of each candidate as its own q=1 batch from (mu, var).
  * d_z: [S] shared Sobol-normal base samples (MC kinds; ignored for analytic kinds).
  * Replaces qLogExpectedImprovement.forward etc. (class picked at acquisition/base.py:162-181). */
@@ -428,6 +438,28 @@ int bb_objective_score(const bb_acq_spec* a, const bb_objective* obj, int64_t N,
                        int32_t n_pending, const float* d_cross, const float* d_linv, const float* d_w,
                        const float* d_pend_terms, const float* d_z, int32_t S, const uint8_t* d_keep, float* d_score,
                        int64_t* d_best_key, int64_t index_offset, void* stream);
+
+/* ---- noisy expected improvement of one new point per candidate of a discrete space (qNoisyExpectedImprovement,
+ * log_nei = 0, or qLogNoisyExpectedImprovement, log_nei = 1; baybe/acquisition/acqfs.py:226-243; set-up on the host
+ * by baybe_b200/noisy.py).  The conditioning set C (n_cond <= BB_MAX_PENDING points: the pruned baseline, the pending
+ * points, then the n_batch other points of a q-batch) is sampled jointly by the caller:
+ *   d_mu / d_var [N], d_cross [N][n_cond]: bb_posterior of the candidates with C as its pending points;
+ *   d_linv [n_cond][n_cond] = L_C^-1 (row-major, lower triangular), L_C L_C^T = Sigma_CC;
+ *   d_w [n_cond][S] = L_C^-T z_{s,C} stored sample-minor (entry (j, s) at j * S + s);
+ *   d_z [S][n_cond + 1]: base samples, column n_cond the candidate's;
+ *   d_g [S]: per-sample incumbent, the maximum of o over baseline and pending points;
+ *   d_batch_terms [S][n_batch]: per-sample terms of the other batch points (nullable when n_batch = 0).
+ * Per sample o_s = obj_scale * (mu + c . w_s + sqrt(max(var - |L_C^-1 c|^2, 0)) z_{s,n_cond}) + obj_shift and
+ *   qNEI    : t_s = relu(o_s - g_s), joined with the batch terms by max, value = mean_s;
+ *   qLogNEI : t_s = log tau_relu + log fatplus((o_s - g_s) / tau_relu), joined by fatmax (tau_max), value =
+ *             logmeanexp_s.
+ * Writes the value of every candidate to d_score (nullable) and folds d_keep (nullable) and index_offset into
+ * *d_best_key like bb_argmax (initialise with bb_best_init).  S in [1, 1024]. */
+int bb_nei_score(int32_t log_nei, float obj_scale, float obj_shift, float tau_relu, float tau_max, int64_t N,
+                 const float* d_mu, const float* d_var, int32_t n_cond, const float* d_cross, const float* d_linv,
+                 const float* d_w, const float* d_z, int32_t S, const float* d_g, int32_t n_batch,
+                 const float* d_batch_terms, const uint8_t* d_keep, float* d_score, int64_t* d_best_key,
+                 int64_t index_offset, void* stream);
 
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
