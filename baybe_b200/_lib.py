@@ -27,6 +27,9 @@ HVI_MAX_CELLS = 1024
 # never by the fused kernels: hybrid spaces (qNEI only) by baybe_b200/hybrid.py (conditional form + bb_nei_reduce),
 # discrete spaces by baybe_b200/noisy.py (bb_nei_score)
 NEI_KINDS = ("qNEI", "qLogNEI")
+# never by the fused kernels: Pareto objectives by random Chebyshev scalarisation, baybe_b200/parego.py
+PAREGO_KINDS = ("qLogNParEGO",)
+PAREGO_MAX_TARGETS = 8  # BB_OBJ_MAX_TARGETS
 MAX_PENDING = 31
 MAX_TRAIN = 1024
 
@@ -143,6 +146,9 @@ _SIGNATURES = {
     "bb_joint_posterior": (C.c_int, [C.POINTER(Model), _vp, _i32, _vp, _vp, _vp, _vp, _sz, _vp]),
     "bb_nei_score": (C.c_int, [_i32, C.c_float, C.c_float, C.c_float, C.c_float, _i64, _vp, _vp, _i32, _vp, _vp, _vp,
                                _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64, _vp]),
+    "bb_parego_score": (C.c_int, [_i32, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float, C.c_float,
+                                  _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64,
+                                  _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),

@@ -11,6 +11,7 @@ import pandas as pd
 from attrs import define, field
 from attrs.validators import instance_of
 
+from baybe_b200 import _lib
 from baybe_b200.engine import AcqConfig
 
 __all__ = [
@@ -20,7 +21,7 @@ __all__ = [
     "UpperConfidenceBound", "qUpperConfidenceBound", "convert_acqf",
     "PM", "PSTD", "qSR", "EI", "qEI", "LogEI", "qLogEI", "PI", "qPI", "UCB", "qUCB",
     "qNoisyExpectedImprovement", "qNEI", "qLogNoisyExpectedImprovement", "qLogNEI",
-    "qExpectedHypervolumeImprovement", "qEHVI", "qLogExpectedHypervolumeImprovement", "qLogEHVI",
+    "qExpectedHypervolumeImprovement", "qEHVI", "qLogExpectedHypervolumeImprovement", "qLogEHVI", "qLogNParEGO",
 ]
 
 
@@ -350,6 +351,52 @@ class qLogExpectedHypervolumeImprovement(_ExpectedHypervolumeImprovement):
     abbreviation: ClassVar[str] = "qLogEHVI"
 
 
+@define(frozen=True)
+class qLogNParEGO(AcquisitionFunction):
+    """acquisition/acqfs.py:328-336: Pareto objectives of 2 to 8 targets on discrete search spaces, scored by
+    ``bb_parego_score`` (``baybe_b200.parego``): random simplex weights, augmented Chebyshev scalarisation of the
+    normalised oriented targets and a qLogNEI of it over the measured rows, pruned as ``prune_baseline`` says (at
+    most 31 points together with the pending points without pruning); tau_relu = 1e-6 and tau_max = 1e-2 as in
+    ``AcqConfig``."""
+
+    abbreviation: ClassVar[str] = "qLogNParEGO"
+    supports_multi_output: ClassVar[bool] = True
+    prune_baseline: bool = field(default=True, validator=instance_of(bool))
+
+    def to_engine(self, surrogate, searchspace, objective, measurements, pending_experiments=None) -> AcqConfig:
+        raise IncompatibleAcquisitionFunctionError(
+            f"'{type(self).__name__}' needs a multi-output objective; it is evaluated by "
+            "baybe_b200.parego.ParegoScorer (see scorer())")
+
+    def scorer(self, surrogate, searchspace, objective, measurements):
+        """Check the objective and the space, fit the per-target surrogates (a ``CompositeSurrogate``), then draw
+        the weights and set up the baseline and its pruning (``baybe_b200.parego.build_parego_scorer``)."""
+        from baybe_b200.multiobjective import _error, target_orientations
+        from baybe_b200.parego import build_parego_scorer
+
+        if not getattr(objective, "is_multi_output", False):
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
+        kind = _space_kind(searchspace)
+        if kind != "DISCRETE":
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
+        n_targets = len(objective.targets)
+        if not 2 <= n_targets <= _lib.PAREGO_MAX_TARGETS:
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"{self.abbreviation} on the B200 engine supports 2 to {_lib.PAREGO_MAX_TARGETS} targets "
+                f"(got {n_targets})")
+        target_orientations(objective)  # before the fit: a target that is not affine raises here
+        surrogate.fit(searchspace, objective, measurements)
+        gps = [s.device_gp for s in surrogate._surrogates_flat]
+        return build_parego_scorer(self, gps, searchspace, objective, measurements)
+
+    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
+                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
+        scorer = self.scorer(surrogate, searchspace, objective, measurements)
+        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
+
+
 qNEI, qLogNEI = qNoisyExpectedImprovement, qLogNoisyExpectedImprovement
 qEHVI, qLogEHVI = qExpectedHypervolumeImprovement, qLogExpectedHypervolumeImprovement
 PM, PSTD, qSR = PosteriorMean, PosteriorStandardDeviation, qSimpleRegret
@@ -357,7 +404,7 @@ EI, qEI, LogEI, qLogEI = ExpectedImprovement, qExpectedImprovement, LogExpectedI
 PI, qPI, UCB, qUCB = ProbabilityOfImprovement, qProbabilityOfImprovement, UpperConfidenceBound, qUpperConfidenceBound
 
 _BY_NAME = {c.__name__: c for c in (PM, PSTD, qSR, EI, qEI, LogEI, qLogEI, PI, qPI, UCB, qUCB, qNEI, qLogNEI,
-                                    qEHVI, qLogEHVI)}
+                                    qEHVI, qLogEHVI, qLogNParEGO)}
 _BY_NAME.update({c.abbreviation: c for c in list(_BY_NAME.values())})
 
 

@@ -77,17 +77,20 @@ class AcqConfig:
     tau_pi: float = 1e-3
 
     def __post_init__(self):
-        if self.kind not in _lib.ACQ_KIND and self.kind not in _lib.NEI_KINDS:
+        if self.kind not in _lib.ACQ_KIND and self.kind not in _lib.NEI_KINDS and self.kind not in _lib.PAREGO_KINDS:
             raise ValueError(f"unsupported acquisition function {self.kind!r}")
 
     @property
     def is_mc(self) -> bool:
-        return self.kind in _lib.MC_KINDS or self.kind in _lib.NEI_KINDS
+        return self.kind in _lib.MC_KINDS or self.kind in _lib.NEI_KINDS or self.kind in _lib.PAREGO_KINDS
 
     def to_c(self) -> _lib.AcqSpec:
         if self.kind in _lib.NEI_KINDS:
             raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.noisy.NeiScorer (discrete spaces) or "
                                       "baybe_b200.hybrid.NeiScorer (hybrid spaces), not by the fused kernels")
+        if self.kind in _lib.PAREGO_KINDS:
+            raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.parego.ParegoScorer, not by the fused "
+                                      "kernels")
         return _lib.AcqSpec(
             _lib.ACQ_KIND[self.kind], int(self.maximize), self.best_f, self.beta, self.obj_scale,
             self.obj_shift, self.tau_relu, self.tau_max, self.tau_pi,
@@ -713,6 +716,50 @@ def _op_nei_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | Non
 @_op_nei_score.register_fake
 def _(mu, var, cross, linv, w, z, g, batch_terms, keep, log_nei, params, index_offset, want_scores):
     return (mu.new_empty(mu.shape[0] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
+
+
+@torch.library.custom_op("baybe_b200::parego_score", mutates_args=())
+def _op_parego_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | None, linv: torch.Tensor | None,
+                     w: torch.Tensor | None, z: torch.Tensor, g: torch.Tensor, batch_terms: torch.Tensor | None,
+                     keep: torch.Tensor | None, weight: list[float], offset: list[float], params: list[float],
+                     index_offset: int, want_scores: bool) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_parego_score``: mu/var [M, N]; with |C| conditioning points cross [M, N, |C|], linv [M, |C|, |C|]
+    (L_C^-1 per target) and w [M, |C|, S] (sample-minor); z [S, M(1 + |C|)]; g [S]; batch_terms [S, Q] for the other
+    Q points of a q-batch; p_m = weight[m] y_m + offset[m]; params = [alpha, tau_relu, tau_max]."""
+    M, N = mu.shape
+    Cn = 0 if cross is None else cross.shape[2]
+    S = z.shape[0]
+    if z.dim() != 2 or z.shape[1] != M * (Cn + 1):
+        raise ValueError(f"base samples must be (S, {M * (Cn + 1)})")
+    if len(weight) != M or len(offset) != M:
+        raise ValueError(f"one scalarisation weight and offset per target ({M})")
+    if g.numel() != S:
+        raise ValueError(f"incumbents must be (S,) = ({S},)")
+    if Cn and (linv is None or tuple(linv.shape) != (M, Cn, Cn) or w is None or tuple(w.shape) != (M, Cn, S)):
+        raise ValueError(f"conditioning needs linv ({M}, {Cn}, {Cn}) and w ({M}, {Cn}, {S})")
+    Q = 0 if batch_terms is None else batch_terms.shape[1]
+    if Q and tuple(batch_terms.shape) != (S, Q):
+        raise ValueError(f"batch terms must be (S, Q) = ({S}, {Q})")
+    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
+        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
+    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
+    key = torch.empty(1, dtype=torch.int64, device=mu.device)
+    alpha, tau_relu, tau_max = (float(v) for v in params)
+    fw = (C.c_float * M)(*weight)
+    fv = (C.c_float * M)(*offset)
+    lib = _lib.load()
+    with torch.cuda.device(mu.device):
+        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        _lib.check(lib.bb_parego_score(M, fw, fv, alpha, tau_relu, tau_max, N, _ptr(mu), _ptr(var), Cn, _ptr(cross),
+                                       _ptr(linv), _ptr(w), _ptr(z), S, _ptr(g), Q, _ptr(batch_terms), _ptr(keep),
+                                       _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
+                                       _stream_ptr()), "bb_parego_score")
+    return score, key
+
+
+@_op_parego_score.register_fake
+def _(mu, var, cross, linv, w, z, g, batch_terms, keep, weight, offset, params, index_offset, want_scores):
+    return (mu.new_empty(mu.shape[1] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
 
 
 def objective_struct(n_targets: int, scalarizer: int, programs, weights) -> _lib.Objective:

@@ -22,7 +22,8 @@ import torch
 from baybe_b200 import _lib
 from baybe_b200.engine import AcqConfig, sobol_normal_samples
 
-__all__ = ["PRUNE_SAMPLES", "PRUNE_SEED", "prune_winners", "kept_points", "NeiScorer", "build_nei_scorer"]
+__all__ = ["PRUNE_SAMPLES", "PRUNE_SEED", "prune_winners", "kept_points", "capped_baseline", "condition_on",
+           "NeiScorer", "build_nei_scorer"]
 
 PRUNE_SAMPLES = 2048  # botorch prune_inferior_points' num_samples
 # botorch draws the pruning samples from the global RNG; a fixed seed keeps the pruned baseline the same in every call
@@ -56,6 +57,35 @@ def kept_points(winners: np.ndarray, counts: np.ndarray, cap: int) -> np.ndarray
     if len(winners) <= cap:
         return winners
     return np.sort(winners[np.argsort(-counts, kind="stable")[:cap]])
+
+
+def capped_baseline(name: str, winners: np.ndarray, counts: np.ndarray, n_rows: int, prune: bool,
+                    n_other: int) -> tuple[np.ndarray, int]:
+    """The baseline rows (indices into the `n_rows` measured rows) that condition an evaluation with `n_other`
+    pending and batch points, and how many winners were left out: ``kept_points`` capped at ``MAX_PENDING`` -
+    `n_other`; without pruning every row, or ``NotImplementedError`` if they do not fit."""
+    cap = _lib.MAX_PENDING - n_other
+    if not prune and n_rows > cap:
+        raise NotImplementedError(
+            f"{name} with prune_baseline=False conditions on all {n_rows} measured rows plus "
+            f"{n_other} pending/batch points; the B200 engine conditions on at most {_lib.MAX_PENDING} points "
+            "(BB_MAX_PENDING): use prune_baseline=True or fewer measurements")
+    if cap < 1:
+        raise NotImplementedError(
+            f"{name} with {n_other} pending/batch points leaves no room for a baseline point; the B200 "
+            f"engine conditions on at most {_lib.MAX_PENDING} points (BB_MAX_PENDING)")
+    kept = kept_points(winners, counts, cap)
+    return kept, len(winners) - len(kept)
+
+
+def condition_on(gp, rows: np.ndarray):
+    """Float64 posterior mean mu [R] of the conditioning rows under one model, the Cholesky factor L [R, R] of their
+    covariance and L^-1, and the (rows, beta) pair ``cross_covariance`` takes for them."""
+    from baybe_b200.multiobjective import _psd_cholesky
+
+    mu, cov, cond = _joint_posterior(gp, rows, with_beta=True)
+    L = _psd_cholesky(0.5 * (cov + cov.T))
+    return mu, L, np.linalg.inv(L), cond
 
 
 def _log_fatplus(u: np.ndarray, tau: float) -> np.ndarray:
@@ -94,18 +124,8 @@ class NeiScorer:
     # ---- candidate-independent set-up of one evaluation ----------------------------------------------------
     def kept_baseline(self, n_other: int) -> np.ndarray:
         """Indices of the baseline rows that condition an evaluation with `n_other` pending and batch points."""
-        cap = _lib.MAX_PENDING - n_other
-        if not self.prune and len(self.baseline) > cap:
-            raise NotImplementedError(
-                f"{self.cfg.kind} with prune_baseline=False conditions on all {len(self.baseline)} measured rows plus "
-                f"{n_other} pending/batch points; the B200 engine conditions on at most {_lib.MAX_PENDING} points "
-                "(BB_MAX_PENDING): use prune_baseline=True or fewer measurements")
-        if cap < 1:
-            raise NotImplementedError(
-                f"{self.cfg.kind} with {n_other} pending/batch points leaves no room for a baseline point; the B200 "
-                f"engine conditions on at most {_lib.MAX_PENDING} points (BB_MAX_PENDING)")
-        kept = kept_points(self.winners, self.counts, cap)
-        self.n_dropped = len(self.winners) - len(kept)
+        kept, self.n_dropped = capped_baseline(self.cfg.kind, self.winners, self.counts, len(self.baseline),
+                                               self.prune, n_other)
         return kept
 
     def n_conditioning(self, n_other: int) -> int:
@@ -122,11 +142,7 @@ class NeiScorer:
         nc, Q = len(rows), len(batch)
         if z.shape[1] != nc + 1:
             raise ValueError(f"base samples must be (S, {nc + 1})")
-        from baybe_b200.multiobjective import _psd_cholesky
-
-        mu, cov, cond = _joint_posterior(self.gp, rows, with_beta=True)
-        L = _psd_cholesky(0.5 * (cov + cov.T))
-        linv = np.linalg.inv(L)
+        mu, L, linv, cond = condition_on(self.gp, rows)
         zc = z[:, :nc]
         o = self.cfg.obj_scale * (mu[None, :] + zc @ L.T) + self.cfg.obj_shift
         g = o[:, : nc - Q].max(axis=1)

@@ -461,6 +461,31 @@ int bb_nei_score(int32_t log_nei, float obj_scale, float obj_shift, float tau_re
                  const float* d_batch_terms, const uint8_t* d_keep, float* d_score, int64_t* d_best_key,
                  int64_t index_offset, void* stream);
 
+/* ---- Pareto objectives by random Chebyshev scalarisation: qLogNParEGO (baybe/acquisition/acqfs.py:328-336, built
+ * with X_baseline = the measured rows at acquisition/_builder.py:195-209, 319-334; set-up on the host by
+ * baybe_b200/parego.py).  n_targets = M in [2, BB_OBJ_MAX_TARGETS], one model per target.  The host folds the oriented
+ * target, its normalisation and the simplex weight into one affine map per target, p_m = weight[m] * y_m + offset[m]
+ * (weight / offset: host arrays of M floats), and scalarises cheb = min_m p_m + alpha * sum_m p_m.  The conditioning
+ * set C (n_cond <= BB_MAX_PENDING points: the pruned baseline, the pending points, then the n_batch other points of a
+ * q-batch) is shared by the targets and sampled jointly per target by the caller:
+ *   d_mu / d_var [M][N], d_cross [M][N][n_cond]: bb_posterior of the candidates per target model, C its pending points;
+ *   d_linv [M][n_cond][n_cond] = L_C,m^-1 (row-major, lower triangular);
+ *   d_w [M][n_cond][S] = L_C,m^-T z_{s,C,m} stored sample-minor (entry (m, j, s) at (m * n_cond + j) * S + s);
+ *   d_z [S][M(n_cond + 1)]: base samples, column m(n_cond+1)+j conditioning point j of target m, m(n_cond+1)+n_cond
+ *     the candidate's;
+ *   d_g [S]: per-sample incumbent, the maximum of cheb over baseline and pending points;
+ *   d_batch_terms [S][n_batch]: per-sample terms of the other batch points (nullable when n_batch = 0).
+ * Per sample y_m = mu_m + c_m . w_m,s + sqrt(max(var_m - |L_C,m^-1 c_m|^2, 0)) z_{s,m(n_cond+1)+n_cond},
+ *   t_s = log tau_relu + log fatplus((cheb_s - g_s) / tau_relu), joined with the batch terms by fatmax (tau_max),
+ *   value = logmeanexp_s.
+ * Writes the value of every candidate to d_score (nullable) and folds d_keep (nullable) and index_offset into
+ * *d_best_key like bb_argmax (initialise with bb_best_init).  S in [1, 1024]. */
+int bb_parego_score(int32_t n_targets, const float* weight, const float* offset, float alpha, float tau_relu,
+                    float tau_max, int64_t N, const float* d_mu, const float* d_var, int32_t n_cond,
+                    const float* d_cross, const float* d_linv, const float* d_w, const float* d_z, int32_t S,
+                    const float* d_g, int32_t n_batch, const float* d_batch_terms, const uint8_t* d_keep,
+                    float* d_score, int64_t* d_best_key, int64_t index_offset, void* stream);
+
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
 int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
