@@ -215,14 +215,98 @@ __device__ __forceinline__ void tc_distances(float (&dacc)[32], uint32_t a2_addr
   wg_commit();
 }
 
+// The chunk loop of one tile with the schedule fixed at compile time: a tensor-core model without task kernel or output
+// scale whose V is one panel of NC = n_chunks sub-blocks.  The same MMAs and the same sums in the same order as the
+// run-time loops of k_fused, as straight-line code: an MMA turn is wait, fence, the chunk's (NC - c) x 12 V MMAs, the
+// next chunk's distances, hand-over; ring slots and operand descriptors are worked out before the turn is asked for.
+// Called by the 128 threads of warpgroup wg; `ring` is the warpgroup's position in the ring of L^-1 tiles.
+template <int FAMILY, int K2, int NC>
+__device__ __forceinline__ void tc_chunks_fixed(const FusedParams& p, const FusedSmem& s, int wg, int t, int lane,
+                                                int it, uint32_t a2_addr, uint32_t ring_addr, RingPos& ring,
+                                                float& mean0, float& mean1, float& vq0, float& vq1) {
+  const uint32_t bt_addr = smem_u32(s.bt), bsplit = (uint32_t)p.n_pad * K2 * 2u;
+  const uint32_t stages = (uint32_t)p.stages_b;
+  const float* alpha_t = s.alpha_s + 2 * (lane & 3);
+  float acc[NC][32];
+#pragma unroll
+  for (int j = 0; j < NC; ++j)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+  float dacc[32];
+  uint32_t slot[NC];    // ring slots of the chunk whose V MMAs are in flight: sub-block c + q reads slot[q]
+  uint64_t b_desc[NC];  // and the descriptors of their hi halves
+  mma_turn_wait(wg);  // the tile's first turn: the distances of chunk 0
+  if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnBegin);
+  tc_distances<K2>(dacc, a2_addr, bt_addr, bsplit);
+  mma_turn_pass(wg);
+  if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnEnd);
+#pragma unroll
+  for (int c = 0; c < NC; ++c) {
+    wg_wait<0>();  // the distances of chunk c, and the V MMAs of chunk c - 1: release their L^-1 tiles
+    if (c > 0 && t == 0)
+#pragma unroll
+      for (int q = 0; q <= NC - c; ++q) mbar_arrive(&s.b_empty[slot[q]]);
+    // kernel values in the accumulator layout = the A-fragment layout of the V MMAs
+    uint32_t ahi[4][4], alo[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int i = 8 * kk + 2 * q;
+        const float k0 = kernel_from_t<FAMILY>(dacc[i] * p.ts_g), k1 = kernel_from_t<FAMILY>(dacc[i + 1] * p.ts_g);
+        const float2 al = *reinterpret_cast<const float2*>(alpha_t + c * kChunk + 8 * (i >> 2));
+        const float mp = fmaf(k0, al.x, k1 * al.y);
+        if ((q & 1) != 0) mean1 += mp;  // accumulator rows ra + 8
+        else mean0 += mp;
+        split_pair(k0 * p.ts_kscale, k1 * p.ts_kscale, ahi[kk][q], alo[kk][q]);
+      }
+#pragma unroll
+    for (int q = 0; q < NC - c; ++q) {
+      slot[q] = ring.slot;
+      b_desc[q] = make_wg_desc<64>(ring_addr + ring.slot * kStageBBytes);
+      mbar_wait(&s.b_full[ring.slot], ring.phase);
+      ring.advance(stages);
+    }
+    mma_turn_wait(wg);
+    if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnBegin);
+    wg_fence();
+    // V[:, sb] += K*[:, chunk c] Linv[sb, chunk c]^T for the sub-blocks sb >= c
+#pragma unroll
+    for (int j = c; j < NC; ++j)
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+        const uint64_t b_hi = b_desc[j - c] + (uint64_t)(kk * 2), b_lo = b_hi + (8192u >> 4);
+        wgmma_64x64_rs(acc[j], ahi[kk], b_hi);
+        wgmma_64x64_rs(acc[j], ahi[kk], b_lo);
+        wgmma_64x64_rs(acc[j], alo[kk], b_hi);
+      }
+    wg_commit();
+    if (c + 1 < NC) tc_distances<K2>(dacc, a2_addr, bt_addr + (uint32_t)(c + 1) * tc_panel<K2>(), bsplit);
+    mma_turn_pass(wg);
+    if (t == 0) trace_ev(p, it, 100 * wg + kEvTurnEnd);
+  }
+  wg_wait<0>();
+  if (t == 0) mbar_arrive(&s.b_empty[slot[0]]);
+#pragma unroll
+  for (int j = 0; j < NC; ++j)
+#pragma unroll
+    for (int i = 0; i < 32; i += 4) {
+      vq0 = fmaf(acc[j][i], acc[j][i], fmaf(acc[j][i + 1], acc[j][i + 1], vq0));
+      vq1 = fmaf(acc[j][i + 2], acc[j][i + 2], fmaf(acc[j][i + 3], acc[j][i + 3], vq1));
+    }
+}
+
 // PRE = true (wide-feature path): the K* block was materialised by k_kmat_wg (wide.cu) and is read from
 // p.kpre instead of being assembled here; FAMILY is then irrelevant.
 // TCK = 32 / 64 (n_pad <= 256, d <= 62, Matern-3/2, -5/2, RBF): the distances of a chunk come from an augmented GEMM on
 // the tensor cores, and its accumulator, converted to kernel values in registers, is the register A operand of the
 // chunk's V MMAs.  Otherwise the distances run on the CUDA cores and the K* chunk goes through shared memory.
-template <int FAMILY, bool PRE, int TCK>
+// NC = 1..4 (tensor-core path only): the model has n_chunks = NC, one V panel and neither task kernel nor output scale,
+// and its chunk loop is tc_chunks_fixed; NC = 0: the run-time loops below.
+template <int FAMILY, bool PRE, int TCK, int NC = 0>
 __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p) {
   constexpr bool TC = TCK > 0;
+  static_assert(NC == 0 || (TC && !PRE && NC <= kPanelSB), "a fixed chunk schedule is one panel of the tensor-core path");
   constexpr int K2 = TC ? TCK : 32;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   FusedSmem s;
@@ -326,7 +410,10 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
     uint8_t* abuf = s.abuf + wg * kABytes;
     const uint64_t a_hi = make_wg_desc<64>(smem_u32(abuf)), a_lo = make_wg_desc<64>(smem_u32(abuf + 8192));
     const uint32_t ring_addr = smem_u32(s.ring_b);
-    uint32_t bcount = 0;  // L^-1 tiles consumed so far: ring slot bcount % stages_b, phase (bcount / stages_b) & 1
+    // L^-1 tiles consumed so far.  Run-time schedule: a count, ring slot bcount % stages_b, phase (bcount / stages_b) & 1
+    // (stepping the position instead costs these instantiations more spills); fixed schedule: the position itself.
+    uint32_t bcount = 0;
+    RingPos ring;
     unsigned rows_have = 0;
     StageRegs regs;
     uint8_t* a2w = s.a2 + wg * 3 * tc_panel<K2>();
@@ -362,7 +449,9 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
         an1 = cand_sqnorm(sm, m1);
       }
       float mean0 = 0.f, mean1 = 0.f, vq0 = 0.f, vq1 = 0.f;
-      for (int lo = 0; lo < C; lo += p.panel_sb) {
+      if constexpr (NC > 0)
+        tc_chunks_fixed<FAMILY, K2, NC>(p, s, wg, t, lane, it, smem_u32(a2w), ring_addr, ring, mean0, mean1, vq0, vq1);
+      for (int lo = 0; lo < (NC > 0 ? 0 : C); lo += p.panel_sb) {  // the run-time schedule (none where it is fixed)
         const int hi = min(C, lo + p.panel_sb);
         const bool last_panel = hi == C;  // covers every chunk: the mean is formed here
         float acc[kPanelSB][32];
@@ -657,14 +746,14 @@ __global__ void __launch_bounds__(kFusedThreads, 1) k_fused(const FusedParams p)
     // =====================================================================================
     setmaxnreg_dec<kProducerRegs>();
     if (warp == kWarpProducer && elect_one()) {
-      uint32_t idx = 0;
+      RingPos ring;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x)
         for (int lo = 0; lo < C; lo += p.panel_sb) {
           const int hi = min(C, lo + p.panel_sb);
           for (int c = 0; c < hi; ++c)
-            for (int sb = c > lo ? c : lo; sb < hi; ++sb, ++idx) {
-              const uint32_t st = idx % (uint32_t)p.stages_b, ph = (idx / (uint32_t)p.stages_b) & 1u;
-              mbar_wait_relaxed(&s.b_empty[st], ph ^ 1u);
+            for (int sb = c > lo ? c : lo; sb < hi; ++sb, ring.advance((uint32_t)p.stages_b)) {
+              const uint32_t st = ring.slot;
+              mbar_wait_relaxed(&s.b_empty[st], ring.phase ^ 1u);
               mbar_expect_tx(&s.b_full[st], kStageBBytes);
               bulk_g2s(s.ring_b + (size_t)st * kStageBBytes, p.rimg + rimg_tile(c, sb, C) * kStageBBytes, kStageBBytes,
                        &s.b_full[st]);
@@ -906,9 +995,9 @@ __global__ void __launch_bounds__(256) k_mc_table_grid(const float* __restrict__
 
 // Launch on `stream`.  after_table: k_mc_table_grid was launched just before, so this is a programmatic dependent
 // launch: the prologue overlaps the table kernel and waits for it (griddepcontrol.wait) only before it reads it.
-template <int FAMILY, bool PRE, int TC = 0>
+template <int FAMILY, bool PRE, int TC = 0, int NC = 0>
 static int launch_one(const FusedParams& p, int grid, size_t smem, cudaStream_t stream, bool after_table) {
-  BB_SMEM_OPTIN_ONCE((k_fused<FAMILY, PRE, TC>));
+  BB_SMEM_OPTIN_ONCE((k_fused<FAMILY, PRE, TC, NC>));
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3((unsigned)grid);
@@ -920,8 +1009,23 @@ static int launch_one(const FusedParams& p, int grid, size_t smem, cudaStream_t 
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = after_table ? 1 : 0;
-  BB_CUDA(cudaLaunchKernelEx(&cfg, k_fused<FAMILY, PRE, TC>, p));
+  BB_CUDA(cudaLaunchKernelEx(&cfg, k_fused<FAMILY, PRE, TC, NC>, p));
   return BB_OK;
+}
+
+// Tensor-core path.  The chunk schedule is fixed at compile time (NC = n_chunks) where the model has neither task
+// kernel nor output scale and its V is one panel, the common case; task models, scaled models and a K = 64 model whose
+// ring only holds a two-sub-block panel run the run-time loops (NC = 0), one instantiation per family and K.
+template <int FAMILY, int TC>
+static int launch_tc(const FusedParams& p, int grid, size_t smem, cudaStream_t stream, bool after_table) {
+  static_assert(kPanelSB == 4, "one case per chunk count of a panel");
+  switch (!p.scaled && p.n_chunks <= p.panel_sb ? p.n_chunks : 0) {
+    case 1: return launch_one<FAMILY, false, TC, 1>(p, grid, smem, stream, after_table);
+    case 2: return launch_one<FAMILY, false, TC, 2>(p, grid, smem, stream, after_table);
+    case 3: return launch_one<FAMILY, false, TC, 3>(p, grid, smem, stream, after_table);
+    case 4: return launch_one<FAMILY, false, TC, 4>(p, grid, smem, stream, after_table);
+    default: return launch_one<FAMILY, false, TC>(p, grid, smem, stream, after_table);
+  }
 }
 
 // The widest V panel (kPanelSB sub-blocks, else 2) whose ring fits, with as many L^-1 stages as fit; returns the
@@ -1064,8 +1168,7 @@ int launch_fused(const bb_model* m, const void* d_x, int32_t layout, int64_t N, 
     });
   return dispatch_family<false>(m->family, [&](auto fam) {
     constexpr int F = decltype(fam)::value;
-    return p.tc == 32 ? launch_one<F, false, 32>(p, grid, smem, stream, dep)
-                      : launch_one<F, false, 64>(p, grid, smem, stream, dep);
+    return p.tc == 32 ? launch_tc<F, 32>(p, grid, smem, stream, dep) : launch_tc<F, 64>(p, grid, smem, stream, dep);
   });
 }
 

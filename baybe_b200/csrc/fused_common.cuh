@@ -113,6 +113,18 @@ __device__ __forceinline__ void bar_compute() { asm volatile("bar.sync 1, 256;" 
 __device__ __forceinline__ void mma_turn_wait(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(4 + wg) : "memory"); }
 __device__ __forceinline__ void mma_turn_pass(int wg) { asm volatile("bar.arrive %0, 256;" ::"r"(5 - wg) : "memory"); }
 
+// Position in the ring of L^-1 tiles: the slot of the next tile and the parity of its mbarriers' current phase.
+// Producer and consumers step it tile by tile (a compare and a wrap, no division by the run-time stage count).
+struct RingPos {
+  uint32_t slot = 0, phase = 0;
+  __device__ __forceinline__ void advance(uint32_t stages) {
+    if (++slot == stages) {
+      slot = 0;
+      phase ^= 1u;
+    }
+  }
+};
+
 template <int N>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N>

@@ -2,7 +2,7 @@
 
 usage: python scripts/trace_timeline.py [posterior|score]
 Prints one line per event (SM clocks since the first one), then per warpgroup the clocks per tile, the share of the
-tile spent in the chunk loop, and how many of one warpgroup's gaps between MMA turns (kernel values and epilogue on the
+tile spent in the chunk loop, the length of its MMA turns, and how many of one warpgroup's gaps between MMA turns (kernel values and epilogue on the
 CUDA cores) see the other warpgroup issue its MMAs."""
 import ctypes as C, sys
 from pathlib import Path
@@ -75,6 +75,9 @@ if len(per_wg) == 2:
     for wg, mine, other in ((0, t0s, t1s), (1, t1s, t0s)):
         # gaps between my turns = time on the CUDA cores (kernel values, epilogue) or waiting
         gaps = [(a1, b0) for (_, a1), (b0, _) in zip(mine, mine[1:]) if lo <= a1 and b0 <= hi]
+        if mine:
+            print(f"wg {wg}: {len(mine)} MMA turns (granted -> MMAs issued), mean {sum(b - a for a, b in mine) / len(mine):.0f} "
+                  f"clocks, longest {max(b - a for a, b in mine)}")
         if gaps:
             print(f"wg {wg}: {len(gaps)} gaps between its MMA turns, mean {sum(b - a for a, b in gaps) / len(gaps):.0f} "
                   f"clocks; the other warpgroup issues MMAs inside {covered(gaps, other)} of them")
