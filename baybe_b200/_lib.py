@@ -9,7 +9,7 @@ import ctypes as C
 from pathlib import Path
 
 LIB_PATH = Path(__file__).resolve().parent / "_C" / "libbaybe_b200.so"
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 # enums (mirror include/baybe_b200.h)
 KERNEL_FAMILY = {"matern12": 0, "matern32": 1, "matern52": 2, "rbf": 3}
@@ -30,6 +30,9 @@ NEI_KINDS = ("qNEI", "qLogNEI")
 # never by the fused kernels: Pareto objectives by random Chebyshev scalarisation, baybe_b200/parego.py
 PAREGO_KINDS = ("qLogNParEGO",)
 PAREGO_MAX_TARGETS = 8  # BB_OBJ_MAX_TARGETS
+# never by the fused kernels: Pareto objectives with a sampled front, baybe_b200/nehvi.py (bb_hvi_decompose, then
+# bb_hvi_score with the qEHVI kind)
+NEHVI_KINDS = ("qNEHVI",)
 MAX_PENDING = 31
 MAX_TRAIN = 1024
 
@@ -149,6 +152,7 @@ _SIGNATURES = {
     "bb_parego_score": (C.c_int, [_i32, C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_float, C.c_float, C.c_float,
                                   _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64,
                                   _vp]),
+    "bb_hvi_decompose": (C.c_int, [_i32, C.POINTER(C.c_double), _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),

@@ -22,6 +22,7 @@ __all__ = [
     "PM", "PSTD", "qSR", "EI", "qEI", "LogEI", "qLogEI", "PI", "qPI", "UCB", "qUCB",
     "qNoisyExpectedImprovement", "qNEI", "qLogNoisyExpectedImprovement", "qLogNEI",
     "qExpectedHypervolumeImprovement", "qEHVI", "qLogExpectedHypervolumeImprovement", "qLogEHVI", "qLogNParEGO",
+    "qNoisyExpectedHypervolumeImprovement", "qNEHVI",
 ]
 
 
@@ -397,14 +398,69 @@ class qLogNParEGO(AcquisitionFunction):
         return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
 
 
+@define(frozen=True)
+class qNoisyExpectedHypervolumeImprovement(AcquisitionFunction):
+    """acquisition/acqfs.py:467-474: Pareto objectives of 2 to 4 targets on discrete search spaces
+    (``baybe_b200.nehvi``): the improvement of a candidate over the sampled front of the measured rows, pruned as
+    ``prune_baseline`` says (at most 31 points together with the pending points without pruning), one exact box
+    decomposition per base sample (``bb_hvi_decompose``) and the hypervolume-improvement kernel ``bb_hvi_score``.
+    ``reference_point``: None (default factor 0.1), a factor, or coordinates in the oriented objective space; the
+    partitioning is always exact."""
+
+    abbreviation: ClassVar[str] = "qNEHVI"
+    supports_multi_output: ClassVar[bool] = True
+    reference_point: float | tuple[float, ...] | None = field(default=None, converter=_reference_point)
+    prune_baseline: bool = field(default=True, validator=instance_of(bool))
+
+    @staticmethod
+    def compute_ref_point(array, maximize=None, factor: float = 0.1):
+        from baybe_b200.multiobjective import compute_ref_point
+
+        return compute_ref_point(array, maximize, factor)
+
+    def to_engine(self, surrogate, searchspace, objective, measurements, pending_experiments=None) -> AcqConfig:
+        raise IncompatibleAcquisitionFunctionError(
+            f"'{type(self).__name__}' needs a multi-output objective; it is evaluated by "
+            "baybe_b200.nehvi.NehviScorer (see scorer())")
+
+    def scorer(self, surrogate, searchspace, objective, measurements):
+        """Check the objective and the space, fit the per-target surrogates (a ``CompositeSurrogate``), then set up
+        the reference point, the baseline and its pruning (``baybe_b200.nehvi.build_nehvi_scorer``)."""
+        from baybe_b200.multiobjective import _error, target_orientations
+        from baybe_b200.nehvi import build_nehvi_scorer
+
+        if not getattr(objective, "is_multi_output", False):
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
+        kind = _space_kind(searchspace)
+        if kind != "DISCRETE":
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
+        n_targets = len(objective.targets)
+        if not 2 <= n_targets <= _lib.HVI_MAX_TARGETS:
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"{self.abbreviation} on the B200 engine supports 2 to {_lib.HVI_MAX_TARGETS} targets "
+                f"(got {n_targets})")
+        target_orientations(objective)  # before the fit: a target that is not affine raises here
+        surrogate.fit(searchspace, objective, measurements)
+        gps = [s.device_gp for s in surrogate._surrogates_flat]
+        return build_nehvi_scorer(self, gps, searchspace, objective, measurements)
+
+    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
+                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
+        scorer = self.scorer(surrogate, searchspace, objective, measurements)
+        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
+
+
 qNEI, qLogNEI = qNoisyExpectedImprovement, qLogNoisyExpectedImprovement
+qNEHVI = qNoisyExpectedHypervolumeImprovement
 qEHVI, qLogEHVI = qExpectedHypervolumeImprovement, qLogExpectedHypervolumeImprovement
 PM, PSTD, qSR = PosteriorMean, PosteriorStandardDeviation, qSimpleRegret
 EI, qEI, LogEI, qLogEI = ExpectedImprovement, qExpectedImprovement, LogExpectedImprovement, qLogExpectedImprovement
 PI, qPI, UCB, qUCB = ProbabilityOfImprovement, qProbabilityOfImprovement, UpperConfidenceBound, qUpperConfidenceBound
 
 _BY_NAME = {c.__name__: c for c in (PM, PSTD, qSR, EI, qEI, LogEI, qLogEI, PI, qPI, UCB, qUCB, qNEI, qLogNEI,
-                                    qEHVI, qLogEHVI, qLogNParEGO)}
+                                    qEHVI, qLogEHVI, qLogNParEGO, qNEHVI)}
 _BY_NAME.update({c.abbreviation: c for c in list(_BY_NAME.values())})
 
 

@@ -74,7 +74,8 @@ class EngineAcquisitionFunction:
         self.X_pending = X_pending
         # what the fused path does not serve: baybe_b200.multiobjective.HviScorer (Pareto),
         # baybe_b200.objectives.ObjectiveScorer (desirability, non-affine single targets) or
-        # baybe_b200.noisy.NeiScorer (qNEI / qLogNEI on discrete spaces) or baybe_b200.parego.ParegoScorer (qLogNParEGO)
+        # baybe_b200.noisy.NeiScorer (qNEI / qLogNEI on discrete spaces), baybe_b200.parego.ParegoScorer (qLogNParEGO)
+        # or baybe_b200.nehvi.NehviScorer (qNEHVI)
         self.scorer = scorer
         self.seed = _draw_sampler_seed()  # botorch samplers draw their seed once, at construction
 
@@ -146,8 +147,9 @@ class B200BotorchRecommender(BayesianRecommender):
         replication is done here -- with BayBE's OWN ``CompositeSurrogate``, which only needs ``fit`` and
         ``posterior_stats`` of its members.  This happens whenever the objective models more than one quantity
         (``Objective._is_multi_model``: Pareto objectives and desirability objectives that are not applied as a
-        pre-transformation).  Pareto objectives recommend with qEHVI / qLogEHVI (``baybe_b200.multiobjective``) or
-        qLogNParEGO (``baybe_b200.parego``), desirability objectives with ``baybe_b200.objectives``."""
+        pre-transformation).  Pareto objectives recommend with qEHVI / qLogEHVI (``baybe_b200.multiobjective``),
+        qNEHVI (``baybe_b200.nehvi``) or qLogNParEGO (``baybe_b200.parego``), desirability objectives with
+        ``baybe_b200.objectives``."""
         multi_model = getattr(objective, "_is_multi_model", objective.is_multi_output)
         if multi_model and isinstance(self._surrogate_model, GaussianProcessSurrogate):
             from baybe.surrogates.composite import CompositeSurrogate
@@ -163,11 +165,11 @@ class B200BotorchRecommender(BayesianRecommender):
         acqf = self._get_acquisition_function(objective)
         self._scorer = None
         if objective.is_multi_output:
-            if getattr(type(acqf), "abbreviation", None) not in _lib.HVI_KINDS + _lib.PAREGO_KINDS:
+            if getattr(type(acqf), "abbreviation", None) not in _lib.HVI_KINDS + _lib.PAREGO_KINDS + _lib.NEHVI_KINDS:
                 raise IncompatibleAcquisitionFunctionError(
                     f"recommending for multi-output objectives on the B200 engine needs "
-                    f"qExpectedHypervolumeImprovement (qEHVI), qLogExpectedHypervolumeImprovement (qLogEHVI) or "
-                    f"qLogNParEGO; "
+                    f"qExpectedHypervolumeImprovement (qEHVI), qLogExpectedHypervolumeImprovement (qLogEHVI), "
+                    f"qNoisyExpectedHypervolumeImprovement (qNEHVI) or qLogNParEGO; "
                     f"'{type(acqf).__name__}' is not implemented (the default for multi-output objectives is "
                     f"qLogNEHVI, bayesian/base.py:73)")
         surrogate = self.get_surrogate(searchspace, objective, measurements)

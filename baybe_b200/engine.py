@@ -77,12 +77,12 @@ class AcqConfig:
     tau_pi: float = 1e-3
 
     def __post_init__(self):
-        if self.kind not in _lib.ACQ_KIND and self.kind not in _lib.NEI_KINDS and self.kind not in _lib.PAREGO_KINDS:
+        if self.kind not in tuple(_lib.ACQ_KIND) + _lib.NEI_KINDS + _lib.PAREGO_KINDS + _lib.NEHVI_KINDS:
             raise ValueError(f"unsupported acquisition function {self.kind!r}")
 
     @property
     def is_mc(self) -> bool:
-        return self.kind in _lib.MC_KINDS or self.kind in _lib.NEI_KINDS or self.kind in _lib.PAREGO_KINDS
+        return self.kind in _lib.MC_KINDS + _lib.NEI_KINDS + _lib.PAREGO_KINDS + _lib.NEHVI_KINDS
 
     def to_c(self) -> _lib.AcqSpec:
         if self.kind in _lib.NEI_KINDS:
@@ -90,6 +90,9 @@ class AcqConfig:
                                       "baybe_b200.hybrid.NeiScorer (hybrid spaces), not by the fused kernels")
         if self.kind in _lib.PAREGO_KINDS:
             raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.parego.ParegoScorer, not by the fused "
+                                      "kernels")
+        if self.kind in _lib.NEHVI_KINDS:
+            raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.nehvi.NehviScorer, not by the fused "
                                       "kernels")
         return _lib.AcqSpec(
             _lib.ACQ_KIND[self.kind], int(self.maximize), self.best_f, self.beta, self.obj_scale,
@@ -649,6 +652,38 @@ def _op_hvi_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | Non
 def _(mu, var, cross, linv, w, z, lower, upper, n_cells, keep, kind, params, obj_scale, obj_shift, index_offset,
       want_scores):
     return (mu.new_empty(mu.shape[1] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
+
+
+@torch.library.custom_op("baybe_b200::hvi_decompose", mutates_args=())
+def _op_hvi_decompose(points: torch.Tensor, n_points: torch.Tensor | None, ref: list[float],
+                      cell_stride: int) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """``bb_hvi_decompose``: points [S, n, M] float32 (maximisation), n_points [S] int32 or None, ref [M] (float64
+    on the host) -> lower/upper [S, cell_stride, M] float32, n_cells [S] int32 (above cell_stride: did not fit) and
+    the hypervolume hv [S] float64 of every sample's points."""
+    if points.dim() != 3 or points.dtype != torch.float32 or not points.is_contiguous():
+        raise ValueError("points must be a contiguous float32 (S, n, M) tensor")
+    S, n, M = points.shape
+    if len(ref) != M:
+        raise ValueError(f"one reference coordinate per target ({M})")
+    if n_points is not None and (n_points.dtype != torch.int32 or n_points.numel() != S):
+        raise ValueError(f"n_points must be an int32 tensor of {S} entries")
+    dev = points.device
+    lower = torch.empty((S, cell_stride, M), dtype=torch.float32, device=dev)
+    upper = torch.empty((S, cell_stride, M), dtype=torch.float32, device=dev)
+    n_cells = torch.empty(S, dtype=torch.int32, device=dev)
+    hv = torch.empty(S, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().bb_hvi_decompose(M, (C.c_double * M)(*ref), S, n, _ptr(points), _ptr(n_points),
+                                                int(cell_stride), _ptr(lower), _ptr(upper), _ptr(n_cells), _ptr(hv),
+                                                _stream_ptr()), "bb_hvi_decompose")
+    return lower, upper, n_cells, hv
+
+
+@_op_hvi_decompose.register_fake
+def _(points, n_points, ref, cell_stride):
+    S, _, M = points.shape
+    return (points.new_empty((S, cell_stride, M)), points.new_empty((S, cell_stride, M)),
+            points.new_empty(S, dtype=torch.int32), points.new_empty(S, dtype=torch.float64))
 
 
 @torch.library.custom_op("baybe_b200::joint_posterior", mutates_args=())

@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define BB_ABI_VERSION 3
+#define BB_ABI_VERSION 4
 
 typedef enum bb_status {
   BB_OK = 0,
@@ -377,6 +377,24 @@ int bb_hvi_score(const bb_acq_spec* a, int32_t n_targets, const float* obj_scale
                  const float* d_w, const float* d_z, int32_t S, const float* d_lower, const float* d_upper,
                  const int32_t* d_n_cells, int32_t cell_stride, const uint8_t* d_keep, float* d_score,
                  int64_t* d_best_key, int64_t index_offset, void* stream);
+
+/* ---- exact box decompositions of S small point sets, one per sample, in the layout bb_hvi_score reads
+ * (qNoisyExpectedHypervolumeImprovement, whose front is sampled: acqfs.py:468-474 via botorch's
+ * qNoisyExpectedHypervolumeImprovement; set-up on the host by baybe_b200/nehvi.py).  Maximisation.
+ *   ref [n_targets]: HOST array of float64, finite; 2 <= n_targets <= BB_HVI_MAX_TARGETS.
+ *   d_points [S][n][n_targets] float32, n in [0, BB_MAX_PENDING]; d_n_points [S] (nullable) uses only the first
+ *     d_n_points[s] points of sample s (clamped to [0, n]).  S in [1, 1024].
+ * For every sample: the points strictly above ref in every output, deduplicated, reduced to the non-dominated ones;
+ * one box per column of the grid over their first n_targets - 1 outputs; then boxes that touch along output j and
+ * share every other bound joined, for j = n_targets - 2 down to 0 -- the same set of boxes as
+ * baybe_b200.multiobjective.box_decomposition of the same points (as float64), in the order of their lower corners
+ * on the grid (the same points always give the same layout).  Writes the boxes to
+ * d_lower / d_upper [S][cell_stride][n_targets] (+inf: an open side), their number to d_n_cells [S] and the
+ * hypervolume of the points (float64) to d_hv [S].  A count above cell_stride (<= BB_HVI_MAX_CELLS) means the
+ * decomposition did not fit: that sample's boxes are incomplete and the caller must not use them. */
+int bb_hvi_decompose(int32_t n_targets, const double* ref, int32_t S, int32_t n, const float* d_points,
+                     const int32_t* d_n_points, int32_t cell_stride, float* d_lower, float* d_upper,
+                     int32_t* d_n_cells, double* d_hv, void* stream);
 
 /* ---- Monte-Carlo (and, for affine MEAN desirability, analytic) acquisition values of an objective that is not
  * affine in the modelled targets: DesirabilityObjective (baybe/objectives/desirability.py:229-264, weighted MEAN or
