@@ -30,6 +30,10 @@ class IncompatibleAcquisitionFunctionError(Exception):
     """Same name/meaning as baybe.exceptions.IncompatibleAcquisitionFunctionError."""
 
 
+def _space_kind(searchspace) -> str:
+    return getattr(getattr(searchspace, "type", None), "name", "DISCRETE")
+
+
 @define(frozen=True)
 class AcquisitionFunction:
     """Base class (acquisition/base.py:29-54): flags derive from the leading ``q``."""
@@ -79,16 +83,22 @@ class AcquisitionFunction:
                             obj_scale=a, obj_shift=b, maximize=cfg.maximize)
         return cfg
 
+    def uses_scorer(self, objective, searchspace) -> bool:
+        """True where ``scorer()`` (a ``baybe_b200.scoring.Scorer``) serves this spec on this objective and search
+        space, False where the fused path does (``to_engine``)."""
+        from baybe_b200.objectives import uses_objective_scorer
+
+        return uses_objective_scorer(objective)
+
     def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
                  pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
         """Acquisition values of the given candidates (acquisition/base.py:112-159)."""
         import torch
 
         from baybe_b200.engine import DEFAULT_MC_SAMPLES
-        from baybe_b200.objectives import uses_objective_scorer
         from baybe_b200.recommenders import _draw_sampler_seed, _scores_for
 
-        if uses_objective_scorer(objective):
+        if self.uses_scorer(objective, searchspace):
             if pending_experiments is not None and not self.supports_pending_experiments:
                 raise IncompatibleAcquisitionFunctionError(
                     f"The chosen acquisition function of type '{type(self).__name__}' "
@@ -131,7 +141,7 @@ class AcquisitionFunction:
         and the compiled objective (``baybe_b200.objectives``)."""
         from baybe_b200.objectives import build_objective_scorer
 
-        kind = getattr(getattr(searchspace, "type", None), "name", "DISCRETE")
+        kind = _space_kind(searchspace)
         if kind != "DISCRETE":
             raise IncompatibleAcquisitionFunctionError(
                 f"'{type(objective).__name__}' with a non-affine objective is served on discrete search spaces only "
@@ -143,12 +153,8 @@ class AcquisitionFunction:
 
 
 def _evaluate_with_scorer(acqf, scorer, candidates: pd.DataFrame, searchspace, pending_experiments, jointly: bool):
-    """``evaluate`` through a scorer that runs its own rounds (``HviScorer``, ``ObjectiveScorer``): one value per
-    candidate, or the joint value of the batch [candidates; pending] with the first candidate scored against the
-    rest."""
-    import numpy as np
-
-    from baybe_b200._lib import MAX_PENDING
+    """``evaluate`` through a ``baybe_b200.scoring.Scorer``: one value per candidate, or the joint value of the batch
+    [candidates; pending] (``Scorer.joint_value``)."""
     from baybe_b200.engine import DEFAULT_MC_SAMPLES
     from baybe_b200.recommenders import _draw_sampler_seed
 
@@ -157,16 +163,11 @@ def _evaluate_with_scorer(acqf, scorer, candidates: pd.DataFrame, searchspace, p
     if pending_experiments is not None and len(pending_experiments) > 0:
         pend = searchspace.transform(pending_experiments, allow_extra=True).to_numpy(dtype="float64")
     seed = _draw_sampler_seed()
-    if jointly and hasattr(scorer, "joint_value"):  # the scorer tells batch points from pending points itself
-        return scorer.joint_value(rows, pend, seed, DEFAULT_MC_SAMPLES)
-    if jointly:  # candidate first, then the rest of the batch and the pending points
-        rest = rows[1:] if pend is None else np.concatenate([rows[1:], pend], axis=0)
-        if len(rest) and not scorer.cfg.is_mc:
+    if jointly:
+        if len(rows) + (0 if pend is None else len(pend)) > 1 and not scorer.cfg.is_mc:
             raise IncompatibleAcquisitionFunctionError(
                 f"'{type(acqf).__name__}' is analytic and cannot value a batch of {len(rows)} points jointly.")
-        if len(rest) > MAX_PENDING:
-            raise NotImplementedError(f"joint evaluation supports at most {MAX_PENDING + 1} points")
-        return float(scorer.scores(rows[:1], rest if len(rest) else None, seed, DEFAULT_MC_SAMPLES)[0])
+        return scorer.joint_value(rows, pend, seed, DEFAULT_MC_SAMPLES)
     return pd.Series(scorer.scores(rows, pend, seed, DEFAULT_MC_SAMPLES), index=candidates.index)
 
 
@@ -237,10 +238,6 @@ class qUpperConfidenceBound(AcquisitionFunction):
         return {"beta": self.beta}
 
 
-def _space_kind(searchspace) -> str:
-    return getattr(getattr(searchspace, "type", None), "name", "DISCRETE")
-
-
 @define(frozen=True)
 class _NoisyExpectedImprovement(AcquisitionFunction):
     """The noisy-EI family on discrete search spaces: ``baybe_b200.noisy.NeiScorer`` (``bb_nei_score``) with the
@@ -261,13 +258,9 @@ class _NoisyExpectedImprovement(AcquisitionFunction):
                 f"'{type(self).__name__}' is scored by baybe_b200.noisy on discrete search spaces only (got {kind})")
         return build_nei_scorer(self, surrogate, searchspace, objective, measurements)
 
-    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
-                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
-        if _space_kind(searchspace) != "DISCRETE":
-            return super().evaluate(candidates, surrogate, searchspace, objective, measurements, pending_experiments,
-                                    jointly=jointly)
-        scorer = self.scorer(surrogate, searchspace, objective, measurements)
-        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
+    def uses_scorer(self, objective, searchspace) -> bool:
+        """Discrete spaces: ``NeiScorer``; hybrid spaces: the fused path (``baybe_b200.hybrid``)."""
+        return _space_kind(searchspace) == "DISCRETE" or super().uses_scorer(objective, searchspace)
 
 
 @define(frozen=True)
@@ -296,14 +289,11 @@ def _reference_point(v):
 
 
 @define(frozen=True)
-class _ExpectedHypervolumeImprovement(AcquisitionFunction):
-    """acquisition/acqfs.py:342-418: Pareto objectives of 2 to 4 targets, scored by ``bb_hvi_score``
-    (``baybe_b200.multiobjective``).  ``reference_point``: None (default factor 0.1), a factor, or coordinates in
-    the oriented objective space; ``alpha``: None or 0.0 (exact partitioning)."""
+class _ScoredAcquisitionFunction(AcquisitionFunction):
+    """Specs for Pareto objectives that only a ``baybe_b200.scoring.Scorer`` serves (``scorer()``)."""
 
     supports_multi_output: ClassVar[bool] = True
-    reference_point: float | tuple[float, ...] | None = field(default=None, converter=_reference_point)
-    alpha: float | None = field(default=None, converter=lambda v: None if v is None else float(v))
+    _scorer_module: ClassVar[str] = ""
 
     @staticmethod
     def compute_ref_point(array, maximize=None, factor: float = 0.1):
@@ -311,31 +301,59 @@ class _ExpectedHypervolumeImprovement(AcquisitionFunction):
 
         return compute_ref_point(array, maximize, factor)
 
+    def uses_scorer(self, objective, searchspace) -> bool:
+        return bool(getattr(objective, "is_multi_output", False))
+
     def to_engine(self, surrogate, searchspace, objective, measurements, pending_experiments=None) -> AcqConfig:
         raise IncompatibleAcquisitionFunctionError(
             f"'{type(self).__name__}' needs a multi-output objective; it is evaluated by "
-            "baybe_b200.multiobjective.HviScorer (see scorer())")
-
-    def scorer(self, surrogate, searchspace, objective, measurements):
-        """Fit the per-target surrogates (a ``CompositeSurrogate``, surrogates/composite.py:96) and set up the
-        reference point and the partitioning of the posterior-mean front."""
-        from baybe_b200.multiobjective import _error, build_hvi_scorer
-
-        if not getattr(objective, "is_multi_output", False):
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
-        kind = getattr(getattr(searchspace, "type", None), "name", "DISCRETE")
-        if kind != "DISCRETE":
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
-        surrogate.fit(searchspace, objective, measurements)
-        gps = [s.device_gp for s in surrogate._surrogates_flat]
-        return build_hvi_scorer(self, gps, searchspace, objective, measurements)
+            f"{self._scorer_module} (see scorer())")
 
     def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
                  pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
         scorer = self.scorer(surrogate, searchspace, objective, measurements)
         return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
+
+    def _check_pareto(self, objective, searchspace, max_targets: int | None = None) -> None:
+        """A multi-output objective on a discrete space and, with `max_targets`, 2 to `max_targets` affine targets
+        (checked before the surrogate fit)."""
+        from baybe_b200.multiobjective import _error, target_orientations
+
+        if not getattr(objective, "is_multi_output", False):
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
+        kind = _space_kind(searchspace)
+        if kind != "DISCRETE":
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
+        if max_targets is None:
+            return
+        n_targets = len(objective.targets)
+        if not 2 <= n_targets <= max_targets:
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"{self.abbreviation} on the B200 engine supports 2 to {max_targets} targets (got {n_targets})")
+        target_orientations(objective)  # a target that is not affine raises here
+
+
+@define(frozen=True)
+class _ExpectedHypervolumeImprovement(_ScoredAcquisitionFunction):
+    """acquisition/acqfs.py:342-418: Pareto objectives of 2 to 4 targets, scored by ``bb_hvi_score``
+    (``baybe_b200.multiobjective``).  ``reference_point``: None (default factor 0.1), a factor, or coordinates in
+    the oriented objective space; ``alpha``: None or 0.0 (exact partitioning)."""
+
+    _scorer_module: ClassVar[str] = "baybe_b200.multiobjective.HviScorer"
+    reference_point: float | tuple[float, ...] | None = field(default=None, converter=_reference_point)
+    alpha: float | None = field(default=None, converter=lambda v: None if v is None else float(v))
+
+    def scorer(self, surrogate, searchspace, objective, measurements):
+        """Fit the per-target surrogates (a ``CompositeSurrogate``, surrogates/composite.py:96) and set up the
+        reference point and the partitioning of the posterior-mean front."""
+        from baybe_b200.multiobjective import build_hvi_scorer
+
+        self._check_pareto(objective, searchspace)
+        surrogate.fit(searchspace, objective, measurements)
+        gps = [s.device_gp for s in surrogate._surrogates_flat]
+        return build_hvi_scorer(self, gps, searchspace, objective, measurements)
 
 
 @define(frozen=True)
@@ -353,7 +371,7 @@ class qLogExpectedHypervolumeImprovement(_ExpectedHypervolumeImprovement):
 
 
 @define(frozen=True)
-class qLogNParEGO(AcquisitionFunction):
+class qLogNParEGO(_ScoredAcquisitionFunction):
     """acquisition/acqfs.py:328-336: Pareto objectives of 2 to 8 targets on discrete search spaces, scored by
     ``bb_parego_score`` (``baybe_b200.parego``): random simplex weights, augmented Chebyshev scalarisation of the
     normalised oriented targets and a qLogNEI of it over the measured rows, pruned as ``prune_baseline`` says (at
@@ -361,45 +379,22 @@ class qLogNParEGO(AcquisitionFunction):
     ``AcqConfig``."""
 
     abbreviation: ClassVar[str] = "qLogNParEGO"
-    supports_multi_output: ClassVar[bool] = True
+    _scorer_module: ClassVar[str] = "baybe_b200.parego.ParegoScorer"
     prune_baseline: bool = field(default=True, validator=instance_of(bool))
-
-    def to_engine(self, surrogate, searchspace, objective, measurements, pending_experiments=None) -> AcqConfig:
-        raise IncompatibleAcquisitionFunctionError(
-            f"'{type(self).__name__}' needs a multi-output objective; it is evaluated by "
-            "baybe_b200.parego.ParegoScorer (see scorer())")
 
     def scorer(self, surrogate, searchspace, objective, measurements):
         """Check the objective and the space, fit the per-target surrogates (a ``CompositeSurrogate``), then draw
         the weights and set up the baseline and its pruning (``baybe_b200.parego.build_parego_scorer``)."""
-        from baybe_b200.multiobjective import _error, target_orientations
         from baybe_b200.parego import build_parego_scorer
 
-        if not getattr(objective, "is_multi_output", False):
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
-        kind = _space_kind(searchspace)
-        if kind != "DISCRETE":
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
-        n_targets = len(objective.targets)
-        if not 2 <= n_targets <= _lib.PAREGO_MAX_TARGETS:
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"{self.abbreviation} on the B200 engine supports 2 to {_lib.PAREGO_MAX_TARGETS} targets "
-                f"(got {n_targets})")
-        target_orientations(objective)  # before the fit: a target that is not affine raises here
+        self._check_pareto(objective, searchspace, _lib.PAREGO_MAX_TARGETS)
         surrogate.fit(searchspace, objective, measurements)
         gps = [s.device_gp for s in surrogate._surrogates_flat]
         return build_parego_scorer(self, gps, searchspace, objective, measurements)
 
-    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
-                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
-        scorer = self.scorer(surrogate, searchspace, objective, measurements)
-        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
-
 
 @define(frozen=True)
-class qNoisyExpectedHypervolumeImprovement(AcquisitionFunction):
+class qNoisyExpectedHypervolumeImprovement(_ScoredAcquisitionFunction):
     """acquisition/acqfs.py:467-474: Pareto objectives of 2 to 4 targets on discrete search spaces
     (``baybe_b200.nehvi``): the improvement of a candidate over the sampled front of the measured rows, pruned as
     ``prune_baseline`` says (at most 31 points together with the pending points without pruning), one exact box
@@ -408,48 +403,19 @@ class qNoisyExpectedHypervolumeImprovement(AcquisitionFunction):
     partitioning is always exact."""
 
     abbreviation: ClassVar[str] = "qNEHVI"
-    supports_multi_output: ClassVar[bool] = True
+    _scorer_module: ClassVar[str] = "baybe_b200.nehvi.NehviScorer"
     reference_point: float | tuple[float, ...] | None = field(default=None, converter=_reference_point)
     prune_baseline: bool = field(default=True, validator=instance_of(bool))
-
-    @staticmethod
-    def compute_ref_point(array, maximize=None, factor: float = 0.1):
-        from baybe_b200.multiobjective import compute_ref_point
-
-        return compute_ref_point(array, maximize, factor)
-
-    def to_engine(self, surrogate, searchspace, objective, measurements, pending_experiments=None) -> AcqConfig:
-        raise IncompatibleAcquisitionFunctionError(
-            f"'{type(self).__name__}' needs a multi-output objective; it is evaluated by "
-            "baybe_b200.nehvi.NehviScorer (see scorer())")
 
     def scorer(self, surrogate, searchspace, objective, measurements):
         """Check the objective and the space, fit the per-target surrogates (a ``CompositeSurrogate``), then set up
         the reference point, the baseline and its pruning (``baybe_b200.nehvi.build_nehvi_scorer``)."""
-        from baybe_b200.multiobjective import _error, target_orientations
         from baybe_b200.nehvi import build_nehvi_scorer
 
-        if not getattr(objective, "is_multi_output", False):
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
-        kind = _space_kind(searchspace)
-        if kind != "DISCRETE":
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
-        n_targets = len(objective.targets)
-        if not 2 <= n_targets <= _lib.HVI_MAX_TARGETS:
-            raise _error("IncompatibleAcquisitionFunctionError")(
-                f"{self.abbreviation} on the B200 engine supports 2 to {_lib.HVI_MAX_TARGETS} targets "
-                f"(got {n_targets})")
-        target_orientations(objective)  # before the fit: a target that is not affine raises here
+        self._check_pareto(objective, searchspace, _lib.HVI_MAX_TARGETS)
         surrogate.fit(searchspace, objective, measurements)
         gps = [s.device_gp for s in surrogate._surrogates_flat]
         return build_nehvi_scorer(self, gps, searchspace, objective, measurements)
-
-    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
-                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False):
-        scorer = self.scorer(surrogate, searchspace, objective, measurements)
-        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
 
 
 qNEI, qLogNEI = qNoisyExpectedImprovement, qLogNoisyExpectedImprovement

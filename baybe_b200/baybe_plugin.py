@@ -93,14 +93,9 @@ class EngineAcquisitionFunction:
             if not self.scorer.cfg.is_mc:
                 raise IncompatibleAcquisitionFunctionError("analytic acquisition functions value single points only")
             out = torch.empty(b, dtype=torch.float64)
-            if hasattr(self.scorer, "joint_value"):  # batch points and pending points play different roles
-                pn = None if pend is None or len(pend) == 0 else pend.cpu().numpy()
-                for i in range(b):
-                    out[i] = self.scorer.joint_value(X[i].cpu().numpy(), pn, self.seed, self.n_mc_samples)
-                return out
+            pn = None if pend is None or len(pend) == 0 else pend.cpu().numpy()
             for i in range(b):
-                rest = X[i, 1:, :] if pend is None else torch.cat([X[i, 1:, :], pend.to(X)], dim=0)
-                out[i] = float(self.scorer.scores(X[i, :1, :], rest.cpu().numpy(), self.seed, self.n_mc_samples)[0])
+                out[i] = self.scorer.joint_value(X[i].cpu().numpy(), pn, self.seed, self.n_mc_samples)
             return out
         gp = self.model.device_gp
         if q == 1 and (pend is None or len(pend) == 0):
@@ -160,8 +155,6 @@ class B200BotorchRecommender(BayesianRecommender):
     # ---- acquisition set-up: the engine config takes the place of the botorch acquisition function ----------
     def _setup_botorch_acqf(self, searchspace, objective, measurements, pending_experiments=None) -> None:
         self._objective = objective
-        from baybe_b200.objectives import uses_objective_scorer
-
         acqf = self._get_acquisition_function(objective)
         self._scorer = None
         if objective.is_multi_output:
@@ -174,8 +167,7 @@ class B200BotorchRecommender(BayesianRecommender):
                     f"qLogNEHVI, bayesian/base.py:73)")
         surrogate = self.get_surrogate(searchspace, objective, measurements)
         spec = mirror_acquisition_function(acqf)
-        discrete_nei = spec.abbreviation in _lib.NEI_KINDS and searchspace.type is SearchSpaceType.DISCRETE
-        if objective.is_multi_output or uses_objective_scorer(objective) or discrete_nei:
+        if spec.uses_scorer(objective, searchspace):
             if pending_experiments is not None and not spec.supports_pending_experiments:
                 raise IncompatibleAcquisitionFunctionError(
                     f"The chosen acquisition function of type '{type(spec).__name__}' "

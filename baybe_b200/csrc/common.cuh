@@ -71,14 +71,18 @@ static inline int device_limits(int* sms, int* max_smem) {
 }
 
 // Opt a kernel into the full dynamic shared-memory carve-out once per device (function-local static per
-// instantiation site), instead of one cudaFuncSetAttribute per launch.
+// instantiation site), instead of one cudaFuncSetAttribute per launch.  The 227 KB a block may opt in to include the
+// kernel's static shared memory, so the dynamic limit is what that leaves.
 #define BB_SMEM_OPTIN_ONCE(kernel)                                                                         \
   do {                                                                                                     \
     static unsigned long long done_mask_ = 0ull;                                                           \
     int dev_ = 0;                                                                                          \
     BB_CUDA(cudaGetDevice(&dev_));                                                                         \
     if (dev_ < 0 || dev_ >= 64 || !((done_mask_ >> dev_) & 1ull)) {                                        \
-      BB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));      \
+      cudaFuncAttributes fa_;                                                                              \
+      BB_CUDA(cudaFuncGetAttributes(&fa_, kernel));                                                        \
+      BB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,                    \
+                                   227 * 1024 - (int)fa_.sharedSizeBytes));                                \
       if (dev_ >= 0 && dev_ < 64) done_mask_ |= 1ull << dev_;                                              \
     }                                                                                                      \
   } while (0)

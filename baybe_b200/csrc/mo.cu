@@ -15,25 +15,14 @@
 // |L^-1 c|^2 is a sum of squares: no cancellation against var for nearly collinear pending points.
 #include <math.h>
 
-#include "acq_math.cuh"
-#include "common.cuh"
+#include "score_common.cuh"
 
 namespace bb {
 
-struct HviParams {
-  int64_t N;
-  const float *mu, *var;      // [M][N]
-  const float* cross;         // [M][N][P]
-  const float* linv;          // [M][P][P] L_PP^-1 per target, row-major
-  const float* w;             // [M][S][P]
-  const float* z;             // [S][M(1+P)]
-  const float *lower, *upper; // [n_dec][C][M]
-  const int32_t* n_cells;     // [n_dec]
-  const uint8_t* keep;
-  float* score;
-  long long* key;
-  int64_t index_offset;
-  int P, S, C, n_dec;
+struct HviParams : ScoreParams {  // C = P pending points; w: [M][S][P]
+  const float *lower, *upper;  // [n_dec][cells][M]
+  const int32_t* n_cells;      // [n_dec]
+  int cells, n_dec;            // cell stride, decompositions (1, or S with pending points)
   float tau_relu, tau_max;
   float a[BB_HVI_MAX_TARGETS], b[BB_HVI_MAX_TARGETS];
 };
@@ -49,19 +38,20 @@ constexpr int kHviThreads = 256;
 template <int M, bool LOG>
 __global__ void __launch_bounds__(kHviThreads) k_hvi(const HviParams p) {
   extern __shared__ __align__(16) float smem_h[];
-  const int P = p.P, S = p.S, Q = P + 1;
+  // float offsets by hand, not SmemCarver: placing the same buffers through it makes ptxas give k_hvi<3, false> 40
+  // registers and spill, and k_hvi<4, true> 48 registers and 84 B of spills
+  const int P = p.C, S = p.S, Q = P + 1;
   float* zc = smem_h;              // [S][M] candidate base samples
   float* linv = zc + S * M;        // [M][P][P]
-  float* cl = linv + M * P * P;    // [C][M] cells of the single decomposition (P = 0)
-  float* cu = cl + p.C * M;
-  __shared__ long long red[kHviThreads / 32];
+  float* cl = linv + M * P * P;    // [cells][M] bounds of the single decomposition (P = 0)
+  float* cu = cl + p.cells * M;
   for (int e = threadIdx.x; e < S * M; e += blockDim.x) {
     const int s = e / M, m = e - s * M;
     zc[e] = __ldg(p.z + (size_t)s * (M * Q) + m * Q + P);
   }
   for (int e = threadIdx.x; e < M * P * P; e += blockDim.x) linv[e] = __ldg(p.linv + e);
   const bool shared_cells = p.n_dec == 1;
-  const int nc0 = shared_cells ? min(__ldg(p.n_cells), p.C) : 0;
+  const int nc0 = shared_cells ? min(__ldg(p.n_cells), p.cells) : 0;
   for (int e = threadIdx.x; e < nc0 * M; e += blockDim.x) {
     cl[e] = __ldg(p.lower + e);
     cu[e] = __ldg(p.upper + e);
@@ -75,18 +65,7 @@ __global__ void __launch_bounds__(kHviThreads) k_hvi(const HviParams p) {
   long long best = kEmptyKey;
   for (int64_t i = warp_global; i < p.N; i += nwarps) {
     float mu[M], sd[M], cm[M];
-#pragma unroll
-    for (int m = 0; m < M; ++m) {
-      mu[m] = __ldg(p.mu + m * p.N + i);
-      const float v = __ldg(p.var + m * p.N + i);
-      float r2 = 0.f;
-      cm[m] = 0.f;
-      if (P > 0) {
-        cm[m] = (lane < P) ? __ldg(p.cross + ((size_t)m * p.N + i) * P + lane) : 0.f;
-        r2 = pending_r2_warp(cm[m], linv + m * P * P, P, lane);
-      }
-      sd[m] = sqrtf(fmaxf(v - r2, 0.f));
-    }
+    warp_cond_moments<M>(p, linv, P, i, lane, mu, sd, cm);
     float run_max = -INFINITY, run_sum = 0.f;  // LOG: logsumexp over samples; else the plain sum
     for (int s0 = 0; s0 < S; s0 += 32) {
       const int s = s0 + lane;
@@ -95,7 +74,7 @@ __global__ void __launch_bounds__(kHviThreads) k_hvi(const HviParams p) {
 #pragma unroll
       for (int m = 0; m < M; ++m) {
         float dm = 0.f;
-        if (P > 0) dm = pending_cw_warp(cm[m], p.w + ((size_t)m * S + (valid ? s : 0)) * P, P);
+        if (P > 0) dm = warp_cond_shift<false>(p.w, cm[m], m, valid ? s : 0, P, S);
         const float zz = valid ? zc[s * M + m] : 0.f;
         y[m] = fmaf(p.a[m], mu[m] + dm + sd[m] * zz, p.b[m]);
       }
@@ -103,9 +82,9 @@ __global__ void __launch_bounds__(kHviThreads) k_hvi(const HviParams p) {
       const float *L = cl, *U = cu;
       int nc = nc0;
       if (!shared_cells) {
-        nc = min(__ldg(p.n_cells + s), p.C);
-        L = p.lower + (size_t)s * p.C * M;
-        U = p.upper + (size_t)s * p.C * M;
+        nc = min(__ldg(p.n_cells + s), p.cells);
+        L = p.lower + (size_t)s * p.cells * M;
+        U = p.upper + (size_t)s * p.cells * M;
       }
       if (LOG) {
         float cmax = -INFINITY, csum = 0.f;
@@ -132,50 +111,24 @@ __global__ void __launch_bounds__(kHviThreads) k_hvi(const HviParams p) {
     }
     float result;
     if (LOG) {
-      for (int o = 16; o > 0; o >>= 1) {
-        const float om = __shfl_xor_sync(0xffffffffu, run_max, o);
-        const float os = __shfl_xor_sync(0xffffffffu, run_sum, o);
-        const float nm = fmaxf(run_max, om);
-        float acc = 0.f;
-        if (run_max > -INFINITY) acc += run_sum * __expf(run_max - nm);
-        if (om > -INFINITY) acc += os * __expf(om - nm);
-        run_max = nm;
-        run_sum = acc;
-      }
+      lse_warp_combine(run_max, run_sum);
       // the M log(tau_relu) of every cell term is added once
       result = run_max + logf(run_sum) - logf((float)S) + (float)M * logf(p.tau_relu);
     } else {
       for (int o = 16; o > 0; o >>= 1) run_sum += __shfl_xor_sync(0xffffffffu, run_sum, o);
       result = run_sum / (float)S;
     }
-    if (lane == 0) {
-      if (p.score) p.score[i] = result;
-      if ((p.keep == nullptr || p.keep[i] != 0) && !(result != result)) {
-        const long long k = pack_key(result, (uint32_t)(i + p.index_offset));
-        best = k > best ? k : best;
-      }
-    }
+    warp_offer_best(p, i, result, lane, best);
   }
-  if (lane == 0) red[threadIdx.x >> 5] = best;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long b = red[0];
-    for (int w = 1; w < kHviThreads / 32; ++w) b = red[w] > b ? red[w] : b;
-    if (b != kEmptyKey) atomicMax(p.key, b);
-  }
+  block_flush_best<kHviThreads>(best, p.key);
 }
 
 template <int M, bool LOG>
-static int launch_hvi(const HviParams& p, cudaStream_t stream) {
-  const size_t smem = ((size_t)p.S * M + (size_t)M * p.P * p.P + (p.n_dec == 1 ? 2 * (size_t)p.C * M : 0)) * 4;
-  // at most 48 KB + 15 KB: S*M samples and, for P = 0 only, 2*C*M cell bounds (S = C = 1024, M = 4), or with P = 31
-  // the S*M samples and M*P*P entries of L^-1; the opt-in covers the dynamic part only, next to `red`
-  BB_CUDA(cudaFuncSetAttribute(k_hvi<M, LOG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int64_t blocks = (p.N + kHviThreads / 32 - 1) / (kHviThreads / 32);
-  if (blocks > kSMs * 4) blocks = kSMs * 4;
-  k_hvi<M, LOG><<<(int)blocks, kHviThreads, smem, stream>>>(p);
-  BB_LAUNCH_CHECK();
-  return BB_OK;
+static int launch_hvi(const HviParams& p, cudaStream_t st) {
+  // at most 48 KB + 15 KB: S*M samples and, for P = 0 only, 2*cells*M bounds (S = cells = 1024, M = 4), or with
+  // P = 31 the S*M samples and M*P*P entries of L^-1
+  const size_t smem = ((size_t)p.S * M + (size_t)M * p.C * p.C + (p.n_dec == 1 ? 2 * (size_t)p.cells * M : 0)) * 4;
+  return launch_warp_per_candidate<k_hvi<M, LOG>, kHviThreads, 4>(p, smem, st);
 }
 
 }  // namespace bb
@@ -196,14 +149,10 @@ extern "C" int bb_hvi_score(const bb_acq_spec* a, int32_t n_targets, const float
   BB_CHECK_SUPPORTED(n_targets >= 2 && n_targets <= BB_HVI_MAX_TARGETS,
                      "bb_hvi_score: n_targets=%d outside [2,%d]", n_targets, BB_HVI_MAX_TARGETS);
   BB_CHECK_ARG(obj_scale != nullptr && obj_shift != nullptr, "bb_hvi_score: null objective scale/shift");
-  BB_CHECK_ARG(N >= 0 && N + index_offset < 0xffffffffLL && index_offset >= 0,
-               "bb_hvi_score: index outside 32-bit key range");
-  BB_CHECK_ARG(n_pending >= 0 && n_pending <= BB_MAX_PENDING, "bb_hvi_score: n_pending=%d outside [0,%d]", n_pending,
-               BB_MAX_PENDING);
-  BB_CHECK_ARG(S >= 1 && S <= 1024, "bb_hvi_score: S=%d outside [1,1024]", S);
+  const int rc = check_score_args("bb_hvi_score", "n_pending", N, index_offset, n_pending, S, true, d_best_key);
+  if (rc != BB_OK) return rc;
   BB_CHECK_SUPPORTED(cell_stride >= 1 && cell_stride <= BB_HVI_MAX_CELLS,
                      "bb_hvi_score: cell_stride=%d outside [1,%d]", cell_stride, BB_HVI_MAX_CELLS);
-  BB_CHECK_ARG(d_best_key != nullptr, "bb_hvi_score: null best key");
   if (N == 0) return BB_OK;
   BB_CHECK_ARG(d_mu && d_var && d_z && d_lower && d_upper && d_n_cells, "bb_hvi_score: null buffer");
   BB_CHECK_ARG(n_pending == 0 || (d_cross && d_linv && d_w), "bb_hvi_score: pending points need cross, linv and w");
@@ -215,16 +164,16 @@ extern "C" int bb_hvi_score(const bb_acq_spec* a, int32_t n_targets, const float
   p.linv = d_linv;
   p.w = d_w;
   p.z = d_z;
-  p.lower = d_lower;
-  p.upper = d_upper;
-  p.n_cells = d_n_cells;
   p.keep = d_keep;
   p.score = d_score;
   p.key = reinterpret_cast<long long*>(d_best_key);
   p.index_offset = index_offset;
-  p.P = n_pending;
+  p.C = n_pending;
   p.S = S;
-  p.C = cell_stride;
+  p.lower = d_lower;
+  p.upper = d_upper;
+  p.n_cells = d_n_cells;
+  p.cells = cell_stride;
   p.n_dec = n_pending == 0 ? 1 : S;
   p.tau_relu = a->tau_relu;
   p.tau_max = a->tau_max;

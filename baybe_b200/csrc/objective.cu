@@ -11,31 +11,18 @@
 // terms (computed once per round on the host, baybe_b200/objectives.py) by max, or fatmax for qLogEI.  The programs are
 // a kernel parameter (bb_objective, 4.2 KB): every lane runs the same opcode, and two streams never share state.
 //
-// Mapping (DESIGN.md section 4.3): one warp per candidate, lane l takes samples l, l+32, ...; the candidate's
-// conditional moments are formed once per warp with the helpers k_hvi uses, the S x M candidate base samples sit in
-// shared memory.  Reductions over lanes are fixed xor trees, so a row's value does not depend on where it runs.
+// Mapping (DESIGN.md section 4.3, score_common.cuh): one warp per candidate, lane l takes samples l, l+32, ...; the
+// S x M candidate base samples sit in shared memory.
 #include <math.h>
 
-#include "acq_math.cuh"
-#include "common.cuh"
+#include "score_common.cuh"
 
 namespace bb {
 
-struct ObjParams {
+struct ObjParams : ScoreParams {  // C = P pending points; w: [M][S][P]
   bb_objective obj;
   bb_acq_spec a;
-  int64_t N;
-  const float *mu, *var;  // [M][N]
-  const float* cross;     // [M][N][P]
-  const float* linv;      // [M][P][P]
-  const float* w;         // [M][S][P]
-  const float* pend;      // [S][P] pending terms
-  const float* z;         // [S][M(1+P)]
-  const uint8_t* keep;
-  float* score;
-  long long* key;
-  int64_t index_offset;
-  int P, S;
+  const float* pend;  // [S][P] pending terms
 };
 
 constexpr int kObjThreads = 256;
@@ -88,10 +75,9 @@ __device__ __forceinline__ float run_program(const bb_obj_instr* prog, int n, fl
 
 __global__ void __launch_bounds__(kObjThreads) k_objective(const __grid_constant__ ObjParams p) {
   extern __shared__ __align__(16) float smem_o[];
-  const int M = p.obj.n_targets, P = p.P, S = p.S, Q = P + 1;
+  const int M = p.obj.n_targets, P = p.C, S = p.S, Q = P + 1;
   float* zc = smem_o;          // [S][M] candidate base samples
   float* linv = zc + S * M;    // [M][P][P]
-  __shared__ long long red[kObjThreads / 32];
   for (int e = threadIdx.x; e < S * M; e += blockDim.x) {
     const int s = e / M, m = e - s * M;
     zc[e] = __ldg(p.z + (size_t)s * (M * Q) + m * Q + P);
@@ -109,6 +95,7 @@ __global__ void __launch_bounds__(kObjThreads) k_objective(const __grid_constant
   const float ucb_c = sqrtf(a.beta * 1.5707963267948966f);
   long long best = kEmptyKey;
   for (int64_t i = warp_global; i < p.N; i += nwarps) {
+    // not warp_cond_moments: M is known only at run time here, and the analytic kinds take sd = var
     float mu[BB_OBJ_MAX_TARGETS], sd[BB_OBJ_MAX_TARGETS], cm[BB_OBJ_MAX_TARGETS];
 #pragma unroll
     for (int m = 0; m < BB_OBJ_MAX_TARGETS; ++m) {
@@ -190,16 +177,9 @@ __global__ void __launch_bounds__(kObjThreads) k_objective(const __grid_constant
         else if (kind == BB_ACQ_QSR) term = o;
         else if (kind == BB_ACQ_QPI) term = 1.0f / (1.0f + __expf(-(o - a.best_f) / a.tau_pi));
         else term = mo + ucb_c * fabsf(o - mo);
-        float mx = term;
-        li_arr[0] = term;
-        const float* pr = p.pend + (size_t)s * P;
-        for (int j = 0; j < P; ++j) {
-          const float v = __ldg(pr + j);
-          li_arr[j + 1] = v;
-          mx = fmaxf(mx, v);
-        }
-        if (kind == BB_ACQ_QLOGEI) lse_push(fatmax_q(li_arr, Q, mx, a.tau_max), run_max, run_sum);
-        else s0a += mx;
+        term = join_terms(term, p.pend + (size_t)s * P, P, li_arr, kind == BB_ACQ_QLOGEI, a.tau_max);
+        if (kind == BB_ACQ_QLOGEI) lse_push(term, run_max, run_sum);
+        else s0a += term;
       }
       if (kind == BB_ACQ_QLOGEI && P == 0) {
         for (int o = 16; o > 0; o >>= 1) {
@@ -215,21 +195,9 @@ __global__ void __launch_bounds__(kObjThreads) k_objective(const __grid_constant
         result = s0a / (float)S;
       }
     }
-    if (lane == 0) {
-      if (p.score) p.score[i] = result;
-      if ((p.keep == nullptr || p.keep[i] != 0) && !(result != result)) {
-        const long long k = pack_key(result, (uint32_t)(i + p.index_offset));
-        best = k > best ? k : best;
-      }
-    }
+    warp_offer_best(p, i, result, lane, best);
   }
-  if (lane == 0) red[threadIdx.x >> 5] = best;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long b = red[0];
-    for (int w = 1; w < kObjThreads / 32; ++w) b = red[w] > b ? red[w] : b;
-    if (b != kEmptyKey) atomicMax(p.key, b);
-  }
+  block_flush_best<kObjThreads>(best, p.key);
 }
 
 // Dry run of one program on the host: opcodes, op count and stack depth (BB_OBJ_MAX_STACK).
@@ -293,40 +261,32 @@ extern "C" int bb_objective_score(const bb_acq_spec* a, const bb_objective* obj,
       BB_CHECK_SUPPORTED(obj->n_ops[m] == 0 || (obj->n_ops[m] == 1 && obj->prog[m][0].op == BB_OBJ_AFFINE),
                          "bb_objective_score: analytic kinds need affine targets (target %d is not)", m);
   }
-  BB_CHECK_ARG(N >= 0 && N + index_offset < 0xffffffffLL && index_offset >= 0,
-               "bb_objective_score: index outside 32-bit key range");
-  BB_CHECK_ARG(n_pending >= 0 && n_pending <= BB_MAX_PENDING, "bb_objective_score: n_pending=%d outside [0,%d]",
-               n_pending, BB_MAX_PENDING);
+  const int rc = check_score_args("bb_objective_score", "n_pending", N, index_offset, n_pending, S, !analytic,
+                                  d_best_key);
+  if (rc != BB_OK) return rc;
   BB_CHECK_ARG(!analytic || n_pending == 0, "bb_objective_score: analytic kinds take no pending points");
-  BB_CHECK_ARG(analytic || (S >= 1 && S <= 1024), "bb_objective_score: S=%d outside [1,1024]", S);
-  BB_CHECK_ARG(d_best_key != nullptr, "bb_objective_score: null best key");
   if (N == 0) return BB_OK;
   BB_CHECK_ARG(d_mu && d_var && (analytic || d_z), "bb_objective_score: null buffer");
   BB_CHECK_ARG(n_pending == 0 || (d_cross && d_linv && d_w && d_pend_terms),
                "bb_objective_score: pending points need cross, linv, w and pending terms");
   ObjParams p;
-  p.obj = *obj;
-  p.a = *a;
   p.N = N;
   p.mu = d_mu;
   p.var = d_var;
   p.cross = d_cross;
   p.linv = d_linv;
   p.w = d_w;
-  p.pend = d_pend_terms;
   p.z = d_z;
   p.keep = d_keep;
   p.score = d_score;
   p.key = reinterpret_cast<long long*>(d_best_key);
   p.index_offset = index_offset;
-  p.P = n_pending;
+  p.C = n_pending;
   p.S = analytic ? 0 : S;
-  // at most 32 KB of candidate samples (S = 1024, M = 8) + 30 KB of L^-1 (M = 8, P = 31), next to `red`
+  p.obj = *obj;
+  p.a = *a;
+  p.pend = d_pend_terms;
+  // at most 32 KB of candidate samples (S = 1024, M = 8) + 30 KB of L^-1 (M = 8, P = 31)
   const size_t smem = ((size_t)p.S * M + (size_t)M * n_pending * n_pending) * 4;
-  BB_CUDA(cudaFuncSetAttribute(k_objective, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int64_t blocks = (N + kObjThreads / 32 - 1) / (kObjThreads / 32);
-  if (blocks > kSMs * 4) blocks = kSMs * 4;
-  k_objective<<<(int)blocks, kObjThreads, smem, (cudaStream_t)stream>>>(p);
-  BB_LAUNCH_CHECK();
-  return BB_OK;
+  return launch_warp_per_candidate<k_objective, kObjThreads, 4>(p, smem, (cudaStream_t)stream);
 }

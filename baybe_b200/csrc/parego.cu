@@ -9,30 +9,18 @@
 // and scalarised by the augmented Chebyshev form cheb_s = min_m p_m,s + alpha sum_m p_m,s.  With the per-sample
 // incumbent g_s (max of cheb over baseline and pending points) and the per-sample terms of the rest of the batch:
 //   value = logmeanexp_s fatmax(log tau_relu + log fatplus((cheb_s - g_s) / tau_relu), terms_s)   (tau_max)
-// Mapping as k_nei: lane l takes samples l, l+32, ...; the conditional moments come from the shared warp helpers of
-// acq_math.cuh, and every reduction over lanes is a fixed xor tree.  M is a template parameter, so the per-target
-// moments of a candidate (mu, sd and the lane's entry of c) stay in registers across the sample loop.
+// Mapping as k_nei (score_common.cuh).  M is a template parameter, so the per-target moments of a candidate (mu, sd
+// and the lane's entry of c) stay in registers across the sample loop.
 #include <math.h>
 
-#include "acq_math.cuh"
-#include "common.cuh"
+#include "score_common.cuh"
 
 namespace bb {
 
-struct ParegoParams {
-  int64_t N;
-  const float *mu, *var;  // [M][N]
-  const float* cross;     // [M][N][C]
-  const float* linv;      // [M][C][C] L_C,m^-1, row-major
-  const float* w;         // [M][C][S] sample-minor
-  const float* z;         // [S][M(C+1)]
-  const float* g;         // [S]
-  const float* terms;     // [S][Q]
-  const uint8_t* keep;
-  float* score;
-  long long* key;
-  int64_t index_offset;
-  int C, S, Q;
+struct ParegoParams : ScoreParams {  // w: [M][C][S] sample-minor
+  const float* g;      // [S]
+  const float* terms;  // [S][Q]
+  int Q;
   float alpha, tau_relu, tau_max;
   float wt[BB_OBJ_MAX_TARGETS], off[BB_OBJ_MAX_TARGETS];  // p_m = wt_m y_m + off_m
 };
@@ -63,7 +51,6 @@ __global__ void __launch_bounds__(kParegoThreads, kParegoBlocksPerSM) k_parego(c
   const int C = p.C, S = p.S, Q = p.Q;
   ParegoSmem sm;
   carve_parego(smem_pe, M, S, C, sm);
-  __shared__ long long red[kParegoThreads / 32];
   const int zld = M * (C + 1);
   for (int e = threadIdx.x; e < M * S; e += blockDim.x) {
     const int m = e / S, s = e - m * S;
@@ -81,18 +68,7 @@ __global__ void __launch_bounds__(kParegoThreads, kParegoBlocksPerSM) k_parego(c
   float li[BB_MAX_PENDING + 1];
   for (int64_t i = warp_global; i < p.N; i += nwarps) {
     float mu[M], sd[M], cm[M];
-#pragma unroll
-    for (int m = 0; m < M; ++m) {
-      const int64_t row = (int64_t)m * p.N + i;
-      mu[m] = __ldg(p.mu + row);
-      float r2 = 0.f;
-      cm[m] = 0.f;
-      if (C > 0) {
-        cm[m] = (lane < C) ? __ldg(p.cross + row * C + lane) : 0.f;
-        r2 = pending_r2_warp(cm[m], sm.linv + m * C * C, C, lane);
-      }
-      sd[m] = sqrtf(fmaxf(__ldg(p.var + row) - r2, 0.f));
-    }
+    warp_cond_moments<M>(p, sm.linv, C, i, lane, mu, sd, cm);
     float run_max = -INFINITY, run_sum = 0.f;  // online logsumexp over the samples
     for (int s0 = 0; s0 < S; s0 += 32) {
       const int s = s0 + lane;
@@ -101,7 +77,7 @@ __global__ void __launch_bounds__(kParegoThreads, kParegoBlocksPerSM) k_parego(c
       float pmin = INFINITY, psum = 0.f;
 #pragma unroll
       for (int m = 0; m < M; ++m) {
-        const float dm = C > 0 ? pending_cw_warp(cm[m], p.w + (size_t)m * C * S + sv, C, S) : 0.f;
+        const float dm = C > 0 ? warp_cond_shift<true>(p.w, cm[m], m, sv, C, S) : 0.f;
         const float pm = fmaf(p.wt[m], mu[m] + dm + sd[m] * sm.zc[m * S + sv], p.off[m]);
         pmin = fminf(pmin, pm);
         psum += pm;
@@ -109,50 +85,22 @@ __global__ void __launch_bounds__(kParegoThreads, kParegoBlocksPerSM) k_parego(c
       if (!valid) continue;
       const float u = fmaf(p.alpha, psum, pmin) - sm.gs[s];
       float term = log_tr + log_fatplus_t(u * inv_tr);
-      if (Q > 0) {
-        float mx = term;
-        li[0] = term;
-        const float* tr = p.terms + (size_t)s * Q;
-        for (int j = 0; j < Q; ++j) {
-          const float v = __ldg(tr + j);
-          li[j + 1] = v;
-          mx = fmaxf(mx, v);
-        }
-        term = fatmax_q(li, Q + 1, mx, p.tau_max);
-      }
+      if (Q > 0) term = join_terms(term, p.terms + (size_t)s * Q, Q, li, true, p.tau_max);
       lse_push(term, run_max, run_sum);
     }
     lse_warp_combine(run_max, run_sum);
     const float result = run_max + logf(run_sum) - logf((float)S);
-    if (lane == 0) {
-      if (p.score) p.score[i] = result;
-      if ((p.keep == nullptr || p.keep[i] != 0) && !(result != result)) {
-        const long long k = pack_key(result, (uint32_t)(i + p.index_offset));
-        best = k > best ? k : best;
-      }
-    }
+    warp_offer_best(p, i, result, lane, best);
   }
-  if (lane == 0) red[threadIdx.x >> 5] = best;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long b = red[0];
-    for (int w = 1; w < kParegoThreads / 32; ++w) b = red[w] > b ? red[w] : b;
-    if (b != kEmptyKey) atomicMax(p.key, b);
-  }
+  block_flush_best<kParegoThreads>(best, p.key);
 }
 
 template <int M>
 static int launch_parego(const ParegoParams& p, cudaStream_t st) {
-  // at most 32 KB of candidate samples + 4 KB of incumbents (S = 1024, M = 8) + 30.75 KB of L^-1 (M = 8, |C| = 31):
-  // above the 48 KB default, so the launch opts in to what it takes (next to `red`)
+  // at most 32 KB of candidate samples + 4 KB of incumbents (S = 1024, M = 8) + 30.75 KB of L^-1 (M = 8, |C| = 31)
   ParegoSmem s;
   const size_t smem = carve_parego(nullptr, M, p.S, p.C, s);
-  BB_CUDA(cudaFuncSetAttribute(k_parego<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int64_t blocks = (p.N + kParegoThreads / 32 - 1) / (kParegoThreads / 32);
-  if (blocks > kSMs * kParegoBlocksPerSM) blocks = kSMs * kParegoBlocksPerSM;
-  k_parego<M><<<(int)blocks, kParegoThreads, smem, st>>>(p);
-  BB_LAUNCH_CHECK();
-  return BB_OK;
+  return launch_warp_per_candidate<k_parego<M>, kParegoThreads, kParegoBlocksPerSM>(p, smem, st);
 }
 
 }  // namespace bb
@@ -173,14 +121,10 @@ extern "C" int bb_parego_score(int32_t n_targets, const float* weight, const flo
                  "bb_parego_score: scalarisation weight/offset of target %d not finite", m);
   BB_CHECK_ARG(isfinite(alpha), "bb_parego_score: alpha not finite");
   BB_CHECK_ARG(tau_relu > 0.f && tau_max > 0.f, "bb_parego_score: needs tau_relu > 0 and tau_max > 0");
-  BB_CHECK_ARG(N >= 0 && N + index_offset < 0xffffffffLL && index_offset >= 0,
-               "bb_parego_score: index outside 32-bit key range");
-  BB_CHECK_ARG(n_cond >= 0 && n_cond <= BB_MAX_PENDING, "bb_parego_score: n_cond=%d outside [0,%d]", n_cond,
-               BB_MAX_PENDING);
+  const int rc = check_score_args("bb_parego_score", "n_cond", N, index_offset, n_cond, S, true, d_best_key);
+  if (rc != BB_OK) return rc;
   BB_CHECK_ARG(n_batch >= 0 && n_batch <= n_cond, "bb_parego_score: n_batch=%d outside [0,n_cond=%d]", n_batch,
                n_cond);
-  BB_CHECK_ARG(S >= 1 && S <= 1024, "bb_parego_score: S=%d outside [1,1024]", S);
-  BB_CHECK_ARG(d_best_key != nullptr, "bb_parego_score: null best key");
   if (N == 0) return BB_OK;
   BB_CHECK_ARG(d_mu && d_var && d_z && d_g, "bb_parego_score: null buffer");
   BB_CHECK_ARG(n_cond == 0 || (d_cross && d_linv && d_w),
@@ -194,14 +138,14 @@ extern "C" int bb_parego_score(int32_t n_targets, const float* weight, const flo
   p.linv = d_linv;
   p.w = d_w;
   p.z = d_z;
-  p.g = d_g;
-  p.terms = d_batch_terms;
   p.keep = d_keep;
   p.score = d_score;
   p.key = reinterpret_cast<long long*>(d_best_key);
   p.index_offset = index_offset;
   p.C = n_cond;
   p.S = S;
+  p.g = d_g;
+  p.terms = d_batch_terms;
   p.Q = n_batch;
   p.alpha = alpha;
   p.tau_relu = tau_relu;

@@ -587,6 +587,20 @@ def _(mu, var, cross, pend_mu, pend_cov, z, kind, params):
     return torch.empty_like(mu)
 
 
+def _check_keep(keep: torch.Tensor | None, N: int) -> None:
+    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
+        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
+
+
+def _score_and_key(N: int, want_scores: bool, device) -> tuple[torch.Tensor, torch.Tensor]:
+    """The outputs of a scoring op: scores [N] (empty without `want_scores`) and the packed best key, initialised on
+    the current stream (called under ``torch.cuda.device(device)``)."""
+    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=device)
+    key = torch.empty(1, dtype=torch.int64, device=device)
+    _lib.check(_lib.load().bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+    return score, key
+
+
 @torch.library.custom_op("baybe_b200::score_fused", mutates_args=())
 def _op_score_fused(x: torch.Tensor, keep: torch.Tensor | None, z: torch.Tensor | None, handle: int,
                     kind: int, params: list[float], index_offset: int,
@@ -595,14 +609,11 @@ def _op_score_fused(x: torch.Tensor, keep: torch.Tensor | None, z: torch.Tensor 
     acq = AcqConfig.from_params(kind, params).to_c()
     lay, ld = _layout_of(x)
     N = x.shape[0]
-    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=x.device)
-    key = torch.empty(1, dtype=torch.int64, device=x.device)
-    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
-        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
+    _check_keep(keep, N)
     S = 0 if z is None else z.numel()
     lib = _lib.load()
     with torch.cuda.device(x.device):
-        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        score, key = _score_and_key(N, want_scores, x.device)
         _lib.check(lib.bb_score_fused(C.byref(gp.model), C.byref(acq), _ptr(x), lay, N, ld, _ptr(keep),
                                       _ptr(z), S, _ptr(score) if want_scores else None, _ptr(key),
                                       index_offset, _stream_ptr()), "bb_score_fused")
@@ -632,15 +643,12 @@ def _op_hvi_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | Non
     if lower.shape != upper.shape or lower.dim() != 3 or lower.shape[2] != M or n_cells.numel() != lower.shape[0] \
             or n_cells.dtype != torch.int32 or lower.shape[0] != (1 if P == 0 else S):
         raise ValueError("cells must be lower/upper [n_dec, C, M] with n_cells [n_dec] (n_dec = 1 or S)")
-    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
-        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
-    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
-    key = torch.empty(1, dtype=torch.int64, device=mu.device)
+    _check_keep(keep, N)
     fa = (C.c_float * M)(*obj_scale)
     fb = (C.c_float * M)(*obj_shift)
     lib = _lib.load()
     with torch.cuda.device(mu.device):
-        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        score, key = _score_and_key(N, want_scores, mu.device)
         _lib.check(lib.bb_hvi_score(C.byref(acq), M, fa, fb, N, _ptr(mu), _ptr(var), P, _ptr(cross), _ptr(linv),
                                     _ptr(w), _ptr(z), S, _ptr(lower), _ptr(upper), _ptr(n_cells), lower.shape[1],
                                     _ptr(keep), _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
@@ -733,14 +741,11 @@ def _op_nei_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | Non
     Q = 0 if batch_terms is None else batch_terms.shape[1]
     if Q and tuple(batch_terms.shape) != (S, Q):
         raise ValueError(f"batch terms must be (S, Q) = ({S}, {Q})")
-    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
-        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
-    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
-    key = torch.empty(1, dtype=torch.int64, device=mu.device)
+    _check_keep(keep, N)
     a, b, tau_relu, tau_max = (float(v) for v in params)
     lib = _lib.load()
     with torch.cuda.device(mu.device):
-        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        score, key = _score_and_key(N, want_scores, mu.device)
         _lib.check(lib.bb_nei_score(int(log_nei), a, b, tau_relu, tau_max, N, _ptr(mu), _ptr(var), Cn, _ptr(cross),
                                     _ptr(linv), _ptr(w), _ptr(z), S, _ptr(g), Q, _ptr(batch_terms), _ptr(keep),
                                     _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
@@ -775,16 +780,13 @@ def _op_parego_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | 
     Q = 0 if batch_terms is None else batch_terms.shape[1]
     if Q and tuple(batch_terms.shape) != (S, Q):
         raise ValueError(f"batch terms must be (S, Q) = ({S}, {Q})")
-    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
-        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
-    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
-    key = torch.empty(1, dtype=torch.int64, device=mu.device)
+    _check_keep(keep, N)
     alpha, tau_relu, tau_max = (float(v) for v in params)
     fw = (C.c_float * M)(*weight)
     fv = (C.c_float * M)(*offset)
     lib = _lib.load()
     with torch.cuda.device(mu.device):
-        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        score, key = _score_and_key(N, want_scores, mu.device)
         _lib.check(lib.bb_parego_score(M, fw, fv, alpha, tau_relu, tau_max, N, _ptr(mu), _ptr(var), Cn, _ptr(cross),
                                        _ptr(linv), _ptr(w), _ptr(z), S, _ptr(g), Q, _ptr(batch_terms), _ptr(keep),
                                        _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
@@ -832,18 +834,15 @@ def _op_objective_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor
         raise ValueError(f"base samples must be (S, {M * (1 + P)})")
     if P and (pend_terms is None or tuple(pend_terms.shape) != (S, P)):
         raise ValueError(f"pending terms must be (S, P) = ({S}, {P})")
-    if keep is not None and (keep.dtype != torch.uint8 or keep.numel() != N or not keep.is_contiguous()):
-        raise ValueError("keep mask must be a contiguous uint8 tensor with one entry per candidate")
+    _check_keep(keep, N)
     progs, k = [], 0
     for n in n_ops:
         progs.append([(ops[k + i], args[3 * (k + i): 3 * (k + i) + 3]) for i in range(n)])
         k += n
     obj = objective_struct(M, scalarizer, progs, weights)
-    score = torch.empty(N if want_scores else 0, dtype=torch.float32, device=mu.device)
-    key = torch.empty(1, dtype=torch.int64, device=mu.device)
     lib = _lib.load()
     with torch.cuda.device(mu.device):
-        _lib.check(lib.bb_best_init(_ptr(key), _stream_ptr()), "bb_best_init")
+        score, key = _score_and_key(N, want_scores, mu.device)
         _lib.check(lib.bb_objective_score(C.byref(acq), C.byref(obj), N, _ptr(mu), _ptr(var), P, _ptr(cross),
                                           _ptr(linv), _ptr(w), _ptr(pend_terms), _ptr(z), S, _ptr(keep),
                                           _ptr(score) if want_scores else None, _ptr(key), int(index_offset),

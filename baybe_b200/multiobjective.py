@@ -18,7 +18,8 @@ import numpy as np
 import torch
 
 from baybe_b200 import _lib
-from baybe_b200.engine import AcqConfig, sobol_normal_samples
+from baybe_b200.engine import AcqConfig
+from baybe_b200.scoring import Scorer
 
 class IncompleteMeasurementsError(Exception):
     """Same name/meaning as baybe.exceptions.IncompleteMeasurementsError."""
@@ -149,7 +150,7 @@ def _padded(decomps: list[tuple[np.ndarray, np.ndarray]], M: int):
     return lower, upper, counts, C
 
 
-class HviScorer:
+class HviScorer(Scorer):
     """qEHVI / qLogEHVI over one model per target.  `scales`/`shifts` orient target m as o_m = a_m y_m + b_m;
     `front` holds the oriented posterior means at the training inputs; `ref_point` is in the oriented space."""
 
@@ -220,26 +221,12 @@ class HviScorer:
         if self.cfg.kind == "qEHVI":
             return lambda v: v + gain
         lg = math.log(gain)
-        return lambda v: float(np.logaddexp(lg, v))
+        return lambda v: np.logaddexp(lg, v)
 
-    # ---- the interfaces the recommenders use -------------------------------------------------------------------
-    def base_samples(self, n_samples: int, n_pending: int, seed: int) -> torch.Tensor:
-        """Scrambled Sobol normals of dimension M(1+P): column m(1+P)+j is pending point j of target m, the last
-        column of each target block the candidate."""
-        return sobol_normal_samples(n_samples, self.M * (1 + n_pending), seed)
-
-    def round_best(self, x, pend: np.ndarray, keep, index_offset: int, seed: int, n_samples: int):
-        """One sequential-greedy round: (packed best key, report) -- see ``greedy_select``."""
-        P = len(pend)
-        _, key, report = self.values(x, pend if P else None, self.base_samples(n_samples, P, seed), keep,
-                                     index_offset, want_scores=False)
-        return key, report
-
-    def scores(self, x, pend: np.ndarray | None, seed: int, n_samples: int) -> np.ndarray:
-        """Acquisition value of [x_i; pending] for every row (float64 host array)."""
-        P = 0 if pend is None else len(pend)
-        s, _, report = self.values(x, pend if P else None, self.base_samples(n_samples, P, seed))
-        return np.array([report(float(v)) for v in s.double().cpu().numpy()])
+    def n_sample_columns(self, n_other: int) -> int:
+        """M(1+P): column m(1+P)+j is pending point j of target m, the last column of each target block the
+        candidate."""
+        return self.M * (1 + n_other)
 
 
 def _psd_cholesky(K: np.ndarray) -> np.ndarray:

@@ -21,9 +21,9 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from baybe_b200 import _lib, noisy
-from baybe_b200.engine import AcqConfig, sobol_normal_samples
-from baybe_b200.noisy import PRUNE_SAMPLES, PRUNE_SEED, capped_baseline, condition_on
+from baybe_b200 import _lib
+from baybe_b200.engine import AcqConfig
+from baybe_b200.noisy import PRUNE_SAMPLES, PRUNE_SEED, BaselineScorer
 
 __all__ = ["pareto_mask", "NehviScorer", "build_nehvi_scorer"]
 
@@ -56,76 +56,43 @@ def pareto_mask(Y: np.ndarray, ref: np.ndarray) -> np.ndarray:
     return ~(ge & gt).any(-2) & (Y > ref).all(-1)
 
 
-class NehviScorer:
-    """qNEHVI over one model per target; the interface of ``ParegoScorer`` (``values``, ``round_best``, ``scores``,
-    ``base_samples``, ``joint_value``, ``n_dropped``).  `scales`/`shifts` orient target m as o_m = a_m y_m + b_m;
-    `ref_point` is in the oriented space; `baseline`: the measured rows (raw comp-rep).  With `prune`, the baseline is
-    pruned once, from ``PRUNE_SAMPLES`` joint posterior samples drawn with `prune_seed`."""
+class NehviScorer(BaselineScorer):
+    """qNEHVI over one model per target.  `scales`/`shifts` orient target m as o_m = a_m y_m + b_m; `ref_point` is in
+    the oriented space; `baseline`: the measured rows (raw comp-rep).  With `prune`, the baseline is pruned once, from
+    ``PRUNE_SAMPLES`` joint posterior samples drawn with `prune_seed`, to the rows on the sampled Pareto front."""
 
     def __init__(self, gps, cfg: AcqConfig, scales, shifts, ref_point, baseline, prune: bool = True,
                  prune_seed: int = PRUNE_SEED):
-        from baybe_b200.multiobjective import _error, _psd_cholesky
+        from baybe_b200.multiobjective import _error
 
         if cfg.kind not in _lib.NEHVI_KINDS:
             raise ValueError(f"{cfg.kind} is not a noisy hypervolume acquisition function")
-        self.gps, self.cfg, self.prune = list(gps), cfg, bool(prune)
-        self.M = len(self.gps)
-        if not 2 <= self.M <= _lib.HVI_MAX_TARGETS:
+        M = len(gps)
+        if not 2 <= M <= _lib.HVI_MAX_TARGETS:
             raise _error("IncompatibleAcquisitionFunctionError")(
-                f"{cfg.kind} on the B200 engine supports 2 to {_lib.HVI_MAX_TARGETS} targets (got {self.M}); "
+                f"{cfg.kind} on the B200 engine supports 2 to {_lib.HVI_MAX_TARGETS} targets (got {M}); "
                 "above that the reference partitions approximately")
-        self.device = self.gps[0].device
+        super().__init__(gps, cfg, baseline, prune)
         self.a = np.asarray(scales, dtype=np.float64).reshape(self.M)
         self.b = np.asarray(shifts, dtype=np.float64).reshape(self.M)
         self.ref = np.asarray(ref_point, dtype=np.float64).reshape(self.M)
-        self.baseline = np.asarray(baseline, dtype=np.float64).reshape(-1, self.gps[0].d)
         n = len(self.baseline)
-        self.winners, self.counts = np.arange(n), np.ones(n, dtype=np.int64)
         if self.prune and n > 0:
-            post = [noisy._joint_posterior(gp, self.baseline)[:2] for gp in self.gps]
-            z = sobol_normal_samples(PRUNE_SAMPLES, self.M * n, prune_seed).numpy()
-            Ls = [_psd_cholesky(0.5 * (cov + cov.T)) for _, cov in post]
+            mus, Ls, z = self.prune_samples(prune_seed)
             counts = np.zeros(n, dtype=np.int64)
             for s0 in range(0, PRUNE_SAMPLES, _PRUNE_CHUNK):
                 zs = z[s0:s0 + _PRUNE_CHUNK]
-                Y = np.stack([post[m][0][None, :] + zs[:, m * n:(m + 1) * n] @ Ls[m].T for m in range(self.M)], -1)
+                Y = np.stack([mus[m][None, :] + zs[:, m * n:(m + 1) * n] @ Ls[m].T for m in range(self.M)], -1)
                 counts += pareto_mask(Y * self.a + self.b, self.ref).sum(0)
             self.winners = np.flatnonzero(counts)
             self.counts = counts[self.winners]
-        self.n_dropped = 0
-
-    # ---- candidate-independent set-up of one evaluation ----------------------------------------------------
-    def kept_baseline(self, n_other: int) -> np.ndarray:
-        """Indices of the baseline rows that condition an evaluation with `n_other` pending and batch points."""
-        kept, self.n_dropped = capped_baseline(self.cfg.kind, self.winners, self.counts, len(self.baseline),
-                                               self.prune, n_other)
-        return kept
-
-    def n_conditioning(self, n_other: int) -> int:
-        return len(self.kept_baseline(n_other)) + n_other
 
     def conditioning(self, pend: np.ndarray | None, batch: np.ndarray | None, z: np.ndarray):
         """C = [kept baseline; pending; batch] rows; per target L_C^-1 [M, |C|, |C|] and w = (L_C^-T z_C)^T
         [M, S, |C|], the oriented samples of C [S, |C|, M] and the (rows, beta) pair of C per target for
         ``cross_covariance``, all float64.  z: (S, M(1 + |C|)), column m(1 + |C|) + j = point j of target m."""
-        d = self.gps[0].d
-        pend = np.zeros((0, d)) if pend is None else np.asarray(pend, dtype=np.float64).reshape(-1, d)
-        batch = np.zeros((0, d)) if batch is None else np.asarray(batch, dtype=np.float64).reshape(-1, d)
-        rows = np.concatenate([self.baseline[self.kept_baseline(len(pend) + len(batch))], pend, batch])
-        nc, M = len(rows), self.M
-        if z.shape[1] != M * (nc + 1):
-            raise ValueError(f"base samples must be (S, {M * (nc + 1)})")
-        S = z.shape[0]
-        linv, w, Y, conds = np.zeros((M, nc, nc)), np.zeros((M, S, nc)), np.zeros((S, nc, M)), []
-        if nc == 0:
-            return rows, linv, w, Y, conds
-        for m, gp in enumerate(self.gps):
-            mu, L, linv[m], cond = condition_on(gp, rows)
-            zc = z[:, m * (nc + 1): m * (nc + 1) + nc]
-            Y[:, :, m] = mu[None, :] + zc @ L.T
-            w[m] = zc @ linv[m]
-            conds.append(cond)
-        return rows, linv, w, Y * self.a + self.b, conds
+        rows, linv, w, Y, conds = self.condition(pend, batch, z)
+        return rows, linv, w, (Y * self.a + self.b if len(rows) else Y), conds
 
     def _decompose(self, points: np.ndarray):
         lower, upper, n_cells, hv = _hvi_decompose(points, self.ref, self.device)
@@ -167,27 +134,6 @@ class NehviScorer:
             keep, _lib.ACQ_KIND["qEHVI"], AcqConfig(kind="qEHVI").params(), [float(v) for v in self.a],
             [float(v) for v in self.b], int(index_offset), bool(want_scores))
         return (scores if want_scores else None), key, ((lambda v: v + gain) if gain > 0.0 else (lambda v: v))
-
-    # ---- the interfaces the recommenders use -------------------------------------------------------------------
-    def base_samples(self, n_samples: int, n_pending: int, seed: int) -> torch.Tensor:
-        """Scrambled Sobol normals of dimension M(1 + |C|): per target block the conditioning points in the order of
-        C, then the candidate."""
-        return sobol_normal_samples(n_samples, self.M * (1 + self.n_conditioning(n_pending)), seed)
-
-    def round_best(self, x, pend: np.ndarray, keep, index_offset: int, seed: int, n_samples: int):
-        """One sequential-greedy round: (packed best key, report) -- see ``greedy_select``."""
-        P = len(pend)
-        _, key, report = self.values(x, pend if P else None, self.base_samples(n_samples, P, seed), keep,
-                                     index_offset, want_scores=False)
-        return key, report
-
-    def scores(self, x, pend: np.ndarray | None, seed: int, n_samples: int, batch: np.ndarray | None = None):
-        """Acquisition value of every row given the pending points (and the other points of its q-batch), float64."""
-        n_other = (0 if pend is None else len(pend)) + (0 if batch is None else len(batch))
-        z = self.base_samples(n_samples, n_other, seed)
-        s, _, report = self.values(x, pend if pend is not None and len(pend) else None, z,
-                                   batch=batch if batch is not None and len(batch) else None)
-        return np.array([report(float(v)) for v in s.double().cpu().numpy()])
 
     def joint_value(self, rows, pend: np.ndarray | None, seed: int, n_samples: int) -> float:
         """Value of the q-batch `rows` given the pending points: the first row is the candidate, the others join

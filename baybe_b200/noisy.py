@@ -21,9 +21,10 @@ import torch
 
 from baybe_b200 import _lib
 from baybe_b200.engine import AcqConfig, sobol_normal_samples
+from baybe_b200.scoring import Scorer
 
 __all__ = ["PRUNE_SAMPLES", "PRUNE_SEED", "prune_winners", "kept_points", "capped_baseline", "condition_on",
-           "NeiScorer", "build_nei_scorer"]
+           "BaselineScorer", "NeiScorer", "build_nei_scorer"]
 
 PRUNE_SAMPLES = 2048  # botorch prune_inferior_points' num_samples
 # botorch draws the pruning samples from the global RNG; a fixed seed keeps the pruned baseline the same in every call
@@ -94,32 +95,34 @@ def _log_fatplus(u: np.ndarray, tau: float) -> np.ndarray:
     return math.log(tau) + np.log(np.logaddexp(0.0, t) + 0.1 / (1.0 + t * t))
 
 
-class NeiScorer:
-    """qNEI / qLogNEI over one single-task model with an affine objective o = a y + b (``cfg.obj_scale`` /
-    ``cfg.obj_shift``); the interface of ``HviScorer`` (``values``, ``round_best``, ``scores``, ``base_samples``)
-    plus ``joint_value``.  `baseline`: the measured rows (raw comp-rep).  With `prune`, the baseline is pruned once,
-    from ``PRUNE_SAMPLES`` joint posterior samples drawn with `prune_seed`; every evaluation keeps at most
-    ``MAX_PENDING`` - (its other conditioning points) of the winners and records how many it dropped in
-    ``n_dropped``."""
+class BaselineScorer(Scorer):
+    """A scorer over one model per target that conditions every evaluation on a baseline of measured rows (raw
+    comp-rep) and on the pending and batch points: the base of ``NeiScorer`` (one target), ``ParegoScorer`` and
+    ``NehviScorer``.  The winners of the family's pruning rule, counted over ``PRUNE_SAMPLES`` joint posterior
+    samples, are every row once until the subclass prunes; every evaluation keeps at most ``MAX_PENDING`` - (its other
+    conditioning points) of them and records how many it dropped in ``n_dropped``."""
 
-    def __init__(self, gp, cfg: AcqConfig, baseline, prune: bool = True, prune_seed: int = 0):
-        if cfg.kind not in _lib.NEI_KINDS:
-            raise ValueError(f"{cfg.kind} is not a noisy expected improvement")
-        self.gp, self.cfg, self.prune = gp, cfg, bool(prune)
-        self.device = gp.device
-        self.baseline = np.asarray(baseline, dtype=np.float64).reshape(-1, gp.d)
+    def __init__(self, gps, cfg: AcqConfig, baseline, prune: bool):
+        self.gps, self.cfg, self.prune = list(gps), cfg, bool(prune)
+        self.M = len(self.gps)
+        self.device = self.gps[0].device
+        self.baseline = np.asarray(baseline, dtype=np.float64).reshape(-1, self.gps[0].d)
         n = len(self.baseline)
-        if n == 0:
-            raise ValueError("noisy expected improvement needs at least one measured row")
         self.winners, self.counts = np.arange(n), np.ones(n, dtype=np.int64)
-        if self.prune and n > 1:
-            mu, cov, _ = _joint_posterior(gp, self.baseline)
-            from baybe_b200.multiobjective import _psd_cholesky
-
-            L = _psd_cholesky(0.5 * (cov + cov.T))
-            z = sobol_normal_samples(PRUNE_SAMPLES, n, prune_seed).numpy()
-            self.winners, self.counts = prune_winners(cfg.obj_scale * (mu[None, :] + z @ L.T) + cfg.obj_shift)
         self.n_dropped = 0
+
+    def prune_samples(self, prune_seed: int, post=None):
+        """The pruning draw: per target the float64 posterior mean of the baseline and the Cholesky factor of its
+        covariance, and z (PRUNE_SAMPLES, M n), column block m for target m.  `post`: the (mean, covariance) pairs if
+        the caller already has them."""
+        from baybe_b200.multiobjective import _psd_cholesky
+
+        n = len(self.baseline)
+        if post is None:
+            post = [_joint_posterior(gp, self.baseline)[:2] for gp in self.gps]
+        Ls = [_psd_cholesky(0.5 * (cov + cov.T)) for _, cov in post]
+        z = sobol_normal_samples(PRUNE_SAMPLES, self.M * n, prune_seed).numpy()
+        return [mu for mu, _ in post], Ls, z
 
     # ---- candidate-independent set-up of one evaluation ----------------------------------------------------
     def kept_baseline(self, n_other: int) -> np.ndarray:
@@ -131,26 +134,63 @@ class NeiScorer:
     def n_conditioning(self, n_other: int) -> int:
         return len(self.kept_baseline(n_other)) + n_other
 
+    def n_sample_columns(self, n_other: int) -> int:
+        """M(1 + |C|): per target block the conditioning points in the order of C, then the candidate."""
+        return self.M * (1 + self.n_conditioning(n_other))
+
+    def condition(self, pend: np.ndarray | None, batch: np.ndarray | None, z: np.ndarray):
+        """C = [kept baseline; pending; batch] rows and, per target, L_C^-1 [M, |C|, |C|], w = (L_C^-T z_C)^T
+        [M, S, |C|], the joint samples of C [S, |C|, M] and the (rows, beta) pair of C for ``cross_covariance``, all
+        float64.  z: (S, M(1 + |C|)), column m(1 + |C|) + j = point j of target m."""
+        d = self.gps[0].d
+        pend = np.zeros((0, d)) if pend is None else np.asarray(pend, dtype=np.float64).reshape(-1, d)
+        batch = np.zeros((0, d)) if batch is None else np.asarray(batch, dtype=np.float64).reshape(-1, d)
+        rows = np.concatenate([self.baseline[self.kept_baseline(len(pend) + len(batch))], pend, batch])
+        nc, M = len(rows), self.M
+        if z.shape[1] != M * (nc + 1):
+            raise ValueError(f"base samples must be (S, {M * (nc + 1)})")
+        S = z.shape[0]
+        linv, w, Y, conds = np.zeros((M, nc, nc)), np.zeros((M, S, nc)), np.zeros((S, nc, M)), []
+        for m, gp in enumerate(self.gps if nc else ()):
+            mu, L, linv[m], cond = condition_on(gp, rows)
+            zc = z[:, m * (nc + 1): m * (nc + 1) + nc]
+            Y[:, :, m] = mu[None, :] + zc @ L.T
+            w[m] = zc @ linv[m]
+            conds.append(cond)
+        return rows, linv, w, Y, conds
+
+
+class NeiScorer(BaselineScorer):
+    """qNEI / qLogNEI over one single-task model with an affine objective o = a y + b (``cfg.obj_scale`` /
+    ``cfg.obj_shift``).  `baseline`: the measured rows (raw comp-rep).  With `prune`, the baseline is pruned once,
+    from ``PRUNE_SAMPLES`` joint posterior samples drawn with `prune_seed`, to the rows that are the arg-max of o in
+    at least one sample."""
+
+    def __init__(self, gp, cfg: AcqConfig, baseline, prune: bool = True, prune_seed: int = 0):
+        if cfg.kind not in _lib.NEI_KINDS:
+            raise ValueError(f"{cfg.kind} is not a noisy expected improvement")
+        super().__init__([gp], cfg, baseline, prune)
+        self.gp = gp
+        n = len(self.baseline)
+        if n == 0:
+            raise ValueError("noisy expected improvement needs at least one measured row")
+        if self.prune and n > 1:
+            (mu,), (L,), z = self.prune_samples(prune_seed)
+            self.winners, self.counts = prune_winners(cfg.obj_scale * (mu[None, :] + z @ L.T) + cfg.obj_shift)
+
     def conditioning(self, pend: np.ndarray | None, batch: np.ndarray | None, z: np.ndarray):
         """C = [kept baseline; pending; batch] rows, L_C^-1, w = (L_C^-T z_C)^T [S, |C|], the incumbents g [S] and the
         batch terms [S, Q] (None without batch points), all float64, and the (rows, beta) pair of C for
         ``cross_covariance``.  z: (S, 1 + |C|)."""
-        d = self.gp.d
-        pend = np.zeros((0, d)) if pend is None else np.asarray(pend, dtype=np.float64).reshape(-1, d)
-        batch = np.zeros((0, d)) if batch is None else np.asarray(batch, dtype=np.float64).reshape(-1, d)
-        rows = np.concatenate([self.baseline[self.kept_baseline(len(pend) + len(batch))], pend, batch])
-        nc, Q = len(rows), len(batch)
-        if z.shape[1] != nc + 1:
-            raise ValueError(f"base samples must be (S, {nc + 1})")
-        mu, L, linv, cond = condition_on(self.gp, rows)
-        zc = z[:, :nc]
-        o = self.cfg.obj_scale * (mu[None, :] + zc @ L.T) + self.cfg.obj_shift
+        rows, linv, w, Y, (cond,) = self.condition(pend, batch, z)
+        nc, Q = len(rows), 0 if batch is None else len(batch)
+        o = self.cfg.obj_scale * Y[:, :, 0] + self.cfg.obj_shift
         g = o[:, : nc - Q].max(axis=1)
         terms = None
         if Q:
             u = o[:, nc - Q:] - g[:, None]
             terms = _log_fatplus(u, self.cfg.tau_relu) if self.cfg.kind == "qLogNEI" else np.maximum(u, 0.0)
-        return rows, linv, zc @ linv, g, terms, cond
+        return rows, linv[0], w[0], g, terms, cond
 
     def values(self, x, pend: np.ndarray | None, z: torch.Tensor, keep=None, index_offset: int = 0,
                want_scores: bool = True, batch: np.ndarray | None = None):
@@ -167,27 +207,6 @@ class NeiScorer:
             c.kind == "qLogNEI", [c.obj_scale, c.obj_shift, c.tau_relu, c.tau_max], int(index_offset),
             bool(want_scores))
         return (scores if want_scores else None), key, (lambda v: v)
-
-    # ---- the interfaces the recommenders use -------------------------------------------------------------------
-    def base_samples(self, n_samples: int, n_pending: int, seed: int) -> torch.Tensor:
-        """Scrambled Sobol normals of dimension 1 + |C|: the conditioning points in the order of C, then the
-        candidate."""
-        return sobol_normal_samples(n_samples, 1 + self.n_conditioning(n_pending), seed)
-
-    def round_best(self, x, pend: np.ndarray, keep, index_offset: int, seed: int, n_samples: int):
-        """One sequential-greedy round: (packed best key, report) -- see ``greedy_select``."""
-        P = len(pend)
-        _, key, report = self.values(x, pend if P else None, self.base_samples(n_samples, P, seed), keep,
-                                     index_offset, want_scores=False)
-        return key, report
-
-    def scores(self, x, pend: np.ndarray | None, seed: int, n_samples: int, batch: np.ndarray | None = None):
-        """Acquisition value of every row given the pending points (and the other points of its q-batch), float64."""
-        n_other = (0 if pend is None else len(pend)) + (0 if batch is None else len(batch))
-        z = sobol_normal_samples(n_samples, 1 + self.n_conditioning(n_other), seed)
-        s, _, _ = self.values(x, pend if pend is not None and len(pend) else None, z,
-                              batch=batch if batch is not None and len(batch) else None)
-        return s.double().cpu().numpy()
 
     def joint_value(self, rows, pend: np.ndarray | None, seed: int, n_samples: int) -> float:
         """Value of the q-batch `rows` given the pending points: the first row is the candidate, the others join

@@ -17,7 +17,8 @@ import numpy as np
 import torch
 
 from baybe_b200 import _lib
-from baybe_b200.engine import AcqConfig, sobol_normal_samples
+from baybe_b200.engine import AcqConfig
+from baybe_b200.scoring import Scorer
 
 __all__ = ["CompiledObjective", "compile_objective", "evaluate_program", "scalarize", "evaluate_objective",
            "uses_objective_scorer", "pending_conditioning", "ObjectiveScorer", "build_objective_scorer"]
@@ -287,9 +288,9 @@ def pending_conditioning(gps, pend: np.ndarray, z: torch.Tensor):
     return stats, linv, w, ys
 
 
-class ObjectiveScorer:
+class ObjectiveScorer(Scorer):
     """MC (and, for MEAN desirability over affine targets, analytic) acquisition values of a compiled objective over
-    one model per target; the interface of ``HviScorer`` (``values``, ``round_best``, ``scores``, ``base_samples``).
+    one model per target.
     `comp` is evaluated on the samples; `analytic` (analytic kinds only) gives the Gaussian moments."""
 
     def __init__(self, gps, cfg: AcqConfig, comp: CompiledObjective, analytic: CompiledObjective | None = None):
@@ -335,24 +336,9 @@ class ObjectiveScorer:
             bool(want_scores))
         return (scores if want_scores else None), key, (lambda v: v)
 
-    def base_samples(self, n_samples: int, n_pending: int, seed: int) -> torch.Tensor | None:
-        """Scrambled Sobol normals of dimension M(1+P) (the layout of ``HviScorer``); None for analytic kinds."""
-        if not self.cfg.is_mc:
-            return None
-        return sobol_normal_samples(n_samples, self.M * (1 + n_pending), seed)
-
-    def round_best(self, x, pend: np.ndarray, keep, index_offset: int, seed: int, n_samples: int):
-        """One sequential-greedy round: (packed best key, report) -- see ``greedy_select``."""
-        P = len(pend)
-        _, key, report = self.values(x, pend if P else None, self.base_samples(n_samples, P, seed), keep,
-                                     index_offset, want_scores=False)
-        return key, report
-
-    def scores(self, x, pend: np.ndarray | None, seed: int, n_samples: int) -> np.ndarray:
-        """Acquisition value of [x_i; pending] for every row (float64 host array)."""
-        P = 0 if pend is None else len(pend)
-        s, _, _ = self.values(x, pend if P else None, self.base_samples(n_samples, P, seed))
-        return s.double().cpu().numpy()
+    def n_sample_columns(self, n_other: int) -> int | None:
+        """M(1+P) (the layout of ``HviScorer``); None for analytic kinds."""
+        return self.M * (1 + n_other) if self.cfg.is_mc else None
 
 
 def _incompatibility(msg: str) -> Exception:

@@ -21,8 +21,8 @@ import numpy as np
 import torch
 
 from baybe_b200 import _lib, noisy
-from baybe_b200.engine import AcqConfig, sobol_normal_samples
-from baybe_b200.noisy import PRUNE_SAMPLES, PRUNE_SEED, _log_fatplus, capped_baseline, condition_on, prune_winners
+from baybe_b200.engine import AcqConfig
+from baybe_b200.noisy import PRUNE_SEED, BaselineScorer, _log_fatplus, prune_winners
 
 __all__ = ["CHEBYSHEV_ALPHA", "sample_simplex", "chebyshev", "ParegoScorer", "build_parego_scorer"]
 
@@ -49,31 +49,28 @@ def chebyshev(p: np.ndarray, alpha: float = CHEBYSHEV_ALPHA) -> np.ndarray:
     return p.min(axis=-1) + alpha * p.sum(axis=-1)
 
 
-class ParegoScorer:
-    """qLogNParEGO over one model per target; the interface of ``NeiScorer`` (``values``, ``round_best``, ``scores``,
-    ``base_samples``, ``joint_value``, ``n_dropped``).  `scales`/`shifts` orient target m as o_m = a_m y_m + b_m;
-    `baseline`: the measured rows (raw comp-rep); `weights`: the simplex weights lambda.  The normalisation bounds
-    lo_m, hi_m are the extremes of the oriented float64 posterior mean over every measured row; a range that is not
-    positive counts as 1 (botorch would divide by zero).  With `prune`, the baseline is pruned once on the
-    scalarised objective, from ``PRUNE_SAMPLES`` joint posterior samples drawn with `prune_seed`."""
+class ParegoScorer(BaselineScorer):
+    """qLogNParEGO over one model per target.  `scales`/`shifts` orient target m as o_m = a_m y_m + b_m; `baseline`:
+    the measured rows (raw comp-rep); `weights`: the simplex weights lambda.  The normalisation bounds lo_m, hi_m are
+    the extremes of the oriented float64 posterior mean over every measured row; a range that is not positive counts
+    as 1 (botorch would divide by zero).  With `prune`, the baseline is pruned once on the scalarised objective, from
+    ``PRUNE_SAMPLES`` joint posterior samples drawn with `prune_seed`."""
 
     def __init__(self, gps, cfg: AcqConfig, scales, shifts, baseline, weights, prune: bool = True,
                  prune_seed: int = PRUNE_SEED):
         if cfg.kind not in _lib.PAREGO_KINDS:
             raise ValueError(f"{cfg.kind} is not a ParEGO acquisition function")
-        self.gps, self.cfg, self.prune = list(gps), cfg, bool(prune)
-        self.M = len(self.gps)
-        if not 2 <= self.M <= _lib.PAREGO_MAX_TARGETS:
+        M = len(gps)
+        if not 2 <= M <= _lib.PAREGO_MAX_TARGETS:
             from baybe_b200.multiobjective import _error
 
             raise _error("IncompatibleAcquisitionFunctionError")(
-                f"{cfg.kind} on the B200 engine supports 2 to {_lib.PAREGO_MAX_TARGETS} targets (got {self.M})")
-        self.device = self.gps[0].device
+                f"{cfg.kind} on the B200 engine supports 2 to {_lib.PAREGO_MAX_TARGETS} targets (got {M})")
+        super().__init__(gps, cfg, baseline, prune)
         self.a = np.asarray(scales, dtype=np.float64).reshape(self.M)
         self.b = np.asarray(shifts, dtype=np.float64).reshape(self.M)
         self.weights = np.asarray(weights, dtype=np.float64).reshape(self.M)
         self.alpha = CHEBYSHEV_ALPHA
-        self.baseline = np.asarray(baseline, dtype=np.float64).reshape(-1, self.gps[0].d)
         n = len(self.baseline)
         if n == 0:
             raise ValueError("qLogNParEGO needs at least one measured row")
@@ -83,45 +80,18 @@ class ParegoScorer:
         rng = np.where(hi - lo > 0.0, hi - lo, 1.0)
         self.W = self.weights * self.a / rng  # p_m = W_m y_m + V_m
         self.V = self.weights * (self.b - lo) / rng
-        self.winners, self.counts = np.arange(n), np.ones(n, dtype=np.int64)
         if self.prune and n > 1:
-            from baybe_b200.multiobjective import _psd_cholesky
-
-            z = sobol_normal_samples(PRUNE_SAMPLES, self.M * n, prune_seed).numpy()
-            Y = np.stack([mu[None, :] + z[:, m * n:(m + 1) * n] @ _psd_cholesky(0.5 * (cov + cov.T)).T
-                          for m, (mu, cov) in enumerate(post)], axis=-1)  # [samples, n, M]
+            mus, Ls, z = self.prune_samples(prune_seed, post)
+            Y = np.stack([mus[m][None, :] + z[:, m * n:(m + 1) * n] @ Ls[m].T for m in range(self.M)],
+                         axis=-1)  # [samples, n, M]
             self.winners, self.counts = prune_winners(chebyshev(self.W * Y + self.V, self.alpha))
-        self.n_dropped = 0
-
-    # ---- candidate-independent set-up of one evaluation ----------------------------------------------------
-    def kept_baseline(self, n_other: int) -> np.ndarray:
-        """Indices of the baseline rows that condition an evaluation with `n_other` pending and batch points."""
-        kept, self.n_dropped = capped_baseline(self.cfg.kind, self.winners, self.counts, len(self.baseline),
-                                               self.prune, n_other)
-        return kept
-
-    def n_conditioning(self, n_other: int) -> int:
-        return len(self.kept_baseline(n_other)) + n_other
 
     def conditioning(self, pend: np.ndarray | None, batch: np.ndarray | None, z: np.ndarray):
         """C = [kept baseline; pending; batch] rows; per target L_C^-1 [M, |C|, |C|], w = (L_C^-T z_C)^T [M, S, |C|]
         and the (rows, beta) pair of C for ``cross_covariance``; the incumbents g [S] and the batch terms [S, Q]
         (None without batch points), all float64.  z: (S, M(1 + |C|)), column m(1 + |C|) + j = point j of target m."""
-        d = self.gps[0].d
-        pend = np.zeros((0, d)) if pend is None else np.asarray(pend, dtype=np.float64).reshape(-1, d)
-        batch = np.zeros((0, d)) if batch is None else np.asarray(batch, dtype=np.float64).reshape(-1, d)
-        rows = np.concatenate([self.baseline[self.kept_baseline(len(pend) + len(batch))], pend, batch])
-        nc, Q, M = len(rows), len(batch), self.M
-        if z.shape[1] != M * (nc + 1):
-            raise ValueError(f"base samples must be (S, {M * (nc + 1)})")
-        S = z.shape[0]
-        linv, w, Y, conds = np.zeros((M, nc, nc)), np.zeros((M, S, nc)), np.zeros((S, nc, M)), []
-        for m, gp in enumerate(self.gps):
-            mu, L, linv[m], cond = condition_on(gp, rows)
-            zc = z[:, m * (nc + 1): m * (nc + 1) + nc]
-            Y[:, :, m] = mu[None, :] + zc @ L.T
-            w[m] = zc @ linv[m]
-            conds.append(cond)
+        rows, linv, w, Y, conds = self.condition(pend, batch, z)
+        nc, Q = len(rows), 0 if batch is None else len(batch)
         cheb = chebyshev(self.W * Y + self.V, self.alpha)  # [S, |C|]
         g = cheb[:, : nc - Q].max(axis=1)
         terms = _log_fatplus(cheb[:, nc - Q:] - g[:, None], self.cfg.tau_relu) if Q else None
@@ -144,27 +114,6 @@ class ParegoScorer:
             None if terms is None else t(terms), keep, [float(v) for v in self.W], [float(v) for v in self.V],
             [self.alpha, c.tau_relu, c.tau_max], int(index_offset), bool(want_scores))
         return (scores if want_scores else None), key, (lambda v: v)
-
-    # ---- the interfaces the recommenders use -------------------------------------------------------------------
-    def base_samples(self, n_samples: int, n_pending: int, seed: int) -> torch.Tensor:
-        """Scrambled Sobol normals of dimension M(1 + |C|): per target block the conditioning points in the order of
-        C, then the candidate."""
-        return sobol_normal_samples(n_samples, self.M * (1 + self.n_conditioning(n_pending)), seed)
-
-    def round_best(self, x, pend: np.ndarray, keep, index_offset: int, seed: int, n_samples: int):
-        """One sequential-greedy round: (packed best key, report) -- see ``greedy_select``."""
-        P = len(pend)
-        _, key, report = self.values(x, pend if P else None, self.base_samples(n_samples, P, seed), keep,
-                                     index_offset, want_scores=False)
-        return key, report
-
-    def scores(self, x, pend: np.ndarray | None, seed: int, n_samples: int, batch: np.ndarray | None = None):
-        """Acquisition value of every row given the pending points (and the other points of its q-batch), float64."""
-        n_other = (0 if pend is None else len(pend)) + (0 if batch is None else len(batch))
-        z = self.base_samples(n_samples, n_other, seed)
-        s, _, _ = self.values(x, pend if pend is not None and len(pend) else None, z,
-                              batch=batch if batch is not None and len(batch) else None)
-        return s.double().cpu().numpy()
 
     def joint_value(self, rows, pend: np.ndarray | None, seed: int, n_samples: int) -> float:
         """Value of the q-batch `rows` given the pending points: the first row is the candidate, the others join

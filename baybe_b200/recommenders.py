@@ -30,7 +30,6 @@ from attrs.converters import optional
 
 from baybe_b200.acquisition import (AcquisitionFunction, IncompatibleAcquisitionFunctionError,
                                     convert_acqf, qLogExpectedImprovement)
-from baybe_b200._lib import NEI_KINDS
 from baybe_b200.bits import pack_bits
 from baybe_b200.engine import DEFAULT_MC_SAMPLES, AcqConfig, DeviceGP, sobol_normal_samples, unpack_best
 from baybe_b200.surrogates import GaussianProcessSurrogate
@@ -167,19 +166,19 @@ def greedy_select(gp: DeviceGP, cfg: AcqConfig, x_shard: torch.Tensor, d: int, q
                   offset: int = 0, keep_init: torch.Tensor | None = None) -> tuple[list[int], list[float]]:
     """Sequential greedy selection of q rows (global positions) -- ``optimize_acqf_discrete`` with
     ``unique=True``.  `x_shard` holds this rank's rows [offset, offset+len) on the device; the features of each
-    round's winner are fetched from the rank that owns it (``_winner_row``).  A `gp` with a ``round_best`` method
-    (``baybe_b200.multiobjective.HviScorer``, ``baybe_b200.objectives.ObjectiveScorer``, ``baybe_b200.noisy.NeiScorer``)
-    scores a round itself and maps the winner's key value to the reported acquisition value."""
+    round's winner are fetched from the rank that owns it (``_winner_row``).  A ``baybe_b200.scoring.Scorer`` scores
+    a round itself and maps the winner's key value to the reported acquisition value."""
+    from baybe_b200.scoring import Scorer
+
     chosen: list[int] = []
     values: list[float] = []
     keep = (torch.ones(x_shard.shape[0], dtype=torch.uint8, device=x_shard.device)
             if keep_init is None else keep_init.to(device=x_shard.device, dtype=torch.uint8).clone())
     pend = np.zeros((0, d)) if base_pending is None else np.asarray(base_pending, dtype=np.float64).reshape(-1, d)
-    round_best = getattr(gp, "round_best", None)
     for r in range(q):
         report = None
-        if round_best is not None:
-            key, report = round_best(x_shard, pend, keep, offset, seed, n_samples)
+        if isinstance(gp, Scorer):
+            key, report = gp.round_best(x_shard, pend, keep, offset, seed, n_samples)
         elif len(pend) == 0:
             z = sobol_normal_samples(n_samples, 1, seed)[:, 0] if cfg.is_mc else None
             _, key = gp.score(cfg, x_shard, z, keep=keep, index_offset=offset, want_scores=False)
@@ -192,7 +191,7 @@ def greedy_select(gp: DeviceGP, cfg: AcqConfig, x_shard: torch.Tensor, d: int, q
         if idx < 0:
             raise NotEnoughPointsLeftError("no eligible candidate left to recommend")
         chosen.append(idx)
-        values.append(val if report is None else report(val))
+        values.append(val if report is None else float(report(val)))
         if offset <= idx < offset + x_shard.shape[0]:
             keep[idx - offset] = 0
         if r + 1 < q:
@@ -306,13 +305,10 @@ class B200Recommender:
             raise IncompatibleAcquisitionFunctionError(
                 f"The '{type(self).__name__}' only works with Monte Carlo acquisition functions "
                 f"for batch sizes > 1.")
-        from baybe_b200.objectives import uses_objective_scorer
-
         self._objective = objective
         surrogate = self.get_surrogate(searchspace, objective, measurements)
         self._scorer = None
-        # a single target with a non-affine transformation, or the noisy-EI family
-        if uses_objective_scorer(objective) or acqf.abbreviation in NEI_KINDS:
+        if acqf.uses_scorer(objective, searchspace):
             if pending_experiments is not None and not acqf.supports_pending_experiments:
                 raise IncompatibleAcquisitionFunctionError(
                     f"The chosen acquisition function of type '{type(acqf).__name__}' "

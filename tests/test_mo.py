@@ -387,6 +387,28 @@ def test_pareto_campaign_rejections(bb):
         single.acquisition_values(space.discrete.exp_rep.head(5), acquisition_function=qLogEHVI())
 
 
+def test_acquisition_callable_rejects_more_than_31_other_points_before_scoring(bb, monkeypatch):
+    """The joint value of a q-batch with its pending points: up to 31 points besides the candidate are scored, more
+    raise NotImplementedError before the scoring op is called."""
+    from baybe_b200 import surrogates
+    from baybe_b200.engine import AcqConfig
+
+    rng = np.random.default_rng(7)
+    X = rng.random((10, 3))
+    gps = [surrogates.DeviceGP(X, np.sin(3 * X @ rng.normal(size=3)), np.stack([np.zeros(3), np.ones(3)]),
+                               "matern52", 0.5, 1e-3) for _ in range(2)]
+    front = np.stack([gp.posterior(X)[0].double().numpy() for gp in gps], 1)
+    scorer = mo.HviScorer(gps, AcqConfig(kind="qEHVI"), [1.0, 1.0], [0.0, 0.0], mo.compute_ref_point(front), front)
+    calls = []
+    monkeypatch.setattr(mo, "_hvi_score", lambda *a: calls.append(1) or _hvi_score_f64(*a))
+    pend = torch.from_numpy(rng.random((29, 3)))
+    acqf = bb.EngineAcquisitionFunction(None, scorer.cfg, 8, X_pending=pend, scorer=scorer)
+    with pytest.raises(NotImplementedError, match="at most 32 points"):
+        acqf(torch.from_numpy(rng.random((1, 4, 3))))  # 3 batch + 29 pending points besides the candidate
+    assert not calls
+    assert np.isfinite(float(acqf(torch.from_numpy(rng.random((1, 3, 3))))[0])) and len(calls) == 1
+
+
 def test_grid_work_is_bounded_before_the_grid_is_built():
     F = np.random.default_rng(0).normal(size=(400, 4))
     F = F / np.linalg.norm(F, axis=1, keepdims=True)  # points on a sphere: most are non-dominated
