@@ -33,6 +33,10 @@ PAREGO_MAX_TARGETS = 8  # BB_OBJ_MAX_TARGETS
 # never by the fused kernels: Pareto objectives with a sampled front, baybe_b200/nehvi.py (bb_hvi_decompose, then
 # bb_hvi_score with the qEHVI kind)
 NEHVI_KINDS = ("qNEHVI",)
+# never by the fused kernels: integrated posterior variance over fixed integration points, baybe_b200/nipv.py
+# (bb_nipv_score); no base samples, but batches and joint values go through the conditioning set like the MC kinds
+NIPV_KINDS = ("qNIPV",)
+NIPV_MAX_TRAIN = 256
 MAX_PENDING = 31
 MAX_TRAIN = 1024
 
@@ -153,6 +157,8 @@ _SIGNATURES = {
                                   _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _i64,
                                   _vp]),
     "bb_hvi_decompose": (C.c_int, [_i32, C.POINTER(C.c_double), _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "bb_nipv_score": (C.c_int, [C.POINTER(Model), C.POINTER(C.c_float), C.c_float, _vp, _i64, _vp, _i64, _vp, _i32,
+                                _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),

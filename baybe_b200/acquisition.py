@@ -22,7 +22,7 @@ __all__ = [
     "PM", "PSTD", "qSR", "EI", "qEI", "LogEI", "qLogEI", "PI", "qPI", "UCB", "qUCB",
     "qNoisyExpectedImprovement", "qNEI", "qLogNoisyExpectedImprovement", "qLogNEI",
     "qExpectedHypervolumeImprovement", "qEHVI", "qLogExpectedHypervolumeImprovement", "qLogEHVI", "qLogNParEGO",
-    "qNoisyExpectedHypervolumeImprovement", "qNEHVI",
+    "qNoisyExpectedHypervolumeImprovement", "qNEHVI", "qNegIntegratedPosteriorVariance", "qNIPV",
 ]
 
 
@@ -418,6 +418,95 @@ class qNoisyExpectedHypervolumeImprovement(_ScoredAcquisitionFunction):
         return build_nehvi_scorer(self, gps, searchspace, objective, measurements)
 
 
+def _incompatibility(msg: str) -> Exception:
+    try:
+        from baybe.exceptions import IncompatibilityError
+    except ImportError:  # pragma: no cover - baybe absent
+        return NotImplementedError(msg)
+    return IncompatibilityError(msg)
+
+
+def _positive_int_or_none(_, attr, value) -> None:
+    if value is not None and (not isinstance(value, int) or isinstance(value, bool) or value <= 0):
+        raise ValueError(f"'{attr.name}' must be a positive int or None (got {value!r})")
+
+
+@define(frozen=True)
+class qNegIntegratedPosteriorVariance(AcquisitionFunction):
+    """acquisition/acqfs.py:28-138: global active learning on discrete search spaces (``baybe_b200.nipv``): the
+    negative posterior variance averaged over integration points drawn from the whole discrete space, conditional on
+    noisy observations of the candidate, the pending points and the other points of a q-batch (``bb_nipv_score``).
+    Single targets without a transformation only; ``sampling_method``: "Random" (the plugin also takes BayBE's FPS
+    points through the BayBE spec's ``get_integration_points``)."""
+
+    abbreviation: ClassVar[str] = "qNIPV"
+    sampling_n_points: int | None = field(default=None, validator=_positive_int_or_none)
+    sampling_fraction: float | None = field(converter=lambda v: None if v is None else float(v))
+    sampling_method: str = field(default="Random", converter=lambda v: str(getattr(v, "value", v)))
+
+    @sampling_fraction.default
+    def _default_sampling_fraction(self) -> float | None:
+        return 1.0 if self.sampling_n_points is None else None
+
+    @sampling_fraction.validator
+    def _validate_sampling_fraction(self, attr, value) -> None:
+        if value is not None and not 0.0 < value <= 1.0:
+            raise ValueError(f"'{attr.name}' must be in (0, 1] (got {value})")
+        if None not in (self.sampling_fraction, self.sampling_n_points):
+            raise ValueError(
+                f"For '{self.__class__.__name__}', the attributes '{attr.name}' and 'sampling_n_points' cannot "
+                f"be specified at the same time.")
+
+    def get_integration_points(self, searchspace) -> pd.DataFrame:
+        """The integration rows of the discrete part (reference ``get_integration_points``, Random only)."""
+        from baybe_b200.nipv import sample_integration_points
+
+        return sample_integration_points(searchspace.discrete.comp_rep, self.sampling_n_points,
+                                         self.sampling_fraction, self.sampling_method)
+
+    def uses_scorer(self, objective, searchspace) -> bool:
+        return True
+
+    def evaluate(self, candidates: pd.DataFrame, surrogate, searchspace, objective, measurements,
+                 pending_experiments: pd.DataFrame | None = None, *, jointly: bool = False, integration=None):
+        """``AcquisitionFunction.evaluate`` with the integration points `integration` (comp-rep rows; None:
+        ``get_integration_points``)."""
+        if pending_experiments is not None and not self.supports_pending_experiments:  # pragma: no cover - q kind
+            raise IncompatibleAcquisitionFunctionError("qNIPV does not support pending experiments")
+        scorer = self.scorer(surrogate, searchspace, objective, measurements, integration=integration)
+        return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
+
+    def to_engine(self, surrogate, searchspace, objective, measurements, pending_experiments=None) -> AcqConfig:
+        raise IncompatibleAcquisitionFunctionError(
+            "'qNegIntegratedPosteriorVariance' is evaluated by baybe_b200.nipv.NipvScorer (see scorer())")
+
+    def scorer(self, surrogate, searchspace, objective, measurements, integration=None):
+        """Check the objective and the space, fit the surrogate and send the integration points (`integration`, or
+        ``get_integration_points``) to the device."""
+        from baybe_b200.multiobjective import _error
+        from baybe_b200.nipv import NipvScorer
+
+        if getattr(objective, "is_multi_output", False):
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' needs a single-target objective")
+        if type(objective).__name__ == "DesirabilityObjective":
+            raise _incompatibility(f"'{type(self).__name__}' currently supports single-target objectives only.")
+        kind = _space_kind(searchspace)
+        if kind != "DISCRETE":
+            raise _error("IncompatibleAcquisitionFunctionError")(
+                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
+        targets = getattr(objective, "targets", None) or [getattr(objective, "_target", None)]
+        tr = getattr(targets[0], "transformation", None)
+        if tr is not None and type(tr).__name__ != "IdentityTransformation":
+            raise _incompatibility(
+                "'qNegIntegratedPosteriorVariance' currently does not support any target transformations.")
+        surrogate.fit(searchspace, objective, measurements)
+        if integration is None:
+            integration = self.get_integration_points(searchspace)
+        return NipvScorer(surrogate.device_gp, AcqConfig(kind="qNIPV"), integration.to_numpy(dtype="float64"))
+
+
+qNIPV = qNegIntegratedPosteriorVariance
 qNEI, qLogNEI = qNoisyExpectedImprovement, qLogNoisyExpectedImprovement
 qNEHVI = qNoisyExpectedHypervolumeImprovement
 qEHVI, qLogEHVI = qExpectedHypervolumeImprovement, qLogExpectedHypervolumeImprovement
@@ -426,7 +515,7 @@ EI, qEI, LogEI, qLogEI = ExpectedImprovement, qExpectedImprovement, LogExpectedI
 PI, qPI, UCB, qUCB = ProbabilityOfImprovement, qProbabilityOfImprovement, UpperConfidenceBound, qUpperConfidenceBound
 
 _BY_NAME = {c.__name__: c for c in (PM, PSTD, qSR, EI, qEI, LogEI, qLogEI, PI, qPI, UCB, qUCB, qNEI, qLogNEI,
-                                    qEHVI, qLogEHVI, qLogNParEGO, qNEHVI)}
+                                    qEHVI, qLogEHVI, qLogNParEGO, qNEHVI, qNIPV)}
 _BY_NAME.update({c.abbreviation: c for c in list(_BY_NAME.values())})
 
 

@@ -63,6 +63,14 @@ def mirror_acquisition_function(acqf) -> _acq.AcquisitionFunction:
     return cls(**kwargs)
 
 
+def _integration_points(acqf, spec, searchspace) -> dict:
+    """qNIPV given as BayBE's spec: its own draw of the integration points, so that Random and FPS pick exactly the
+    rows BayBE picks (keyword arguments for the engine spec's ``scorer`` / ``evaluate``; empty otherwise)."""
+    if spec.abbreviation in _lib.NIPV_KINDS and hasattr(acqf, "get_integration_points"):
+        return {"integration": acqf.get_integration_points(searchspace)}
+    return {}
+
+
 class EngineAcquisitionFunction:
     """The acquisition callable BayBE hands around (``recommender._botorch_acqf``): ``acqf(X)`` with ``X`` of shape
     ``[b, q, d]`` (un-scaled comp-rep) returns ``[b]`` joint values of ``[X_b ; X_pending]``."""
@@ -172,7 +180,8 @@ class B200BotorchRecommender(BayesianRecommender):
                 raise IncompatibleAcquisitionFunctionError(
                     f"The chosen acquisition function of type '{type(spec).__name__}' "
                     f"does not support pending experiments.")
-            self._scorer = spec.scorer(surrogate, searchspace, objective, measurements)
+            self._scorer = spec.scorer(surrogate, searchspace, objective, measurements,
+                                       **_integration_points(acqf, spec, searchspace))
             cfg = self._scorer.cfg
         else:
             cfg = spec.to_engine(surrogate, searchspace, objective, measurements, pending_experiments)
@@ -258,13 +267,15 @@ class B200BotorchRecommender(BayesianRecommender):
     def acquisition_values(self, candidates, searchspace, objective, measurements, pending_experiments=None,
                            acquisition_function=None) -> pd.Series:
         surrogate = self.get_surrogate(searchspace, objective, measurements)
-        acqf = mirror_acquisition_function(acquisition_function or self._get_acquisition_function(objective))
+        given = acquisition_function or self._get_acquisition_function(objective)
+        acqf = mirror_acquisition_function(given)
         return acqf.evaluate(candidates, surrogate, searchspace, objective, measurements, pending_experiments,
-                             jointly=False)
+                             jointly=False, **_integration_points(given, acqf, searchspace))
 
     def joint_acquisition_value(self, candidates, searchspace, objective, measurements, pending_experiments=None,
                                 acquisition_function=None) -> float:
         surrogate = self.get_surrogate(searchspace, objective, measurements)
-        acqf = mirror_acquisition_function(acquisition_function or self._get_acquisition_function(objective))
+        given = acquisition_function or self._get_acquisition_function(objective)
+        acqf = mirror_acquisition_function(given)
         return acqf.evaluate(candidates, surrogate, searchspace, objective, measurements, pending_experiments,
-                             jointly=True)
+                             jointly=True, **_integration_points(given, acqf, searchspace))

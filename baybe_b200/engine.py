@@ -77,12 +77,13 @@ class AcqConfig:
     tau_pi: float = 1e-3
 
     def __post_init__(self):
-        if self.kind not in tuple(_lib.ACQ_KIND) + _lib.NEI_KINDS + _lib.PAREGO_KINDS + _lib.NEHVI_KINDS:
+        if self.kind not in (tuple(_lib.ACQ_KIND) + _lib.NEI_KINDS + _lib.PAREGO_KINDS + _lib.NEHVI_KINDS
+                             + _lib.NIPV_KINDS):
             raise ValueError(f"unsupported acquisition function {self.kind!r}")
 
     @property
     def is_mc(self) -> bool:
-        return self.kind in _lib.MC_KINDS + _lib.NEI_KINDS + _lib.PAREGO_KINDS + _lib.NEHVI_KINDS
+        return self.kind in _lib.MC_KINDS + _lib.NEI_KINDS + _lib.PAREGO_KINDS + _lib.NEHVI_KINDS + _lib.NIPV_KINDS
 
     def to_c(self) -> _lib.AcqSpec:
         if self.kind in _lib.NEI_KINDS:
@@ -93,6 +94,9 @@ class AcqConfig:
                                       "kernels")
         if self.kind in _lib.NEHVI_KINDS:
             raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.nehvi.NehviScorer, not by the fused "
+                                      "kernels")
+        if self.kind in _lib.NIPV_KINDS:
+            raise NotImplementedError(f"{self.kind} is evaluated by baybe_b200.nipv.NipvScorer, not by the fused "
                                       "kernels")
         return _lib.AcqSpec(
             _lib.ACQ_KIND[self.kind], int(self.maximize), self.best_f, self.beta, self.obj_scale,
@@ -194,6 +198,9 @@ class DeviceGP:
         self.n, self.d, self.n_tasks = n, d, T
         self.family, self.task_col = family, task_col
         self.outputscale = None if outputscale is None else float(outputscale)
+        # the fitted hyper-parameters as given: lengthscale (d,), likelihood noise per task (T,), task covariance
+        # (T, T) or None
+        self.lengthscale, self.noise, self.task_covar = ls, nz, tcv
         self._keepalive = (tx, ty, bnd, ls, nz, mc, tcv)
         dp = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))  # noqa: E731
         lo_arr, hi_arr = np.ascontiguousarray(bnd[0]), np.ascontiguousarray(bnd[1])
@@ -756,6 +763,55 @@ def _op_nei_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | Non
 @_op_nei_score.register_fake
 def _(mu, var, cross, linv, w, z, g, batch_terms, keep, log_nei, params, index_offset, want_scores):
     return (mu.new_empty(mu.shape[0] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
+
+
+_NIPV_WS_CAP = 768 << 20  # workspace of bb_nipv_score: rows are processed in blocks that fit it
+
+
+def nipv_model_terms(gp: DeviceGP) -> tuple[list[float], float]:
+    """The likelihood noise per task (standardised, floored at 1e-4) and the largest prior variance over the tasks
+    (standardised) of a model: what ``bb_nipv_score`` takes besides the model."""
+    scale = 1.0 if gp.outputscale is None else gp.outputscale
+    diag = np.ones(1) if gp.task_covar is None else np.diag(gp.task_covar)
+    return [max(float(v), 1e-4) for v in gp.noise], float(scale * diag.max())
+
+
+@torch.library.custom_op("baybe_b200::nipv_score", mutates_args=())
+def _op_nipv_score(x: torch.Tensor, xm: torch.Tensor, var: torch.Tensor, cross_x: torch.Tensor | None,
+                   cross_m: torch.Tensor | None, linv: torch.Tensor | None, keep: torch.Tensor | None, handle: int,
+                   index_offset: int, want_scores: bool) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_nipv_score``: candidates x [N, d] and integration points xm [M, d] (raw fp32 rows), the candidates'
+    posterior variance var [N]; with |C| conditioning points cross_x [N, |C|], cross_m [M, |C|] and linv [|C|, |C|]
+    (L_C^-1 of K_D(C,C) + noise, original units).  Scores: IVR(x) in original units."""
+    gp = _gp(handle)
+    N, M = x.shape[0], xm.shape[0]
+    for name, t, rows in (("x", x, N), ("xm", xm, M)):
+        if t.dim() != 2 or t.shape[1] != gp.d or t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous float32 ({rows}, {gp.d}) tensor")
+    Cn = 0 if cross_x is None else cross_x.shape[1]
+    if Cn and (cross_m is None or tuple(cross_m.shape) != (M, Cn) or linv is None or tuple(linv.shape) != (Cn, Cn)):
+        raise ValueError(f"conditioning needs cross_m ({M}, {Cn}) and linv ({Cn}, {Cn})")
+    _check_keep(keep, N)
+    f32 = lambda t: None if t is None else t.to(torch.float32).contiguous()  # noqa: E731
+    var, cross_x, cross_m, linv = f32(var), f32(cross_x), f32(cross_m), f32(linv)
+    noise, prior_var = nipv_model_terms(gp)
+    r_pad = -(-(gp.n + Cn) // 64) * 64
+    row_bytes = 4 * r_pad + 4 * gp.d + 12
+    ws_bytes = min(_NIPV_WS_CAP, (N + M + 256) * row_bytes)
+    lib = _lib.load()
+    with torch.cuda.device(x.device):
+        score, key = _score_and_key(N, want_scores, x.device)
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=x.device)
+        _lib.check(lib.bb_nipv_score(C.byref(gp.model), (C.c_float * len(noise))(*noise), prior_var, _ptr(x), N,
+                                     _ptr(xm), M, _ptr(var), Cn, _ptr(cross_x), _ptr(cross_m), _ptr(linv),
+                                     _ptr(keep), _ptr(score) if want_scores else None, _ptr(key), int(index_offset),
+                                     _ptr(ws), ws_bytes, _stream_ptr()), "bb_nipv_score")
+    return score, key
+
+
+@_op_nipv_score.register_fake
+def _(x, xm, var, cross_x, cross_m, linv, keep, handle, index_offset, want_scores):
+    return (x.new_empty(x.shape[0] if want_scores else 0, dtype=torch.float32), x.new_empty(1, dtype=torch.int64))
 
 
 @torch.library.custom_op("baybe_b200::parego_score", mutates_args=())

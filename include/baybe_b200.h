@@ -504,6 +504,30 @@ int bb_parego_score(int32_t n_targets, const float* weight, const float* offset,
                     const float* d_g, int32_t n_batch, const float* d_batch_terms, const uint8_t* d_keep,
                     float* d_score, int64_t* d_best_key, int64_t index_offset, void* stream);
 
+/* ---- integrated posterior variance reduction for global active learning (qNegIntegratedPosteriorVariance,
+ * baybe/acquisition/acqfs.py:28-138; set-up on the host by baybe_b200/nipv.py).  With C the n_cond conditioning
+ * points (pending points and the other points of a q-batch, observed with noise) and k_D the posterior covariance
+ * given the training data, k_C(a,b) = k_D(a,b) - k_D(a,C) (K_D(C,C) + diag sigma_n^2(C))^-1 k_D(C,b).  Writes, for
+ * every candidate x, IVR(x) = sum_m k_C(m,x)^2 / (k_C(x,x) + sigma_n^2(x)) in original units over the M integration
+ * points m (qNIPV(x | C) = -(1/M) [sum_m k_C(m,m) - IVR(x)]; the caller adds the candidate-independent sum).
+ *   m: a non-wide model with n <= 256 training points (else BB_ERR_UNSUPPORTED); noise [n_tasks]: HOST array, the
+ *     likelihood noise per task in standardised units (floored at 1e-4 as in bb_model_desc); prior_var: the largest
+ *     prior variance k(a,a) over the tasks, standardised (sets the power-of-two scale of the fp16 operands).
+ *   d_x [N][d], d_xm [M][d]: raw comp-rep rows, fp32 row-major (M >= 1).
+ *   d_var [N]: bb_posterior's variance of the candidates (original units).
+ *   n_cond in [0, BB_MAX_PENDING].  With n_cond > 0: d_cross_x [N][n_cond] and d_cross_m [M][n_cond], bb_posterior's
+ *     cross covariances with C as its pending points (original units), and d_linv [n_cond][n_cond] = L_C^-1
+ *     (row-major, lower triangular), L_C L_C^T = K_D(C,C) + diag sigma_n^2(C) in original units.
+ *   d_ws: caller-owned workspace of ws_bytes >= 256 * (4 r_pad + 4 d + 12) bytes, r_pad = n + n_cond rounded up to
+ *     64; candidates and integration points are processed in blocks of rows that fit it (all of them with
+ *     (N + M + 256) * (4 r_pad + 4 d + 12) bytes), so device memory is bounded for any N and M.
+ * Writes IVR to d_score (nullable) and folds d_keep (nullable) and index_offset into *d_best_key like bb_argmax
+ * (initialise with bb_best_init).  Deterministic: the same inputs give bit-identical outputs. */
+int bb_nipv_score(const bb_model* m, const float* noise, float prior_var, const float* d_x, int64_t N,
+                  const float* d_xm, int64_t M, const float* d_var, int32_t n_cond, const float* d_cross_x,
+                  const float* d_cross_m, const float* d_linv, const uint8_t* d_keep, float* d_score,
+                  int64_t* d_best_key, int64_t index_offset, void* d_ws, size_t ws_bytes, void* stream);
+
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
 int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
