@@ -37,6 +37,9 @@ NEHVI_KINDS = ("qNEHVI",)
 # (bb_nipv_score); no base samples, but batches and joint values go through the conditioning set like the MC kinds
 NIPV_KINDS = ("qNIPV",)
 NIPV_MAX_TRAIN = 256
+# single-target kinds with a gradient path (bb_acq_grad): continuous and hybrid spaces, baybe_b200/continuous.py
+GRAD_KINDS = ("qLogEI", "qEI", "qUCB", "qSR", "qPI", "UCB", "EI", "LogEI", "PI", "PM", "PSTD")
+GRAD_MAX_NPAD = 256
 MAX_PENDING = 31
 MAX_TRAIN = 1024
 
@@ -159,6 +162,8 @@ _SIGNATURES = {
     "bb_hvi_decompose": (C.c_int, [_i32, C.POINTER(C.c_double), _i32, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "bb_nipv_score": (C.c_int, [C.POINTER(Model), C.POINTER(C.c_float), C.c_float, _vp, _i64, _vp, _i64, _vp, _i32,
                                 _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
+    "bb_acq_grad": (C.c_int, [C.POINTER(Model), C.POINTER(AcqSpec), _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32,
+                              _vp, _vp, _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),

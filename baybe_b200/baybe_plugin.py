@@ -24,18 +24,21 @@ and mapped onto the engine's kinds by their ``abbreviation``.
 """
 from __future__ import annotations
 
+import math
 from typing import ClassVar
 
 import numpy as np
 import pandas as pd
 import torch
 from attrs import define, field, fields_dict
-from attrs.validators import ge, instance_of
+from attrs.converters import optional as optional_c
+from attrs.validators import ge, gt, instance_of
 
 from baybe.exceptions import (IncompatibilityError, IncompatibleAcquisitionFunctionError,  # noqa: E402
                               InfeasibilityError)
 from baybe.recommenders.pure.bayesian.base import BayesianRecommender
 from baybe.searchspace import SearchSpaceType
+from baybe.utils.sampling_algorithms import DiscreteSamplingMethod, sample_numerical_df
 
 from baybe_b200 import _lib
 from baybe_b200 import acquisition as _acq
@@ -122,7 +125,9 @@ class EngineAcquisitionFunction:
 
 @define(kw_only=True)
 class B200BotorchRecommender(BayesianRecommender):
-    """``BotorchRecommender`` for discrete search spaces with the scoring path on the B200 engine."""
+    """``BotorchRecommender`` with the scoring path on the B200 engine: discrete spaces, and continuous and hybrid
+    spaces with the single-target acquisition functions (gradient path, ``baybe_b200.continuous``) or qNEI (hybrid
+    spaces, search by scoring, ``baybe_b200.hybrid``)."""
 
     compatibility: ClassVar[SearchSpaceType] = SearchSpaceType.HYBRID
     supports_discrete_subset_generating_constraints: ClassVar[bool] = True
@@ -136,12 +141,32 @@ class B200BotorchRecommender(BayesianRecommender):
     max_n_subsets: int = field(default=10, validator=[instance_of(int), ge(1)])
     """As ``BotorchRecommender.max_n_subsets`` (botorch/core.py:101-105)."""
 
+    sequential_continuous: bool = field(default=True)
+    """As ``BotorchRecommender.sequential_continuous`` (botorch/core.py:69-72); only sequential greedy is implemented."""
+
+    hybrid_sampler: DiscreteSamplingMethod | None = field(converter=optional_c(DiscreteSamplingMethod), default=None)
+    """As ``BotorchRecommender.hybrid_sampler`` (botorch/core.py:75-79)."""
+
+    sampling_percentage: float = field(default=1.0)
+    """As ``BotorchRecommender.sampling_percentage`` (botorch/core.py:81-83)."""
+
+    n_restarts: int = field(validator=[instance_of(int), gt(0)], default=10)
+    """As ``BotorchRecommender.n_restarts`` (botorch/core.py:85-88): starts polished by L-BFGS-B."""
+
+    n_raw_samples: int = field(validator=[instance_of(int), gt(0)], default=64)
+    """As ``BotorchRecommender.n_raw_samples`` (botorch/core.py:90-93): raw points of the start heuristic."""
+
     _context = field(default=None, init=False, eq=False, repr=False)
     _scorer = field(default=None, init=False, eq=False, repr=False)
     """Objectives the fused path does not serve: the ``HviScorer`` (Pareto) or ``ObjectiveScorer`` (desirability,
     non-affine single targets) set up by ``_setup_botorch_acqf``; on discrete spaces also the ``NeiScorer`` of qNEI /
     qLogNEI (its ``n_dropped``: baseline winners left out by the last evaluation)."""
     _last_acq_values: list = field(factory=list, init=False, eq=False, repr=False)
+
+    @sampling_percentage.validator
+    def _validate_percentage(self, _, value: float) -> None:
+        if not 0 <= value <= 1:
+            raise ValueError(f"Hybrid sampling percentage needs to be between 0 and 1 but is {value}")
 
     # ---- multi-target objectives (SURVEY.md 8f-4, surrogates/composite.py:59-181) ------------------------------
     def get_surrogate(self, searchspace, objective, measurements):
@@ -206,31 +231,85 @@ class B200BotorchRecommender(BayesianRecommender):
             return self._recommend_discrete_with_subsets(subspace_discrete, candidates_exp, batch_size)
         return self._recommend_discrete_without_subsets(subspace_discrete, candidates_exp, batch_size)
 
-    # ---- hybrid spaces (botorch/core.py:221-250 -> hybrid.py:30-161): search by scoring on the device -----------
+    # ---- continuous spaces (botorch/core.py:187-219 -> continuous.py:131-212): gradient path ---------------------
+    def _recommend_continuous(self, subspace_continuous, batch_size: int) -> pd.DataFrame:
+        assert self._objective is not None and self._context is not None
+        if batch_size > 1 and not self._get_acquisition_function(self._objective).supports_batching:
+            raise IncompatibleAcquisitionFunctionError(
+                f"The '{self.__class__.__name__}' only works with Monte Carlo "
+                f"acquisition functions for batch sizes > 1.")
+        _, searchspace, _ = self._context
+        pts, _, _ = self._optimize_gradient(searchspace, np.zeros((1, 0)), batch_size)
+        return pd.DataFrame(pts, columns=subspace_continuous.parameter_names)
+
+    # ---- hybrid spaces (botorch/core.py:221-250 -> hybrid.py:30-161) -------------------------------------------
     def _recommend_hybrid(self, searchspace, candidates_exp: pd.DataFrame, batch_size: int) -> pd.DataFrame:
         from baybe_b200.hybrid import recommend_hybrid
 
         assert self._objective is not None and self._context is not None
         cfg, _, pending = self._context
-        if cfg.kind != "qNEI":
+        if cfg.kind != "qNEI" and (cfg.kind not in _lib.GRAD_KINDS or self._scorer is not None):
             raise IncompatibleAcquisitionFunctionError(
-                "hybrid search spaces are served with qNoisyExpectedImprovement on the B200 engine "
-                f"(got '{cfg.kind}')")
+                "hybrid search spaces are served with qNoisyExpectedImprovement or the single-target acquisition "
+                f"functions {_lib.GRAD_KINDS} on the B200 engine (got '{cfg.kind}')")
         if searchspace.continuous.has_interpoint_constraints or searchspace.continuous.constraints_lin_eq or \
                 searchspace.continuous.constraints_lin_ineq:
             raise IncompatibilityError("continuous constraints are not supported by the B200 hybrid search")
         disc = searchspace.discrete.transform(candidates_exp)  # comp-rep of the discrete part, comes first
-        cb = searchspace.continuous.comp_rep_bounds.to_numpy(dtype=np.float64)
-        pend = None
-        if pending is not None and len(pending) > 0:
-            pend = searchspace.transform(pending, allow_extra=True).to_numpy(dtype=np.float64)
-        pts, idx, value = recommend_hybrid(self._surrogate_model.device_gp, cfg, disc.to_numpy(dtype=np.float64), cb,
-                                           batch_size, pend, self.n_mc_samples, _draw_sampler_seed())
+        if cfg.kind != "qNEI":
+            if batch_size > 1 and not self._get_acquisition_function(self._objective).supports_batching:
+                raise IncompatibleAcquisitionFunctionError(
+                    f"The '{self.__class__.__name__}' only works with Monte Carlo "
+                    f"acquisition functions for batch sizes > 1.")
+            if self.hybrid_sampler is not None:
+                disc = sample_numerical_df(disc, math.ceil(self.sampling_percentage * len(disc.index)),
+                                           method=self.hybrid_sampler)
+            pts, idx, value = self._optimize_gradient(searchspace, disc.to_numpy(dtype=np.float64), batch_size)
+        else:
+            cb = searchspace.continuous.comp_rep_bounds.to_numpy(dtype=np.float64)
+            pend = None
+            if pending is not None and len(pending) > 0:
+                pend = searchspace.transform(pending, allow_extra=True).to_numpy(dtype=np.float64)
+            pts, idx, value = recommend_hybrid(self._surrogate_model.device_gp, cfg, disc.to_numpy(dtype=np.float64),
+                                               cb, batch_size, pend, self.n_mc_samples, _draw_sampler_seed())
         self._last_acq_values[:] = [value]
         rec_disc = searchspace.discrete.exp_rep.loc[disc.index[idx]]
         rec_cont = pd.DataFrame(pts[:, disc.shape[1]:], columns=searchspace.continuous.parameter_names,
                                 index=rec_disc.index)
         return pd.concat([rec_disc, rec_cont], axis=1)
+
+    def _optimize_gradient(self, searchspace, disc_comp: np.ndarray, batch_size: int):
+        """Multi-start L-BFGS-B on ``bb_acq_grad`` over disc_comp x the continuous box (``baybe_b200.continuous``):
+        (points in comp-rep column order, configuration indices, joint value of [batch; pending])."""
+        from baybe.parameters.numerical import _FixedNumericalContinuousParameter
+
+        from baybe_b200.continuous import recommend_continuous_hybrid
+
+        cfg, _, pending = self._context
+        cont = searchspace.continuous
+        if cfg.kind not in _lib.GRAD_KINDS or self._scorer is not None:
+            raise IncompatibleAcquisitionFunctionError(
+                f"continuous search spaces are served with the single-target acquisition functions {_lib.GRAD_KINDS} "
+                f"on the B200 engine (got '{cfg.kind}')")
+        if not self.sequential_continuous:
+            raise NotImplementedError("joint (non-sequential) q-batch optimisation is not implemented by the B200 "
+                                      "engine: use sequential_continuous=True")
+        if cont.has_interpoint_constraints or cont.constraints_lin_eq or cont.constraints_lin_ineq or \
+                cont.n_subsets > 0:
+            raise IncompatibilityError("continuous constraints (linear, interpoint and cardinality) are not supported "
+                                       "by the B200 gradient path")
+        if getattr(searchspace, "task_idx", None) is not None:
+            raise IncompatibilityError("task parameters are not supported by the B200 gradient path")
+        fixed = {j: float(p.value) for j, p in enumerate(cont.parameters)
+                 if isinstance(p, _FixedNumericalContinuousParameter)}
+        pend = None
+        if pending is not None and len(pending) > 0:
+            pend = searchspace.transform(pending, allow_extra=True).to_numpy(dtype=np.float64)
+        pts, idx, value = recommend_continuous_hybrid(
+            self._surrogate_model.device_gp, cfg, disc_comp, cont.comp_rep_bounds.to_numpy(dtype=np.float64),
+            batch_size, pend, self.n_mc_samples, _draw_sampler_seed(), self.n_raw_samples, self.n_restarts, fixed)
+        self._last_acq_values[:] = [value]
+        return pts, idx, value
 
     def _recommend_discrete_without_subsets(self, subspace_discrete, candidates_exp, batch_size) -> pd.Index:
         cfg, searchspace, pending = self._context

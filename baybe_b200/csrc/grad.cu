@@ -1,0 +1,622 @@
+// grad.cu -- value and gradient of a single-target acquisition function at P points (bb_acq_grad).
+//
+// Replaces the autograd pass of the reference's continuous optimiser: optimize_acqf's L-BFGS-B on
+// acqf(X).backward() (baybe/recommenders/pure/bayesian/botorch/continuous.py:184) and the same inside
+// optimize_acqf_mixed with the discrete features held fixed (botorch/hybrid.py:110).
+//
+// One warp per point, all on the CUDA cores in fp32 (the analytic kinds' closed forms in float64, as
+// analytic_value).  With a = x * scale + shift (bb_model's d_cand_scale / d_cand_shift) and b_i the scaled training
+// rows:
+//   k_i = s_f^2 kappa(|a - b_i|),  v = L^-1 k,  u = L^-T v,
+//   mu = y_mean + s_y (c + k . alpha),  var = s_y^2 max(s_f^2 - |v|^2, 1e-10),
+//   c_p = s_y^2 (k(x, x_p) - k . beta_p)                          (pending points p)
+// and, with A_mu, A_var, A_c[p] the partial derivatives of the acquisition value,
+//   dA/dk_i = s_y A_mu alpha_i - 2 s_y^2 A_var u_i - s_y^2 sum_p A_c[p] beta_p,i
+//   grad_x A = (sum_i dA/dk_i dk_i/da + s_y^2 sum_p A_c[p] dk(x, x_p)/da) * scale.
+// v is formed 32 rows at a time: each lane takes every 32nd column of the 32 rows (coalesced loads of L^-1) and a
+// reduce-scatter over the warp leaves row j0 + l in lane l; u needs no reduction (lane l owns column i0 + l).
+// With pending points the value is k_acq_joint's (acq.cu): the Cholesky of [[var, c^T], [c, Sigma_PP]] with the
+// candidate first, the same jitter escalation and the same join of the pending points' terms.  Its reverse pass
+// accumulates dA/dL22 over the samples and goes back through the (1+p) Cholesky with
+//   dA/dA22 = sym(L22^-T Phi(L22^T dL22) L22^-1) / 2  (as torch's cholesky backward),  A22 = Sigma_PP - l l^T,
+// so only dA/dl = -2 (dA/dA22) l is needed: two triangular solves and one matrix-vector product per point.
+// Every reduction has a fixed order and nothing is accumulated atomically: repeated calls are bit-identical.
+#include <math.h>
+
+#include "acq_math.cuh"
+#include "common.cuh"
+#include "fused_common.cuh"
+
+namespace bb {
+
+constexpr int kGradThreads = 128;  // four points per block
+constexpr int kGradWarps = kGradThreads / 32;
+constexpr int kGradMaxNPad = 256;
+constexpr unsigned kFull = 0xffffffffu;
+
+struct GradParams {
+  bb_acq_spec a;
+  const float* x;  // [N][d]
+  int64_t N;
+  const float *cand_scale, *cand_shift, *train_m2, *alpha, *linv;
+  int n, n_pad, d, d_pad;
+  const float* mean_const;  // [1]
+  float y_mean, y_std, sf2;
+  int P;
+  const float *pend_x, *pend_beta, *pend_mu, *pend_cov;  // [P][d], [P][n_pad], [P], [P][P]
+  const float* z;                                          // [S][1+P]
+  int S;
+  float* value;  // [N]
+  float* grad;   // [N][d]
+};
+
+// per-warp scratch in floats: a | k (then dA/dk_i * dk_i/dt) | gk | v | 5 x 32 vectors | L22 | dL22 | 2 x sample chunk
+__host__ __device__ inline int grad_warp_floats(int n_pad, int d_pad, int P) {
+  return (d_pad + 3 * n_pad + 5 * 32 + 2 * P * P + 2 * 32 * (P + 1) + 3) & ~3;
+}
+
+// kernel value k(t) and dk/dt of the scaled squared distance t (the family's constant is folded into the scale)
+template <int FAMILY>
+__device__ __forceinline__ void kernel_and_slope(float t, float& k, float& dkdt) {
+  t = fmaxf(t, 0.f);
+  if constexpr (FAMILY == BB_KERNEL_RBF) {
+    k = exp2f(-t);
+    dkdt = -kLn2 * k;
+  } else {
+    const float s = sqrtf(t), e = expf(-s);
+    if constexpr (FAMILY == BB_KERNEL_MATERN12) {
+      k = e;
+      dkdt = s > 0.f ? -0.5f * e / s : 0.f;  // kappa'(r)/r taken as 0 at r = 0
+    } else if constexpr (FAMILY == BB_KERNEL_MATERN32) {
+      k = (1.f + s) * e;
+      dkdt = -0.5f * e;
+    } else {
+      k = (1.f + s + t * (1.f / 3.f)) * e;
+      dkdt = -(1.f + s) * e * (1.f / 6.f);
+    }
+  }
+}
+
+__device__ __forceinline__ float warp_sum(float v) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
+  return v;
+}
+
+__device__ __forceinline__ float sigmoidf_(float t) { return 1.f / (1.f + expf(-t)); }
+
+// sigmoid'(t) = e / (1 + e)^2, e = exp(-t): no cancellation in 1 - sigmoid(t) where sigmoid(t) is near 1
+__device__ __forceinline__ float dsigmoidf_(float t) {
+  const float e = expf(-t);
+  return isinf(e) ? 0.f : e / ((1.f + e) * (1.f + e));
+}
+
+// d/dt log(softplus(t) + 0.1 / (1 + t^2)) and the value inside the log
+__device__ __forceinline__ float dlog_fatplus_t(float t) {
+  const float q = 1.f / fmaf(t, t, 1.f);
+  const float sp = fmaxf(t, 0.f) + ((fabsf(t) < 30.f) ? log1pf(expf(-fabsf(t))) : 0.f);
+  return (sigmoidf_(t) - 0.2f * (t * q) * q) / (sp + 0.1f * q);
+}
+
+// partial derivatives (A_mu, A_sd) of the analytic kinds, float64
+__device__ __forceinline__ void analytic_partials(const bb_acq_spec& a, float mu, float var, double& dmu,
+                                                  double& dsd) {
+  const double a1 = (double)a.obj_scale, aa = fabs(a1);
+  const double m = a1 * (double)mu + (double)a.obj_shift;
+  const double s = aa * sqrt((double)var);
+  dmu = 0.0;
+  dsd = 0.0;
+  switch (a.kind) {
+    case BB_ACQ_PM: dmu = a1; return;
+    case BB_ACQ_PSTD: dsd = a.maximize ? aa : -aa; return;
+    case BB_ACQ_UCB: dmu = a1; dsd = sqrt((double)a.beta) * aa; return;
+    default: break;
+  }
+  const double u = (m - (double)a.best_f) / s;
+  if (a.kind == BB_ACQ_EI) {
+    dmu = a1 * norm_cdf(u);
+    dsd = aa * norm_pdf(u);
+  } else if (a.kind == BB_ACQ_LOGEI) {
+    // Phi(u) / h(u) = exp(log Phi(u) - log h(u)), h(u) = phi(u) + u Phi(u): never formed as a ratio
+    const double log_Phi = u > -1.0 ? log(norm_cdf(u))
+                                    : log(0.5 * erfcx(-u * 0.7071067811865476)) - 0.5 * u * u;
+    const double r = exp(log_Phi - log_ei_helper(u));
+    dmu = a1 * r / s;
+    dsd = aa * (1.0 - u * r) / s;
+  } else {  // PI
+    dmu = a1 * norm_pdf(u) / s;
+    dsd = -aa * u * norm_pdf(u) / s;
+  }
+}
+
+template <int FAMILY>
+__global__ void __launch_bounds__(kGradThreads) k_acq_grad(const GradParams p) {
+  extern __shared__ __align__(16) float smem_g[];
+  const int P = p.P, Q = P + 1, zs = Q | 1;
+  const bool is_mc = p.a.kind <= BB_ACQ_QPI;
+  const int S = is_mc ? p.S : 0;
+  float* z_s = smem_g;  // [S][zs]
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* wb = z_s + ((S * zs + 3) & ~3) + warp * grad_warp_floats(p.n_pad, p.d_pad, P);
+  float* a_w = wb;
+  float* k_w = a_w + p.d_pad;
+  float* gk_w = k_w + p.n_pad;
+  float* v_w = gk_w + p.n_pad;
+  float* lv = v_w + p.n_pad;  // [32] l = c / sd
+  float* mP = lv + 32;        // [32] pending means
+  float* moP = mP + 32;       // [32] qUCB: sample mean of each pending point's objective
+  float* gkp = moP + 32;      // [32] 2 s_f^2 dk/dt of k(x, x_p)
+  float* acw = gkp + 32;      // [32] A_c[p]
+  float* Lw = acw + 32;       // [P][P] L22
+  float* Lb = Lw + P * P;     // [P][P] dA/dL22
+  float* Wc = Lb + P * P;     // [32][Q] per-sample weights of the current chunk
+  float* Wm = Wc + 32 * Q;    // [32][Q] qUCB: weights of the sample means
+  for (int e = threadIdx.x; e < S * Q; e += blockDim.x) {
+    const int s = e / Q, k = e - s * Q;
+    z_s[s * zs + k] = __ldg(p.z + e);
+  }
+  __syncthreads();
+  const bb_acq_spec a = p.a;
+  const float a1 = a.obj_scale, a0 = a.obj_shift, sy = p.y_std, sy2 = sy * sy;
+  const float ucb_c = sqrtf(a.beta * 1.5707963267948966f);
+  // column means of the base samples (lane k: column k) and, for q = 1, mean |z - mean z|
+  float zb = 0.f, zdev = 0.f;
+  if (is_mc) {
+    if (lane < Q) {
+      for (int s = 0; s < S; ++s) zb += z_s[s * zs + lane];
+      zb /= (float)S;
+    }
+    if (P == 0) {
+      float sz = 0.f;
+      for (int s = lane; s < S; s += 32) sz += z_s[s * zs];
+      const float zm = warp_sum(sz) / (float)S;
+      float sa = 0.f;
+      for (int s = lane; s < S; s += 32) sa += fabsf(z_s[s * zs] - zm);
+      zdev = warp_sum(sa) / (float)S;
+      zb = zm;  // same value in every lane
+    }
+  }
+  const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t c = warp_global; c < p.N; c += nwarps) {
+    // ---- forward: a, k, mu, v, var, cross ----
+    for (int j = lane; j < p.d_pad; j += 32)
+      a_w[j] = j < p.d ? fmaf(__ldg(p.x + c * p.d + j), __ldg(p.cand_scale + j), __ldg(p.cand_shift + j)) : 0.f;
+    __syncwarp();
+    float ka = 0.f;
+    for (int i = lane; i < p.n_pad; i += 32) {
+      float t = 0.f;
+      for (int j = 0; j < p.d; ++j) {
+        const float df = a_w[j] + 0.5f * __ldg(p.train_m2 + (size_t)i * p.d_pad + j);
+        t = fmaf(df, df, t);
+      }
+      float k, dk;
+      kernel_and_slope<FAMILY>(t, k, dk);
+      k = i < p.n ? p.sf2 * k : 0.f;
+      k_w[i] = k;
+      gk_w[i] = i < p.n ? 2.f * p.sf2 * dk : 0.f;
+      ka = fmaf(k, __ldg(p.alpha + i), ka);
+    }
+    ka = warp_sum(ka);
+    __syncwarp();
+    float vv = 0.f;
+    for (int j0 = 0; j0 < p.n_pad; j0 += 32) {
+      float r[32];
+#pragma unroll
+      for (int q = 0; q < 32; ++q) r[q] = 0.f;
+      for (int i0 = 0; i0 <= j0; i0 += 32) {
+        const float ki = k_w[i0 + lane];
+        const float* Lr = p.linv + (size_t)j0 * p.n_pad + i0 + lane;
+#pragma unroll
+        for (int q = 0; q < 32; ++q) r[q] = fmaf(__ldg(Lr + (size_t)q * p.n_pad), ki, r[q]);
+      }
+#pragma unroll
+      for (int off = 16; off >= 1; off >>= 1) {  // reduce-scatter: lane l ends with row j0 + l
+        const bool up = (lane & off) != 0;
+#pragma unroll
+        for (int q = 0; q < off; ++q) {
+          const float send = up ? r[q] : r[q + off];
+          const float keep = up ? r[q + off] : r[q];
+          r[q] = keep + __shfl_xor_sync(kFull, send, off);
+        }
+      }
+      v_w[j0 + lane] = r[0];
+      vv = fmaf(r[0], r[0], vv);
+    }
+    vv = warp_sum(vv);
+    const float vt = p.sf2 - vv;
+    const bool var_free = vt > 1e-10f;  // the clamp passes no gradient
+    const float mu = fmaf(sy, __ldg(p.mean_const) + ka, p.y_mean);
+    const float var = sy2 * fmaxf(vt, 1e-10f);
+    float cr = 0.f;  // lane p < P: c_p
+    for (int q = 0; q < P; ++q) {
+      float kb = 0.f;
+      for (int i = lane; i < p.n_pad; i += 32) kb = fmaf(k_w[i], __ldg(p.pend_beta + (size_t)q * p.n_pad + i), kb);
+      kb = warp_sum(kb);
+      if (lane == q) cr = kb;
+    }
+    if (lane < P) {
+      float t = 0.f;
+      for (int j = 0; j < p.d; ++j) {
+        const float b = fmaf(__ldg(p.pend_x + (size_t)lane * p.d + j), __ldg(p.cand_scale + j), __ldg(p.cand_shift + j));
+        const float df = a_w[j] - b;
+        t = fmaf(df, df, t);
+      }
+      float k, dk;
+      kernel_and_slope<FAMILY>(t, k, dk);
+      cr = sy2 * (p.sf2 * k - cr);
+      gkp[lane] = 2.f * p.sf2 * dk;
+    }
+    __syncwarp();
+    // ---- value and its partial derivatives (A_mu, A_var, A_c) ----
+    float value, g_mu = 0.f, g_var = 0.f;
+    if (!is_mc) {
+      value = analytic_value(a, mu, var);
+      double dmu, dsd;
+      analytic_partials(a, mu, var, dmu, dsd);
+      g_mu = (float)dmu;
+      g_var = (float)(dsd / (2.0 * sqrt((double)var)));
+    } else if (P == 0) {
+      float c0, c1;
+      mc_coef(a, mu, var, c0, c1);
+      const float sd = sqrtf(var);
+      float s0 = 0.f, s1 = 0.f, h0 = 0.f, h1 = 0.f;  // value sums; sums of d(term)/dt and d(term)/dt * z
+      for (int s = lane; s < S; s += 32) {
+        const float zz = z_s[s * zs], t = fmaf(c1, zz, c0);
+        float g = 0.f;
+        if (a.kind == BB_ACQ_QLOGEI) {
+          const float q = 1.f / fmaf(t, t, 1.f);
+          s0 += fmaxf(t, 0.f) + ((fabsf(t) < 30.f) ? log1pf(expf(-fabsf(t))) : 0.f);
+          s1 += q;
+          g = sigmoidf_(t) - 0.2f * (t * q) * q;
+        } else if (a.kind == BB_ACQ_QEI) {
+          s0 += fmaxf(t, 0.f);
+          g = t > 0.f ? 1.f : 0.f;
+        } else if (a.kind == BB_ACQ_QPI) {
+          s0 += sigmoidf_(t);
+          g = dsigmoidf_(t);
+        }
+        h0 += g;
+        h1 = fmaf(g, zz, h1);
+      }
+      s0 = warp_sum(s0);
+      s1 = warp_sum(s1);
+      h0 = warp_sum(h0);
+      h1 = warp_sum(h1);
+      value = mc_finalize(a, mu, var, s0, s1, S, zb, zdev);
+      float d_mu, d_sd;
+      if (a.kind == BB_ACQ_QSR || a.kind == BB_ACQ_QUCB) {
+        d_mu = a1;
+        d_sd = a1 * zb + (a.kind == BB_ACQ_QUCB ? ucb_c * fabsf(a1) * zdev : 0.f);
+      } else {
+        const float inv_tau = a.kind == BB_ACQ_QLOGEI ? 1.f / a.tau_relu : a.kind == BB_ACQ_QPI ? 1.f / a.tau_pi : 1.f;
+        const float norm = a.kind == BB_ACQ_QLOGEI ? 1.f / (s0 + 0.1f * s1) : 1.f / (float)S;
+        d_mu = a1 * inv_tau * h0 * norm;
+        d_sd = a1 * inv_tau * h1 * norm;
+      }
+      g_mu = d_mu;
+      g_var = d_sd / (2.f * sd);
+    } else {
+      // ---- k_acq_joint's forward: Cholesky of the joint covariance, candidate first ----
+      float sd = 0.f;
+      bool ok = false;
+      for (int attempt = 0; attempt < 4 && !ok; ++attempt) {
+        const float jit = attempt == 0 ? 0.f : 1e-6f * __powf(10.f, (float)(attempt - 1));
+        sd = sqrtf(var + jit);
+        const float li = cr / sd;
+        __syncwarp();
+        if (lane < P) {
+          lv[lane] = li;
+          mP[lane] = __ldg(p.pend_mu + lane);
+        }
+        __syncwarp();
+        if (lane < P)
+          for (int j = 0; j <= lane; ++j)
+            Lw[lane * P + j] = __ldg(p.pend_cov + lane * P + j) - li * lv[j] + (j == lane ? jit : 0.f);
+        __syncwarp();
+        bool fail = !(var + jit > 0.f);
+        for (int j = 0; j < P; ++j) {
+          const float dj = Lw[j * P + j];
+          if (!(dj > 0.f)) {
+            fail = true;
+            break;
+          }
+          const float sj = sqrtf(dj);
+          __syncwarp();
+          if (lane == j) Lw[j * P + j] = sj;
+          if (lane > j && lane < P) Lw[lane * P + j] /= sj;
+          __syncwarp();
+          if (lane > j && lane < P) {
+            const float lij = Lw[lane * P + j];
+            for (int k = j + 1; k <= lane; ++k) Lw[lane * P + k] -= lij * Lw[k * P + j];
+          }
+          __syncwarp();
+        }
+        ok = !fail;
+      }
+      __syncwarp();
+      const float zb0 = __shfl_sync(kFull, zb, 0);
+      {
+        float ym = (lane < P) ? fmaf(lv[lane], zb0, mP[lane]) : 0.f;
+        for (int j = 0; j < P; ++j) {
+          const float zbj = __shfl_sync(kFull, zb, 1 + j);
+          if (lane < P && j <= lane) ym = fmaf(Lw[lane * P + j], zbj, ym);
+        }
+        if (lane < P) moP[lane] = fmaf(a1, ym, a0);
+        __syncwarp();
+      }
+      const float mo_c = fmaf(a1, fmaf(sd, zb0, mu), a0);
+      // per-sample terms of point i (0: the candidate) from its objective o
+      auto term = [&](int i, float o) -> float {
+        if (a.kind == BB_ACQ_QLOGEI) return logf(a.tau_relu) + log_fatplus_t((o - a.best_f) / a.tau_relu);
+        if (a.kind == BB_ACQ_QEI) return fmaxf(o - a.best_f, 0.f);
+        if (a.kind == BB_ACQ_QSR) return o;
+        if (a.kind == BB_ACQ_QPI) return 1.0f / (1.0f + __expf(-(o - a.best_f) / a.tau_pi));
+        const float m = i == 0 ? mo_c : moP[i - 1];
+        return m + ucb_c * fabsf(o - m);
+      };
+      auto sample_obj = [&](const float* zr, int i) -> float {  // o of point i >= 1 in sample zr
+        float y = fmaf(lv[i - 1], zr[0], mP[i - 1]);
+        const float* Li = Lw + (i - 1) * P;
+        for (int j = 0; j < i; ++j) y = fmaf(Li[j], zr[1 + j], y);
+        return fmaf(a1, y, a0);
+      };
+      // pass 1: the value, exactly as k_acq_joint forms it
+      float run_max = -INFINITY, run_sum = 0.f;
+      for (int s = lane; s < S; s += 32) {
+        const float* zr = z_s + s * zs;
+        float li_arr[BB_MAX_PENDING + 1];
+        float red = term(0, fmaf(a1, fmaf(sd, zr[0], mu), a0));
+        li_arr[0] = red;
+        for (int i = 1; i < Q; ++i) {
+          const float val = term(i, sample_obj(zr, i));
+          li_arr[i] = val;
+          red = fmaxf(red, val);
+        }
+        if (a.kind == BB_ACQ_QLOGEI) lse_push(fatmax_q(li_arr, Q, red, a.tau_max), run_max, run_sum);
+        else run_sum += red;
+      }
+      float lse = 0.f;
+      if (a.kind == BB_ACQ_QLOGEI) {
+        lse_warp_combine(run_max, run_sum);
+        lse = run_max + logf(run_sum);
+        value = lse - logf((float)S);
+      } else {
+        value = warp_sum(run_sum) / (float)S;
+      }
+      // pass 2: per-sample weights dA/dy_i in chunks of 32 samples, accumulated into dA/d(mu, sd, l, L22)
+      float acc_l = 0.f, acc_m = 0.f, acc_wm = 0.f, acc_mu = 0.f, acc_sd = 0.f;
+      for (int e = lane; e < P * P; e += 32) Lb[e] = 0.f;
+      for (int s0 = 0; s0 < S; s0 += 32) {
+        const int s = s0 + lane;
+        __syncwarp();
+        for (int i = 0; i < Q; ++i) {
+          Wc[lane * Q + i] = 0.f;
+          Wm[lane * Q + i] = 0.f;
+        }
+        if (s < S) {
+          const float* zr = z_s + s * zs;
+          float ob[BB_MAX_PENDING + 1], li_arr[BB_MAX_PENDING + 1];
+          ob[0] = fmaf(a1, fmaf(sd, zr[0], mu), a0);
+          float red = term(0, ob[0]);
+          li_arr[0] = red;
+          int imax = 0;
+          for (int i = 1; i < Q; ++i) {
+            ob[i] = sample_obj(zr, i);
+            const float val = term(i, ob[i]);
+            li_arr[i] = val;
+            if (val > red) {
+              red = val;
+              imax = i;
+            }
+          }
+          float w_s = 1.f / (float)S;  // dA/d(reduced sample)
+          if (a.kind == BB_ACQ_QLOGEI) {
+            const float fm = fatmax_q(li_arr, Q, red, a.tau_max);
+            w_s = expf(fm - lse);
+            const float inv = 1.0f / (2.0f * a.tau_max);
+            float ssum = 0.f;
+            for (int k = 0; k < Q; ++k) {
+              const float w = fmaf(red - li_arr[k], inv, 1.0f);
+              ssum += 1.0f / (w * w);
+            }
+            float rest = 0.f;
+            for (int k = 0; k < Q; ++k) {
+              const float w = fmaf(red - li_arr[k], inv, 1.0f);
+              const float dk = 1.0f / (w * w * w) / ssum;
+              rest += dk;
+              Wc[lane * Q + k] = dk;
+            }
+            Wc[lane * Q + imax] += 1.f - rest;
+            for (int k = 0; k < Q; ++k)
+              Wc[lane * Q + k] *= w_s * a1 * dlog_fatplus_t((ob[k] - a.best_f) / a.tau_relu) / a.tau_relu;
+          } else {
+            float d;
+            const float o = ob[imax];
+            if (a.kind == BB_ACQ_QEI) d = o - a.best_f > 0.f ? 1.f : 0.f;
+            else if (a.kind == BB_ACQ_QSR) d = 1.f;
+            else if (a.kind == BB_ACQ_QPI) {
+              d = dsigmoidf_((o - a.best_f) / a.tau_pi) / a.tau_pi;
+            } else {
+              const float m = imax == 0 ? mo_c : moP[imax - 1];
+              const float sgn = o > m ? 1.f : (o < m ? -1.f : 0.f);
+              d = ucb_c * sgn;
+              Wm[lane * Q + imax] = w_s * a1 * (1.f - d);
+            }
+            Wc[lane * Q + imax] = w_s * a1 * d;
+          }
+        }
+        __syncwarp();
+        const int ns = min(32, S - s0);
+        for (int t = 0; t < ns; ++t) {
+          const float* zr = z_s + (s0 + t) * zs;
+          const float* wr = Wc + t * Q;
+          if (lane < P) {
+            const float w = wr[1 + lane];
+            acc_l = fmaf(w, zr[0], acc_l);
+            acc_wm += Wm[t * Q + 1 + lane];
+            float* Lbr = Lb + lane * P;
+            for (int j = 0; j <= lane; ++j) Lbr[j] = fmaf(w, zr[1 + j], Lbr[j]);
+          } else if (lane == P) {
+            acc_mu += wr[0];
+            acc_sd = fmaf(wr[0], zr[0], acc_sd);
+            acc_m += Wm[t * Q];
+          }
+        }
+      }
+      __syncwarp();
+      // qUCB: the sample means carry weight too (they depend on the inputs like a sample with z = column means)
+      if (a.kind == BB_ACQ_QUCB) {
+        if (lane < P) acc_l = fmaf(acc_wm, zb0, acc_l);
+        for (int j = 0; j < P; ++j) {  // column j + 1's mean sits in lane j + 1
+          const float zbj = __shfl_sync(kFull, zb, 1 + j);
+          if (lane < P && j <= lane) Lb[lane * P + j] = fmaf(acc_wm, zbj, Lb[lane * P + j]);
+        }
+        if (lane == P) {
+          acc_mu += acc_m;
+          acc_sd = fmaf(acc_m, zb0, acc_sd);
+        }
+      }
+      __syncwarp();
+      // ---- back through the Cholesky of A22 = Sigma_PP - l l^T + jit I ----
+      float* Mw = Wc;  // [P][P] tril(L22^T dL22)
+      if (lane < P)
+        for (int j = 0; j <= lane; ++j) {
+          float m = 0.f;
+          for (int k = lane; k < P; ++k) m = fmaf(Lw[k * P + lane], Lb[k * P + j], m);
+          Mw[lane * P + j] = m;
+        }
+      __syncwarp();
+      // w = L22^-1 l (forward substitution), lane i holds w_i
+      float res = lane < P ? lv[lane] : 0.f, wv = 0.f;
+      for (int j = 0; j < P; ++j) {
+        const float wj = __shfl_sync(kFull, res, j) / Lw[j * P + j];
+        if (lane == j) wv = wj;
+        if (lane > j && lane < P) res = fmaf(-Lw[lane * P + j], wj, res);
+      }
+      // h = G w, G = (tril(M) + tril(M, -1)^T) / 2
+      float hv = 0.f;
+      for (int j = 0; j < P; ++j) {
+        const float wj = __shfl_sync(kFull, wv, j);
+        if (lane < P) hv = fmaf(j <= lane ? Mw[lane * P + j] : Mw[j * P + lane], wj, hv);
+      }
+      hv *= 0.5f;
+      // q = L22^-T h (back substitution), lane i holds q_i
+      res = hv;
+      float qv = 0.f;
+      for (int j = P - 1; j >= 0; --j) {
+        const float qj = __shfl_sync(kFull, res, j) / Lw[j * P + j];
+        if (lane == j) qv = qj;
+        if (lane < j) res = fmaf(-Lw[j * P + lane], qj, res);
+      }
+      const float lbar = lane < P ? acc_l - 2.f * qv : 0.f;
+      // l = c / sd: A_c = lbar / sd, and sd picks up -sum_i lbar_i l_i / sd
+      const float sd_l = warp_sum(lane < P ? lbar * lv[lane] : 0.f);
+      const float mu_bar = __shfl_sync(kFull, acc_mu, P), sd_bar = __shfl_sync(kFull, acc_sd, P) - sd_l / sd;
+      g_mu = mu_bar;
+      g_var = sd_bar / (2.f * sd);
+      if (lane < P) acw[lane] = lbar / sd;
+      if (!ok) {
+        value = __int_as_float(0x7fc00000);
+        g_mu = g_var = 0.f;
+        if (lane < P) acw[lane] = 0.f;
+      }
+      __syncwarp();
+    }
+    if (!var_free) g_var = 0.f;
+    // ---- dA/dk_i, folded with dk_i/dt into k_w: coef_i = gk_i dA/dk_i ----
+    const float k_mu = sy * g_mu, k_var = -2.f * sy2 * g_var;
+    for (int i0 = 0; i0 < p.n_pad; i0 += 32) {
+      const int i = i0 + lane;
+      float u = 0.f;
+      for (int j = i0; j < p.n_pad; ++j) u = fmaf(__ldg(p.linv + (size_t)j * p.n_pad + i), v_w[j], u);
+      float kb = fmaf(k_mu, __ldg(p.alpha + i), k_var * u);
+      for (int q = 0; q < P; ++q) kb = fmaf(-sy2 * acw[q], __ldg(p.pend_beta + (size_t)q * p.n_pad + i), kb);
+      k_w[i] = gk_w[i] * kb;
+    }
+    __syncwarp();
+    // ---- gradient: lanes over columns ----
+    for (int j = lane; j < p.d; j += 32) {
+      const float aj = a_w[j];
+      float g = 0.f;
+      for (int i = 0; i < p.n; ++i) g = fmaf(k_w[i], aj + 0.5f * __ldg(p.train_m2 + (size_t)i * p.d_pad + j), g);
+      for (int q = 0; q < P; ++q) {
+        const float b = fmaf(__ldg(p.pend_x + (size_t)q * p.d + j), __ldg(p.cand_scale + j), __ldg(p.cand_shift + j));
+        g = fmaf(sy2 * acw[q] * gkp[q], aj - b, g);
+      }
+      p.grad[c * p.d + j] = g * __ldg(p.cand_scale + j);
+    }
+    if (lane == 0) p.value[c] = value;
+    __syncwarp();
+  }
+}
+
+}  // namespace bb
+
+using namespace bb;
+
+extern "C" int bb_acq_grad(const bb_model* m, const bb_acq_spec* a, const float* d_x, int64_t N, int32_t n_pending,
+                           const float* d_pend_x, const float* d_pend_beta, const float* d_pend_mu,
+                           const float* d_pend_cov, const float* d_z, int32_t S, float* d_value, float* d_grad,
+                           void* stream) {
+  BB_CHECK_ARG(m && m->abi_version == BB_ABI_VERSION, "bb_acq_grad: model struct missing or ABI mismatch");
+  BB_CHECK_ARG(a != nullptr, "bb_acq_grad: acquisition spec is null");
+  BB_CHECK_ARG(a->kind >= BB_ACQ_QLOGEI && a->kind <= BB_ACQ_PSTD, "bb_acq_grad: acquisition kind %d is not one of "
+               "the single-target kinds", a->kind);
+  BB_CHECK_SUPPORTED(!m->wide, "bb_acq_grad: wide-feature models are not supported");
+  BB_CHECK_SUPPORTED(m->task_col < 0, "bb_acq_grad: models with a task parameter are not supported");
+  BB_CHECK_SUPPORTED(m->n_pad <= kGradMaxNPad, "bb_acq_grad: n_pad=%d above %d is not supported", m->n_pad,
+                     kGradMaxNPad);
+  BB_CHECK_ARG(N >= 0, "bb_acq_grad: negative point count");
+  const bool is_mc = a->kind <= BB_ACQ_QPI;
+  BB_CHECK_ARG(n_pending >= 0 && n_pending <= BB_MAX_PENDING, "bb_acq_grad: n_pending=%d outside [0,%d]", n_pending,
+               BB_MAX_PENDING);
+  BB_CHECK_ARG(n_pending == 0 || is_mc, "bb_acq_grad: pending points need a Monte Carlo acquisition function");
+  BB_CHECK_ARG(!is_mc || (S >= 1 && S <= kMaxSamples), "bb_acq_grad: S=%d outside [1,%d]", S, kMaxSamples);
+  BB_CHECK_ARG(!is_mc || d_z != nullptr, "bb_acq_grad: null base samples");
+  BB_CHECK_ARG(n_pending == 0 || (d_pend_x && d_pend_beta && d_pend_mu && d_pend_cov),
+               "bb_acq_grad: null pending buffer");
+  if (N == 0) return BB_OK;
+  BB_CHECK_ARG(d_x && d_value && d_grad, "bb_acq_grad: null buffer");
+  GradParams p;
+  p.a = *a;
+  p.x = d_x;
+  p.N = N;
+  p.cand_scale = m->d_cand_scale;
+  p.cand_shift = m->d_cand_shift;
+  p.train_m2 = m->d_train_m2;
+  p.alpha = m->d_alpha;
+  p.linv = m->d_linv32;
+  p.n = m->n;
+  p.n_pad = m->n_pad;
+  p.d = m->d;
+  p.d_pad = m->d_pad;
+  p.y_mean = m->y_mean;
+  p.y_std = m->y_std;
+  p.P = n_pending;
+  p.pend_x = d_pend_x;
+  p.pend_beta = d_pend_beta;
+  p.pend_mu = d_pend_mu;
+  p.pend_cov = d_pend_cov;
+  p.z = d_z;
+  p.S = is_mc ? S : 0;
+  p.value = d_value;
+  p.grad = d_grad;
+  p.sf2 = m->prior_scale;  // single task: the prior variance s_f^2
+  int sms, max_smem;
+  int rc = device_limits(&sms, &max_smem);
+  if (rc != BB_OK) return rc;
+  p.mean_const = m->d_mean_const;
+  const int zs = (n_pending + 1) | 1;
+  const size_t smem = ((size_t)((p.S * zs + 3) & ~3) + (size_t)kGradWarps * grad_warp_floats(p.n_pad, p.d_pad,
+                                                                                             n_pending)) * 4;
+  BB_CHECK_SUPPORTED(smem <= (size_t)max_smem, "bb_acq_grad: S*(1+n_pending)=%d too large for shared memory",
+                     p.S * zs);
+  int64_t blocks = (N + kGradWarps - 1) / kGradWarps;
+  if (blocks > (int64_t)sms * 8) blocks = (int64_t)sms * 8;
+  return dispatch_family<true>(m->family, [&](auto fam) {
+    BB_SMEM_OPTIN_ONCE(k_acq_grad<decltype(fam)::value>);
+    k_acq_grad<decltype(fam)::value><<<(int)blocks, kGradThreads, smem, (cudaStream_t)stream>>>(p);
+    BB_LAUNCH_CHECK();
+    return BB_OK;
+  });
+}

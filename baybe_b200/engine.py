@@ -407,6 +407,23 @@ class DeviceGP:
         return torch.ops.baybe_b200.acq_score_joint(mu, var, cross, pmu, pcov, zf,
                                                     _lib.ACQ_KIND[acq.kind], acq.params())
 
+    def value_and_grad(self, acq: AcqConfig, x, z: torch.Tensor | None, pending=None):
+        """Acquisition value [N] and its gradient [N, d] with respect to the raw comp-rep rows x (``bb_acq_grad``).
+        Without pending points the value is ``score``'s; with them (Monte Carlo kinds, z of shape (S, 1 + p)) it is
+        ``score_joint``'s value of [x; pending], candidate first."""
+        xd = self.prepare(x).to(torch.float32).contiguous()
+        zf = None
+        if acq.is_mc:
+            if z is None:
+                raise ValueError("Monte Carlo acquisition functions need base samples")
+            zf = z.to(self.device, torch.float32).contiguous()
+        if pending is None or len(pending) == 0:
+            return torch.ops.baybe_b200.acq_grad(xd, None, None, None, None, zf, self.handle, _lib.ACQ_KIND[acq.kind],
+                                                 acq.params())
+        px, beta, pmu, pcov = self.pending_stats(pending)
+        return torch.ops.baybe_b200.acq_grad(xd, px, beta, pmu, pcov, zf, self.handle, _lib.ACQ_KIND[acq.kind],
+                                             acq.params())
+
     def argmax(self, scores: torch.Tensor, keep: torch.Tensor | None, index_offset: int = 0) -> torch.Tensor:
         """Packed (score, lowest global index) key of a score vector (``bb_argmax``)."""
         return torch.ops.baybe_b200.argmax(scores, keep, int(index_offset))
@@ -592,6 +609,35 @@ def _op_acq_score_joint(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor
 @_op_acq_score_joint.register_fake
 def _(mu, var, cross, pend_mu, pend_cov, z, kind, params):
     return torch.empty_like(mu)
+
+
+@torch.library.custom_op("baybe_b200::acq_grad", mutates_args=())
+def _op_acq_grad(x: torch.Tensor, pend_x: torch.Tensor | None, pend_beta: torch.Tensor | None,
+                 pend_mu: torch.Tensor | None, pend_cov: torch.Tensor | None, z: torch.Tensor | None, handle: int,
+                 kind: int, params: list[float]) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_acq_grad``: raw fp32 rows x [N, d] -> value [N], gradient [N, d]; with p pending points their rows
+    pend_x [p, d] and ``pending_stats`` (beta [p, n_pad], mean [p], covariance [p, p]); z [S, 1 + p] (MC kinds)."""
+    gp = _gp(handle)
+    acq = AcqConfig.from_params(kind, params).to_c()
+    N = x.shape[0]
+    if x.dim() != 2 or x.shape[1] != gp.d or x.dtype != torch.float32 or not x.is_contiguous():
+        raise ValueError(f"rows must be a contiguous float32 (N, {gp.d}) tensor")
+    P = 0 if pend_x is None else pend_x.shape[0]
+    if z is not None and (z.dim() != 2 or z.shape[1] != P + 1):
+        raise ValueError(f"base samples must be (S, {P + 1})")
+    value = torch.empty(N, dtype=torch.float32, device=x.device)
+    grad = torch.empty((N, gp.d), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().bb_acq_grad(C.byref(gp.model), C.byref(acq), _ptr(x), N, P, _ptr(pend_x),
+                                           _ptr(pend_beta), _ptr(pend_mu), _ptr(pend_cov), _ptr(z),
+                                           0 if z is None else z.shape[0], _ptr(value), _ptr(grad), _stream_ptr()),
+                   "bb_acq_grad")
+    return value, grad
+
+
+@_op_acq_grad.register_fake
+def _(x, pend_x, pend_beta, pend_mu, pend_cov, z, handle, kind, params):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
 
 
 def _check_keep(keep: torch.Tensor | None, N: int) -> None:

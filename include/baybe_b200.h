@@ -528,6 +528,23 @@ int bb_nipv_score(const bb_model* m, const float* noise, float prior_var, const 
                   const float* d_cross_m, const float* d_linv, const uint8_t* d_keep, float* d_score,
                   int64_t* d_best_key, int64_t index_offset, void* d_ws, size_t ws_bytes, void* stream);
 
+/* ---- value and gradient of a single-target acquisition function at N points, for the continuous optimiser
+ * (L-BFGS-B over the continuous parameters: optimize_acqf's autograd pass, baybe/recommenders/pure/bayesian/botorch/
+ * continuous.py:184, and the same with the discrete features held fixed, botorch/hybrid.py:110).
+ *   m: a non-wide, single-task model with n_pad <= 256 (else BB_ERR_UNSUPPORTED).
+ *   a: one of the kinds BB_ACQ_QLOGEI .. BB_ACQ_PSTD.
+ *   d_x [N][d]: raw comp-rep rows, fp32 row-major.
+ *   n_pending in [0, BB_MAX_PENDING] (Monte Carlo kinds only): d_pend_x [n_pending][d] raw rows and what
+ *     bb_pending_stats returns for them: d_pend_beta [n_pending][n_pad], d_pend_mu [n_pending], d_pend_cov
+ *     [n_pending][n_pending].
+ *   d_z [S][1 + n_pending]: base samples (Monte Carlo kinds; S in [1, 1024]).
+ * Writes d_value [N], the value bb_score_fused reports (without pending points) or bb_acq_score_joint reports for
+ * [x; pending] (candidate first), and d_grad [N][d], its gradient with respect to the raw comp-rep coordinates (zero in
+ * columns with an inactive lengthscale).  Synchronises nothing; no float atomics: repeated calls are bit-identical. */
+int bb_acq_grad(const bb_model* m, const bb_acq_spec* a, const float* d_x, int64_t N, int32_t n_pending,
+                const float* d_pend_x, const float* d_pend_beta, const float* d_pend_mu, const float* d_pend_cov,
+                const float* d_z, int32_t S, float* d_value, float* d_grad, void* stream);
+
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
 int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
