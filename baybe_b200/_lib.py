@@ -164,6 +164,8 @@ _SIGNATURES = {
                                 _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
     "bb_acq_grad": (C.c_int, [C.POINTER(Model), C.POINTER(AcqSpec), _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32,
                               _vp, _vp, _vp]),
+    "bb_objective_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(Objective), _vp,
+                                    _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),

@@ -136,16 +136,12 @@ class AcquisitionFunction:
         return pd.Series(scores.double().cpu().numpy(), index=candidates.index)
 
     def scorer(self, surrogate, searchspace, objective, measurements):
-        """Objectives that are not affine in their targets (desirability, non-affine single targets): fit the
-        surrogate -- one model per target through a ``CompositeSurrogate`` for desirability -- and set up best_f
-        and the compiled objective (``baybe_b200.objectives``)."""
+        """Objectives that are not affine in their targets (desirability, non-affine single targets), on any search
+        space: fit the surrogate -- one model per target through a ``CompositeSurrogate`` for desirability -- and set
+        up best_f and the compiled objective (``baybe_b200.objectives``).  Continuous and hybrid spaces optimise it
+        with ``bb_objective_grad`` (``baybe_b200.continuous``)."""
         from baybe_b200.objectives import build_objective_scorer
 
-        kind = _space_kind(searchspace)
-        if kind != "DISCRETE":
-            raise IncompatibleAcquisitionFunctionError(
-                f"'{type(objective).__name__}' with a non-affine objective is served on discrete search spaces only "
-                f"by the B200 engine (got {kind})")
         surrogate.fit(searchspace, objective, measurements)
         flat = getattr(surrogate, "_surrogates_flat", None)
         gps = [s.device_gp for s in flat] if flat is not None else [surrogate.device_gp]

@@ -126,8 +126,9 @@ class EngineAcquisitionFunction:
 @define(kw_only=True)
 class B200BotorchRecommender(BayesianRecommender):
     """``BotorchRecommender`` with the scoring path on the B200 engine: discrete spaces, and continuous and hybrid
-    spaces with the single-target acquisition functions (gradient path, ``baybe_b200.continuous``) or qNEI (hybrid
-    spaces, search by scoring, ``baybe_b200.hybrid``)."""
+    spaces with the single-target acquisition functions, for single targets and for desirability and transformed
+    targets (gradient path, ``baybe_b200.continuous``), or qNEI (hybrid spaces, search by scoring,
+    ``baybe_b200.hybrid``)."""
 
     compatibility: ClassVar[SearchSpaceType] = SearchSpaceType.HYBRID
     supports_discrete_subset_generating_constraints: ClassVar[bool] = True
@@ -248,7 +249,7 @@ class B200BotorchRecommender(BayesianRecommender):
 
         assert self._objective is not None and self._context is not None
         cfg, _, pending = self._context
-        if cfg.kind != "qNEI" and (cfg.kind not in _lib.GRAD_KINDS or self._scorer is not None):
+        if cfg.kind != "qNEI" and (cfg.kind not in _lib.GRAD_KINDS or not self._gradient_scorer_ok()):
             raise IncompatibleAcquisitionFunctionError(
                 "hybrid search spaces are served with qNoisyExpectedImprovement or the single-target acquisition "
                 f"functions {_lib.GRAD_KINDS} on the B200 engine (got '{cfg.kind}')")
@@ -278,16 +279,24 @@ class B200BotorchRecommender(BayesianRecommender):
                                 index=rec_disc.index)
         return pd.concat([rec_disc, rec_cont], axis=1)
 
+    def _gradient_scorer_ok(self) -> bool:
+        """The gradient path serves the fused path's single targets and the ``ObjectiveScorer`` (desirability,
+        non-affine single targets); the other scorers (Pareto objectives, qNEI / qLogNEI, qNIPV) are not served."""
+        from baybe_b200.objectives import ObjectiveScorer
+
+        return self._scorer is None or isinstance(self._scorer, ObjectiveScorer)
+
     def _optimize_gradient(self, searchspace, disc_comp: np.ndarray, batch_size: int):
-        """Multi-start L-BFGS-B on ``bb_acq_grad`` over disc_comp x the continuous box (``baybe_b200.continuous``):
-        (points in comp-rep column order, configuration indices, joint value of [batch; pending])."""
+        """Multi-start L-BFGS-B on ``bb_acq_grad`` (``bb_objective_grad`` for objectives that are not affine in their
+        targets) over disc_comp x the continuous box (``baybe_b200.continuous``): (points in comp-rep column order,
+        configuration indices, joint value of [batch; pending])."""
         from baybe.parameters.numerical import _FixedNumericalContinuousParameter
 
         from baybe_b200.continuous import recommend_continuous_hybrid
 
         cfg, _, pending = self._context
         cont = searchspace.continuous
-        if cfg.kind not in _lib.GRAD_KINDS or self._scorer is not None:
+        if cfg.kind not in _lib.GRAD_KINDS or not self._gradient_scorer_ok():
             raise IncompatibleAcquisitionFunctionError(
                 f"continuous search spaces are served with the single-target acquisition functions {_lib.GRAD_KINDS} "
                 f"on the B200 engine (got '{cfg.kind}')")
@@ -305,8 +314,9 @@ class B200BotorchRecommender(BayesianRecommender):
         pend = None
         if pending is not None and len(pending) > 0:
             pend = searchspace.transform(pending, allow_extra=True).to_numpy(dtype=np.float64)
+        model = self._scorer if self._scorer is not None else self._surrogate_model.device_gp
         pts, idx, value = recommend_continuous_hybrid(
-            self._surrogate_model.device_gp, cfg, disc_comp, cont.comp_rep_bounds.to_numpy(dtype=np.float64),
+            model, cfg, disc_comp, cont.comp_rep_bounds.to_numpy(dtype=np.float64),
             batch_size, pend, self.n_mc_samples, _draw_sampler_seed(), self.n_raw_samples, self.n_restarts, fixed)
         self._last_acq_values[:] = [value]
         return pts, idx, value

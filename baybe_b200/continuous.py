@@ -18,6 +18,11 @@ serves both: a continuous space is a hybrid space with one empty discrete config
   * q > 1: sequential greedy (``optimize_acqf(sequential=True)``, ``optimize_acqf_mixed``): step j optimises the q = 1
     value given pending = [pending experiments; x_1 ... x_{j-1}].
 
+Objectives that are not affine in their targets (desirability, transformed single targets) come as a
+``baybe_b200.objectives.ObjectiveScorer`` in place of the model: raw and final values from its ``scores`` and
+``joint_value``, gradients from its ``value_and_grad`` (``bb_objective_grad``), base samples of M(1+p) columns from its
+``base_samples``.  Its pending-point conditioning is built once per greedy step and reused by every evaluation.
+
 Deliberate deviation for hybrid spaces: the reference runs a full multi-start optimisation for every discrete
 configuration (its own docstring calls that brute force).  Here the raw sweep ranks every configuration at once and the
 ``n_restarts`` best-placed starts are polished (DESIGN.md section 2).
@@ -74,9 +79,17 @@ def _scores(gp, cfg: AcqConfig, rows: np.ndarray, pending: np.ndarray | None, se
                        n_samples).double().cpu().numpy()
 
 
+def _is_scorer(gp) -> bool:
+    from baybe_b200.objectives import ObjectiveScorer
+
+    return isinstance(gp, ObjectiveScorer)
+
+
 def _polish(gp, cfg: AcqConfig, starts: np.ndarray, free: np.ndarray, lo: np.ndarray, hi: np.ndarray,
             pending: np.ndarray | None, z: torch.Tensor | None, stats: dict | None) -> np.ndarray:
-    """L-BFGS-B over the free columns of the stacked starts on -sum(value); returns the final rows."""
+    """L-BFGS-B over the free columns of the stacked starts on -sum(value); returns the final rows.  `gp`: a model
+    (``value_and_grad(cfg, x, z, pending)``) or an ``ObjectiveScorer`` (``value_and_grad(x, pending, z)``)."""
+    scorer = _is_scorer(gp)
     import time
 
     from scipy.optimize import minimize
@@ -88,7 +101,10 @@ def _polish(gp, cfg: AcqConfig, starts: np.ndarray, free: np.ndarray, lo: np.nda
         t0 = time.perf_counter()
         X = base.copy()
         X[:, free] = v.reshape(k, nf)
-        val, grad = gp.value_and_grad(cfg, torch.from_numpy(X.astype(np.float32)), z, pending)
+        if scorer:
+            val, grad = gp.value_and_grad(torch.from_numpy(X.astype(np.float32)), pending, z)
+        else:
+            val, grad = gp.value_and_grad(cfg, torch.from_numpy(X.astype(np.float32)), z, pending)
         val = np.nan_to_num(val.double().cpu().numpy(), nan=0.0)
         g = np.nan_to_num(grad.double().cpu().numpy()[:, free], nan=0.0)
         if stats is not None:
@@ -117,10 +133,12 @@ def recommend_continuous_hybrid(gp, cfg: AcqConfig, disc_comp: np.ndarray, cont_
 
     ``disc_comp``: (n_configs, d_disc) comp-rep rows of the discrete subspace, which comes first in the comp-rep (a
     continuous space: one row of width 0); ``cont_bounds``: (2, d_cont); ``fixed``: continuous column -> value of the
-    fixed parameters.  ``gp``: a ``DeviceGP`` (or a stand-in with ``value_and_grad``, ``score``, ``score_joint``)."""
+    fixed parameters.  ``gp``: a ``DeviceGP`` (or a stand-in with ``value_and_grad``, ``score``, ``score_joint``), or an
+    ``ObjectiveScorer`` (then ``cfg`` is its ``cfg``)."""
+    scorer = _is_scorer(gp)
     if cfg.kind not in _lib.GRAD_KINDS:
         raise NotImplementedError(f"the gradient path serves {_lib.GRAD_KINDS}, not {cfg.kind!r}")
-    if getattr(gp, "task_col", None) is not None:
+    if any(getattr(m, "task_col", None) is not None for m in (gp.gps if scorer else [gp])):
         raise NotImplementedError("the gradient path supports single-task models")
     disc = np.asarray(disc_comp, dtype=np.float64).reshape(len(disc_comp), -1)
     cb = np.asarray(cont_bounds, dtype=np.float64)
@@ -143,8 +161,12 @@ def recommend_continuous_hybrid(gp, cfg: AcqConfig, disc_comp: np.ndarray, cont_
     for step in range(batch_size):
         pend = np.vstack([pend0] + chosen)
         p = len(pend)
-        z = sobol_normal_samples(n_samples, 1 + p, seed) if cfg.is_mc else None
-        raw = _scores(gp, cfg, rows, pend if p else None, seed, n_samples)
+        if scorer:
+            z = gp.base_samples(n_samples, p, seed)
+            raw = gp.scores(rows, pend if p else None, seed, n_samples)
+        else:
+            z = sobol_normal_samples(n_samples, 1 + p, seed) if cfg.is_mc else None
+            raw = _scores(gp, cfg, rows, pend if p else None, seed, n_samples)
         start_idx = initial_starts(torch.from_numpy(raw), n_restarts, seed + 1 + step).numpy()
         starts = rows[start_idx]
         if len(free):
@@ -152,7 +174,10 @@ def recommend_continuous_hybrid(gp, cfg: AcqConfig, disc_comp: np.ndarray, cont_
             cand = np.vstack([polished, starts])
         else:
             cand = starts
-        val = _scores(gp, cfg, cand, pend if p else None, seed, n_samples)
+        if scorer:
+            val = gp.scores(cand, pend if p else None, seed, n_samples)
+        else:
+            val = _scores(gp, cfg, cand, pend if p else None, seed, n_samples)
         val = np.where(np.isfinite(val), val, -np.inf)
         best = int(np.argmax(val))
         row = cand[best].copy()
@@ -162,6 +187,8 @@ def recommend_continuous_hybrid(gp, cfg: AcqConfig, disc_comp: np.ndarray, cont_
         idx.append(k)
     batch = np.vstack(chosen)
     rest = np.vstack([batch[1:], pend0])
+    if scorer:
+        return batch, idx, gp.joint_value(batch, pend0 if len(pend0) else None, seed, n_samples)
     if len(rest):
         zj = sobol_normal_samples(n_samples, 1 + len(rest), seed)
         value = float(gp.score_joint(cfg, torch.from_numpy(batch[:1]), rest, zj)[0])

@@ -21,18 +21,13 @@
 //   dA/dA22 = sym(L22^-T Phi(L22^T dL22) L22^-1) / 2  (as torch's cholesky backward),  A22 = Sigma_PP - l l^T,
 // so only dA/dl = -2 (dA/dA22) l is needed: two triangular solves and one matrix-vector product per point.
 // Every reduction has a fixed order and nothing is accumulated atomically: repeated calls are bit-identical.
-#include <math.h>
-
-#include "acq_math.cuh"
-#include "common.cuh"
 #include "fused_common.cuh"
+#include "grad_common.cuh"
 
 namespace bb {
 
 constexpr int kGradThreads = 128;  // four points per block
 constexpr int kGradWarps = kGradThreads / 32;
-constexpr int kGradMaxNPad = 256;
-constexpr unsigned kFull = 0xffffffffu;
 
 struct GradParams {
   bb_acq_spec a;
@@ -53,79 +48,6 @@ struct GradParams {
 // per-warp scratch in floats: a | k (then dA/dk_i * dk_i/dt) | gk | v | 5 x 32 vectors | L22 | dL22 | 2 x sample chunk
 __host__ __device__ inline int grad_warp_floats(int n_pad, int d_pad, int P) {
   return (d_pad + 3 * n_pad + 5 * 32 + 2 * P * P + 2 * 32 * (P + 1) + 3) & ~3;
-}
-
-// kernel value k(t) and dk/dt of the scaled squared distance t (the family's constant is folded into the scale)
-template <int FAMILY>
-__device__ __forceinline__ void kernel_and_slope(float t, float& k, float& dkdt) {
-  t = fmaxf(t, 0.f);
-  if constexpr (FAMILY == BB_KERNEL_RBF) {
-    k = exp2f(-t);
-    dkdt = -kLn2 * k;
-  } else {
-    const float s = sqrtf(t), e = expf(-s);
-    if constexpr (FAMILY == BB_KERNEL_MATERN12) {
-      k = e;
-      dkdt = s > 0.f ? -0.5f * e / s : 0.f;  // kappa'(r)/r taken as 0 at r = 0
-    } else if constexpr (FAMILY == BB_KERNEL_MATERN32) {
-      k = (1.f + s) * e;
-      dkdt = -0.5f * e;
-    } else {
-      k = (1.f + s + t * (1.f / 3.f)) * e;
-      dkdt = -(1.f + s) * e * (1.f / 6.f);
-    }
-  }
-}
-
-__device__ __forceinline__ float warp_sum(float v) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
-
-__device__ __forceinline__ float sigmoidf_(float t) { return 1.f / (1.f + expf(-t)); }
-
-// sigmoid'(t) = e / (1 + e)^2, e = exp(-t): no cancellation in 1 - sigmoid(t) where sigmoid(t) is near 1
-__device__ __forceinline__ float dsigmoidf_(float t) {
-  const float e = expf(-t);
-  return isinf(e) ? 0.f : e / ((1.f + e) * (1.f + e));
-}
-
-// d/dt log(softplus(t) + 0.1 / (1 + t^2)) and the value inside the log
-__device__ __forceinline__ float dlog_fatplus_t(float t) {
-  const float q = 1.f / fmaf(t, t, 1.f);
-  const float sp = fmaxf(t, 0.f) + ((fabsf(t) < 30.f) ? log1pf(expf(-fabsf(t))) : 0.f);
-  return (sigmoidf_(t) - 0.2f * (t * q) * q) / (sp + 0.1f * q);
-}
-
-// partial derivatives (A_mu, A_sd) of the analytic kinds, float64
-__device__ __forceinline__ void analytic_partials(const bb_acq_spec& a, float mu, float var, double& dmu,
-                                                  double& dsd) {
-  const double a1 = (double)a.obj_scale, aa = fabs(a1);
-  const double m = a1 * (double)mu + (double)a.obj_shift;
-  const double s = aa * sqrt((double)var);
-  dmu = 0.0;
-  dsd = 0.0;
-  switch (a.kind) {
-    case BB_ACQ_PM: dmu = a1; return;
-    case BB_ACQ_PSTD: dsd = a.maximize ? aa : -aa; return;
-    case BB_ACQ_UCB: dmu = a1; dsd = sqrt((double)a.beta) * aa; return;
-    default: break;
-  }
-  const double u = (m - (double)a.best_f) / s;
-  if (a.kind == BB_ACQ_EI) {
-    dmu = a1 * norm_cdf(u);
-    dsd = aa * norm_pdf(u);
-  } else if (a.kind == BB_ACQ_LOGEI) {
-    // Phi(u) / h(u) = exp(log Phi(u) - log h(u)), h(u) = phi(u) + u Phi(u): never formed as a ratio
-    const double log_Phi = u > -1.0 ? log(norm_cdf(u))
-                                    : log(0.5 * erfcx(-u * 0.7071067811865476)) - 0.5 * u * u;
-    const double r = exp(log_Phi - log_ei_helper(u));
-    dmu = a1 * r / s;
-    dsd = aa * (1.0 - u * r) / s;
-  } else {  // PI
-    dmu = a1 * norm_pdf(u) / s;
-    dsd = -aa * u * norm_pdf(u) / s;
-  }
 }
 
 template <int FAMILY>
@@ -179,6 +101,8 @@ __global__ void __launch_bounds__(kGradThreads) k_acq_grad(const GradParams p) {
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t c = warp_global; c < p.N; c += nwarps) {
     // ---- forward: a, k, mu, v, var, cross ----
+    // (grad_common.cuh's kernel_row_warp, linv_apply_warp and linvt_apply_col are these passes; called from here
+    // they change this kernel's register allocation, so its SASS would no longer be the one measured)
     for (int j = lane; j < p.d_pad; j += 32)
       a_w[j] = j < p.d ? fmaf(__ldg(p.x + c * p.d + j), __ldg(p.cand_scale + j), __ldg(p.cand_shift + j)) : 0.f;
     __syncwarp();

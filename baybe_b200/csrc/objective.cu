@@ -15,6 +15,7 @@
 // S x M candidate base samples sit in shared memory.
 #include <math.h>
 
+#include "objective_common.cuh"
 #include "score_common.cuh"
 
 namespace bb {
@@ -200,31 +201,6 @@ __global__ void __launch_bounds__(kObjThreads) k_objective(const __grid_constant
   block_flush_best<kObjThreads>(best, p.key);
 }
 
-// Dry run of one program on the host: opcodes, op count and stack depth (BB_OBJ_MAX_STACK).
-static int check_program(const bb_objective* obj, int m) {
-  const int n = obj->n_ops[m];
-  BB_CHECK_SUPPORTED(n >= 0 && n <= BB_OBJ_MAX_OPS, "bb_objective_score: target %d has %d ops outside [0,%d]", m, n,
-                     BB_OBJ_MAX_OPS);
-  int depth = 1;
-  for (int i = 0; i < n; ++i) {
-    const bb_obj_instr& in = obj->prog[m][i];
-    BB_CHECK_ARG(in.op >= BB_OBJ_AFFINE && in.op <= BB_OBJ_MUL, "bb_objective_score: target %d op %d: unknown opcode %d",
-                 m, i, in.op);
-    if (in.op == BB_OBJ_DUP_INPUT) ++depth;
-    if (in.op == BB_OBJ_ADD || in.op == BB_OBJ_MUL) {
-      BB_CHECK_ARG(depth >= 2, "bb_objective_score: target %d op %d pops an empty stack", m, i);
-      --depth;
-    }
-    BB_CHECK_SUPPORTED(depth <= BB_OBJ_MAX_STACK, "bb_objective_score: target %d op %d: stack depth %d above %d", m, i,
-                       depth, BB_OBJ_MAX_STACK);
-    if (in.op == BB_OBJ_POW_INT)
-      BB_CHECK_SUPPORTED(in.arg[0] == rintf(in.arg[0]), "bb_objective_score: target %d op %d: non-integer power %g", m,
-                         i, (double)in.arg[0]);
-  }
-  BB_CHECK_ARG(depth == 1, "bb_objective_score: target %d leaves %d stack entries (need 1)", m, depth);
-  return BB_OK;
-}
-
 }  // namespace bb
 
 using namespace bb;
@@ -236,31 +212,10 @@ extern "C" int bb_objective_score(const bb_acq_spec* a, const bb_objective* obj,
                                   void* stream) {
   BB_CHECK_ARG(a != nullptr, "bb_objective_score: acquisition spec is null");
   BB_CHECK_ARG(obj != nullptr, "bb_objective_score: objective is null");
-  BB_CHECK_ARG(a->kind >= BB_ACQ_QLOGEI && a->kind <= BB_ACQ_PSTD,
-               "bb_objective_score: kind %d is not a single-objective acquisition function", a->kind);
-  const bool analytic = a->kind >= BB_ACQ_UCB;
-  BB_CHECK_ARG(!(a->kind == BB_ACQ_QLOGEI) || (a->tau_relu > 0.f && a->tau_max > 0.f),
-               "bb_objective_score: qLogEI needs tau_relu > 0 and tau_max > 0");
-  BB_CHECK_ARG(!(a->kind == BB_ACQ_QPI) || a->tau_pi > 0.f, "bb_objective_score: qPI needs tau_pi > 0");
   const int M = obj->n_targets;
-  BB_CHECK_SUPPORTED(M >= 1 && M <= BB_OBJ_MAX_TARGETS, "bb_objective_score: n_targets=%d outside [1,%d]", M,
-                     BB_OBJ_MAX_TARGETS);
-  BB_CHECK_ARG(obj->scalarizer >= BB_OBJ_SCALAR_NONE && obj->scalarizer <= BB_OBJ_SCALAR_GEOM_MEAN,
-               "bb_objective_score: unknown scalarizer %d", obj->scalarizer);
-  BB_CHECK_ARG((obj->scalarizer == BB_OBJ_SCALAR_NONE) == (M == 1),
-               "bb_objective_score: scalarizer NONE is for exactly one target (got %d targets)", M);
-  for (int m = 0; m < M; ++m) {
-    const int rc = check_program(obj, m);
-    if (rc != BB_OK) return rc;
-    BB_CHECK_ARG(isfinite(obj->weight[m]), "bb_objective_score: weight %d is not finite", m);
-  }
-  if (analytic) {
-    BB_CHECK_SUPPORTED(obj->scalarizer == BB_OBJ_SCALAR_MEAN,
-                       "bb_objective_score: analytic kinds need MEAN scalarisation (the posterior must stay Gaussian)");
-    for (int m = 0; m < M; ++m)
-      BB_CHECK_SUPPORTED(obj->n_ops[m] == 0 || (obj->n_ops[m] == 1 && obj->prog[m][0].op == BB_OBJ_AFFINE),
-                         "bb_objective_score: analytic kinds need affine targets (target %d is not)", m);
-  }
+  const int rc_obj = check_objective("bb_objective_score", a, obj);
+  if (rc_obj != BB_OK) return rc_obj;
+  const bool analytic = a->kind >= BB_ACQ_UCB;
   const int rc = check_score_args("bb_objective_score", "n_pending", N, index_offset, n_pending, S, !analytic,
                                   d_best_key);
   if (rc != BB_OK) return rc;

@@ -958,6 +958,50 @@ def _(mu, var, cross, linv, w, pend_terms, z, keep, kind, params, scalarizer, op
     return (mu.new_empty(mu.shape[1] if want_scores else 0, dtype=torch.float32), mu.new_empty(1, dtype=torch.int64))
 
 
+def _unflatten_programs(ops: list[int], args: list[float], n_ops: list[int]) -> list:
+    progs, k = [], 0
+    for n in n_ops:
+        progs.append([(ops[k + i], args[3 * (k + i): 3 * (k + i) + 3]) for i in range(n)])
+        k += n
+    return progs
+
+
+@torch.library.custom_op("baybe_b200::objective_grad", mutates_args=())
+def _op_objective_grad(x: torch.Tensor, handles: list[int], pend_x: torch.Tensor | None, betas: list[torch.Tensor],
+                       linv: torch.Tensor | None, w: torch.Tensor | None, pend_terms: torch.Tensor | None,
+                       z: torch.Tensor | None, kind: int, params: list[float], scalarizer: int, ops: list[int],
+                       args: list[float], n_ops: list[int], weights: list[float]) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_objective_grad``: raw fp32 rows x [N, d] of the models `handles` (one per target) -> value [N], gradient
+    [N, d].  With P pending points their rows pend_x [P, d], one beta [P, n_pad] per model (``pending_stats``), linv
+    [M, P, P], w [M, S, P] and pend_terms [S, P] (as ``objective_score``); z [S, M(1+P)] (None for analytic kinds)."""
+    gps = [_gp(h) for h in handles]
+    M, N = len(gps), x.shape[0]
+    if x.dim() != 2 or x.shape[1] != gps[0].d or x.dtype != torch.float32 or not x.is_contiguous():
+        raise ValueError(f"rows must be a contiguous float32 (N, {gps[0].d}) tensor")
+    P = 0 if pend_x is None else pend_x.shape[0]
+    if z is not None and (z.dim() != 2 or z.shape[1] != M * (1 + P)):
+        raise ValueError(f"base samples must be (S, {M * (1 + P)})")
+    if P and len(betas) != M:
+        raise ValueError(f"{P} pending points need one beta per model ({M})")
+    acq = AcqConfig.from_params(kind, params).to_c()
+    obj = objective_struct(M, scalarizer, _unflatten_programs(ops, args, n_ops), weights)
+    models = (C.POINTER(_lib.Model) * M)(*(C.pointer(gp.model) for gp in gps))
+    beta_ptrs = (C.c_void_p * M)(*((b.data_ptr() for b in betas) if P else [None] * M))
+    value = torch.empty(N, dtype=torch.float32, device=x.device)
+    grad = torch.empty((N, x.shape[1]), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().bb_objective_grad(models, M, C.byref(acq), C.byref(obj), _ptr(x), N, P, _ptr(pend_x),
+                                                 beta_ptrs if P else None, _ptr(linv), _ptr(w), _ptr(pend_terms),
+                                                 _ptr(z), 0 if z is None else z.shape[0], _ptr(value), _ptr(grad),
+                                                 _stream_ptr()), "bb_objective_grad")
+    return value, grad
+
+
+@_op_objective_grad.register_fake
+def _(x, handles, pend_x, betas, linv, w, pend_terms, z, kind, params, scalarizer, ops, args, n_ops, weights):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+
+
 @torch.library.custom_op("baybe_b200::argmax", mutates_args=())
 def _op_argmax(score: torch.Tensor, keep: torch.Tensor | None, index_offset: int) -> torch.Tensor:
     key = torch.empty(1, dtype=torch.int64, device=score.device)

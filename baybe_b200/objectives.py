@@ -33,6 +33,13 @@ def _objective_score(*args):
     return torch.ops.baybe_b200.objective_score(*args)
 
 
+def _objective_grad(*args):
+    """``baybe_b200::objective_grad`` (engine.py) on the models' handles; a module-level seam so that CPU tests can put
+    a float64 stand-in here (same arguments, with the models themselves in place of their handles)."""
+    gps, rest = args[0], args[1:]
+    return torch.ops.baybe_b200.objective_grad(rest[0], [gp.handle for gp in gps], *rest[1:])
+
+
 class CompiledObjective:
     """Per-target programs [(opcode name, (arg0, arg1, arg2)), ...] (model order), the scalarizer
     ("NONE" / "MEAN" / "GEOM_MEAN") and the normalised weights."""
@@ -288,6 +295,13 @@ def pending_conditioning(gps, pend: np.ndarray, z: torch.Tensor):
     return stats, linv, w, ys
 
 
+def _same(a, b) -> bool:
+    """Equal arrays or tensors (shape and every entry), or both None."""
+    if a is None or b is None:
+        return a is None and b is None
+    return tuple(a.shape) == tuple(b.shape) and bool((a == b).all())
+
+
 class ObjectiveScorer(Scorer):
     """MC (and, for MEAN desirability over affine targets, analytic) acquisition values of a compiled objective over
     one model per target.
@@ -302,30 +316,48 @@ class ObjectiveScorer(Scorer):
         self.kernel_comp = analytic if not cfg.is_mc else comp
         if self.kernel_comp is None:
             raise ValueError(f"{cfg.kind} needs the analytic (Gaussian) form of the objective")
+        self._cond = None  # (pending rows, base samples, conditioning) of the last step
+
+    def conditioning(self, pend: np.ndarray | None, z: torch.Tensor | None):
+        """What the pending points contribute to every evaluation of one greedy step, on the device: (P, per-model
+        (pending rows, beta), linv [M,P,P], w [M,S,P], pending terms [S,P], z [S, M(1+P)] fp32).  ``pending_conditioning``
+        runs host Cholesky factorisations, so the last result is kept and reused while the pending points and the base
+        samples stay the same (the raw sweep, every L-BFGS-B evaluation and the final scoring of a step)."""
+        M = self.M
+        P = 0 if pend is None else len(pend)
+        if z is not None:
+            z = torch.as_tensor(z, dtype=torch.float64).reshape(-1, M * (1 + P))
+        key = None if pend is None else np.asarray(pend, dtype=np.float64)
+        if self._cond is not None and _same(self._cond[0], key) and _same(self._cond[1], z):
+            return self._cond[2]
+        zd = None if z is None else z.to(self.device, torch.float32).contiguous()
+        if P == 0:
+            cond = (0, None, None, None, None, zd)
+        else:
+            stats, linv_h, w_h, ys = pending_conditioning(self.gps, np.asarray(pend, dtype=np.float64), z)
+            linv = torch.from_numpy(linv_h).to(self.device, torch.float32)
+            w = torch.from_numpy(w_h).to(self.device, torch.float32)
+            terms = torch.from_numpy(kind_terms(self.cfg, evaluate_objective(self.comp, ys))).to(
+                self.device, torch.float32).contiguous()
+            cond = (P, stats, linv, w, terms, zd)
+        self._cond = (key, None if z is None else z.clone(), cond)
+        return cond
 
     def values(self, x, pend: np.ndarray | None, z: torch.Tensor | None, keep=None, index_offset: int = 0,
                want_scores: bool = True):
         """(scores or None, packed best key, report) for every row of x; the kernel's value already is the value of
         the batch [x; pending], so `report` is the identity."""
-        M = self.M
         P = 0 if pend is None else len(pend)
         if P and not self.cfg.is_mc:
             raise ValueError(f"{self.cfg.kind} is analytic and takes no pending points")
         xd = self.gps[0].prepare(x)
-        cross = linv = w = terms = zd = None
-        if z is not None:
-            z = torch.as_tensor(z, dtype=torch.float64).reshape(-1, M * (1 + P))
-            zd = z.to(self.device, torch.float32).contiguous()
+        P, stats, linv, w, terms, zd = self.conditioning(pend if P else None, z)
+        cross = None
         if P == 0:
             post = [gp.posterior(xd) for gp in self.gps]
         else:
-            stats, linv_h, w_h, ys = pending_conditioning(self.gps, np.asarray(pend, dtype=np.float64), z)
             post = [gp.cross_covariance(xd, px, beta) for gp, (px, beta) in zip(self.gps, stats)]
             cross = torch.stack([c for _, _, c in post]).contiguous()
-            linv = torch.from_numpy(linv_h).to(self.device, torch.float32)
-            w = torch.from_numpy(w_h).to(self.device, torch.float32)
-            terms = torch.from_numpy(kind_terms(self.cfg, evaluate_objective(self.comp, ys))).to(
-                self.device, torch.float32).contiguous()
         mu = torch.stack([p[0] for p in post]).contiguous()
         var = torch.stack([p[1] for p in post]).contiguous()
         kc = self.kernel_comp
@@ -335,6 +367,25 @@ class ObjectiveScorer(Scorer):
             _lib.OBJ_SCALARIZER[kc.scalarizer], ops, args, n_ops, [float(v) for v in kc.weights], int(index_offset),
             bool(want_scores))
         return (scores if want_scores else None), key, (lambda v: v)
+
+    def value_and_grad(self, x, pend: np.ndarray | None, z: torch.Tensor | None):
+        """Acquisition value [N] and its gradient [N, d] with respect to the raw comp-rep rows x
+        (``bb_objective_grad``): the value ``values`` reports for [x; pending], with the base samples z of
+        ``base_samples`` (M(1+P) columns; None for analytic kinds)."""
+        P = 0 if pend is None else len(pend)
+        if P and not self.cfg.is_mc:
+            raise ValueError(f"{self.cfg.kind} is analytic and takes no pending points")
+        if self.cfg.is_mc and z is None:
+            raise ValueError("Monte Carlo acquisition functions need base samples")
+        xd = self.gps[0].prepare(x).to(torch.float32).contiguous()
+        P, stats, linv, w, terms, zd = self.conditioning(pend if P else None, z if self.cfg.is_mc else None)
+        px = stats[0][0] if P else None
+        betas = [beta for _, beta in stats] if P else []
+        kc = self.kernel_comp
+        ops, args, n_ops = kc.flat()
+        return _objective_grad(self.gps, xd, px, betas, linv, w, terms, zd, _lib.ACQ_KIND[self.cfg.kind],
+                               self.cfg.params(), _lib.OBJ_SCALARIZER[kc.scalarizer], ops, args, n_ops,
+                               [float(v) for v in kc.weights])
 
     def n_sample_columns(self, n_other: int) -> int | None:
         """M(1+P) (the layout of ``HviScorer``); None for analytic kinds."""

@@ -545,6 +545,28 @@ int bb_acq_grad(const bb_model* m, const bb_acq_spec* a, const float* d_x, int64
                 const float* d_pend_x, const float* d_pend_beta, const float* d_pend_mu, const float* d_pend_cov,
                 const float* d_z, int32_t S, float* d_value, float* d_grad, void* stream);
 
+/* ---- value and gradient of the acquisition value bb_objective_score reports (an objective that is not affine in its
+ * targets: desirability, transformed single targets) at N points, for the continuous optimiser.
+ *   models: host array of n_targets = M in [1, BB_OBJ_MAX_TARGETS] models, one per target in objective order; each
+ *     non-wide, single-task, n_pad <= 256 (else BB_ERR_UNSUPPORTED); they share d and the kernel family, and may
+ *     differ in n, scaling and hyper-parameters.
+ *   a, obj: as bb_objective_score (obj->n_targets = M; analytic kinds only for MEAN over affine targets and without
+ *     pending points).
+ *   d_x [N][d]: raw comp-rep rows, fp32 row-major.
+ *   n_pending = P in [0, BB_MAX_PENDING].  With P > 0: d_pend_x [P][d] raw rows; d_pend_beta: host array of M device
+ *     pointers, entry m the [P][n_pad_m] beta bb_pending_stats returns for model m; d_linv [M][P][P], d_w [M][S][P]
+ *     and d_pend_terms [S][P] as bb_objective_score takes them.
+ *   d_z [S][M(1+P)]: base samples as bb_objective_score (column m(1+P)+P the candidate's; Monte Carlo kinds, S in
+ *     [1, 1024]).
+ * The mean, variance and cross covariances of every target are formed from x (as bb_acq_grad).  Writes d_value [N],
+ * the value bb_objective_score reports, and d_grad [N][d], its gradient with respect to the raw comp-rep coordinates.
+ * Synchronises nothing; no float atomics: repeated calls are bit-identical. */
+int bb_objective_grad(const bb_model* const* models, int32_t n_targets, const bb_acq_spec* a, const bb_objective* obj,
+                      const float* d_x, int64_t N, int32_t n_pending, const float* d_pend_x,
+                      const float* const* d_pend_beta, const float* d_linv, const float* d_w,
+                      const float* d_pend_terms, const float* d_z, int32_t S, float* d_value, float* d_grad,
+                      void* stream);
+
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
 int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
