@@ -37,6 +37,10 @@ NEHVI_KINDS = ("qNEHVI",)
 # (bb_nipv_score); no base samples, but batches and joint values go through the conditioning set like the MC kinds
 NIPV_KINDS = ("qNIPV",)
 NIPV_MAX_TRAIN = 256
+# qNIPV's gradient path (bb_nipv_phi, bb_nipv_grad): the pair pass runs on a fixed number of CTAs, each writing one
+# partial sum per point, so the workspace depends on M only up to that count
+NIPV_GRAD_CTAS = 264
+NIPV_IMAGE_CAP = 4 << 30  # bytes of the integration points' image, (n + |C| + d) M fp32
 # single-target kinds with a gradient path (bb_acq_grad): continuous and hybrid spaces, baybe_b200/continuous.py
 GRAD_KINDS = ("qLogEI", "qEI", "qUCB", "qSR", "qPI", "UCB", "EI", "LogEI", "PI", "PM", "PSTD")
 GRAD_MAX_NPAD = 256
@@ -166,6 +170,9 @@ _SIGNATURES = {
                               _vp, _vp, _vp]),
     "bb_objective_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(Objective), _vp,
                                     _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "bb_nipv_phi": (C.c_int, [C.POINTER(Model), _vp, _i64, _i32, _vp, _vp, _vp, _vp]),
+    "bb_nipv_grad": (C.c_int, [C.POINTER(Model), C.POINTER(C.c_float), C.c_float, _vp, _i64, _vp, _i64, _i32, _vp, _vp,
+                               _vp, _vp, _vp, _vp, _sz, _vp]),
     "bb_decode_codes":(C.c_int, [_vp, _i32, _i64, _i32, _i64, _vp, _i32, _vp, _i64, _vp]),
     "bb_peer_slots_init": (C.c_int, [_vp, _vp, _vp]),
     "bb_allreduce_best": (C.c_int, [C.POINTER(PeerGroup), _vp, C.c_uint32, _vp, _vp, _vp]),
@@ -173,6 +180,11 @@ _SIGNATURES = {
     "bb_debug_set_trace": (C.c_int, [_vp, _i64]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
+
+
+def nipv_grad_ws_bytes(P: int, M: int, n: int, n_cond: int, d: int) -> int:
+    """Smallest workspace of ``bb_nipv_grad``: 4 P (n + n_cond + d + 1) (1 + min(ceil(M / 64), 264)) bytes."""
+    return 4 * P * (n + n_cond + d + 1) * (1 + min(-(-M // 64), NIPV_GRAD_CTAS))
 
 
 def load() -> C.CDLL:

@@ -429,11 +429,12 @@ def _positive_int_or_none(_, attr, value) -> None:
 
 @define(frozen=True)
 class qNegIntegratedPosteriorVariance(AcquisitionFunction):
-    """acquisition/acqfs.py:28-138: global active learning on discrete search spaces (``baybe_b200.nipv``): the
-    negative posterior variance averaged over integration points drawn from the whole discrete space, conditional on
-    noisy observations of the candidate, the pending points and the other points of a q-batch (``bb_nipv_score``).
-    Single targets without a transformation only; ``sampling_method``: "Random" (the plugin also takes BayBE's FPS
-    points through the BayBE spec's ``get_integration_points``)."""
+    """acquisition/acqfs.py:28-138: global active learning (``baybe_b200.nipv``): the negative posterior variance
+    averaged over integration points drawn from the whole search space, conditional on noisy observations of the
+    candidate, the pending points and the other points of a q-batch (``bb_nipv_score``; on continuous and hybrid
+    spaces optimised with ``bb_nipv_grad``).  Single targets without a transformation only; ``sampling_method``:
+    "Random" (the plugin also takes BayBE's FPS points through the BayBE spec's ``get_integration_points``, which also
+    samples the continuous part of continuous and hybrid spaces)."""
 
     abbreviation: ClassVar[str] = "qNIPV"
     sampling_n_points: int | None = field(default=None, validator=_positive_int_or_none)
@@ -478,7 +479,8 @@ class qNegIntegratedPosteriorVariance(AcquisitionFunction):
 
     def scorer(self, surrogate, searchspace, objective, measurements, integration=None):
         """Check the objective and the space, fit the surrogate and send the integration points (`integration`, or
-        ``get_integration_points``) to the device."""
+        ``get_integration_points`` on discrete spaces) to the device.  Continuous and hybrid spaces need
+        `integration`: the plugin passes the draw of BayBE's own ``get_integration_points``."""
         from baybe_b200.multiobjective import _error
         from baybe_b200.nipv import NipvScorer
 
@@ -488,9 +490,10 @@ class qNegIntegratedPosteriorVariance(AcquisitionFunction):
         if type(objective).__name__ == "DesirabilityObjective":
             raise _incompatibility(f"'{type(self).__name__}' currently supports single-target objectives only.")
         kind = _space_kind(searchspace)
-        if kind != "DISCRETE":
+        if kind != "DISCRETE" and integration is None:
             raise _error("IncompatibleAcquisitionFunctionError")(
-                f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
+                f"'{type(self).__name__}' on {kind} search spaces needs the integration points of BayBE's own spec "
+                "(its get_integration_points samples the continuous part), which the B200 recommender passes")
         targets = getattr(objective, "targets", None) or [getattr(objective, "_target", None)]
         tr = getattr(targets[0], "transformation", None)
         if tr is not None and type(tr).__name__ != "IdentityTransformation":

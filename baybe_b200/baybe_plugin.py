@@ -68,8 +68,16 @@ def mirror_acquisition_function(acqf) -> _acq.AcquisitionFunction:
 
 def _integration_points(acqf, spec, searchspace) -> dict:
     """qNIPV given as BayBE's spec: its own draw of the integration points, so that Random and FPS pick exactly the
-    rows BayBE picks (keyword arguments for the engine spec's ``scorer`` / ``evaluate``; empty otherwise)."""
+    rows BayBE picks (keyword arguments for the engine spec's ``scorer`` / ``evaluate``; empty otherwise).  A continuous
+    part with constraints would be sampled from its polytope; the gradient path rejects such spaces, so they are
+    rejected here before the draw."""
     if spec.abbreviation in _lib.NIPV_KINDS and hasattr(acqf, "get_integration_points"):
+        cont = getattr(searchspace, "continuous", None)
+        if cont is not None and not cont.is_empty and (
+                cont.has_interpoint_constraints or cont.constraints_lin_eq or cont.constraints_lin_ineq
+                or cont.n_subsets > 0):
+            raise IncompatibilityError("continuous constraints (linear, interpoint and cardinality) are not supported "
+                                       "by the B200 gradient path")
         return {"integration": acqf.get_integration_points(searchspace)}
     return {}
 
@@ -127,7 +135,7 @@ class EngineAcquisitionFunction:
 class B200BotorchRecommender(BayesianRecommender):
     """``BotorchRecommender`` with the scoring path on the B200 engine: discrete spaces, and continuous and hybrid
     spaces with the single-target acquisition functions, for single targets and for desirability and transformed
-    targets (gradient path, ``baybe_b200.continuous``), or qNEI (hybrid spaces, search by scoring,
+    targets, and with qNIPV (gradient path, ``baybe_b200.continuous``), or qNEI (hybrid spaces, search by scoring,
     ``baybe_b200.hybrid``)."""
 
     compatibility: ClassVar[SearchSpaceType] = SearchSpaceType.HYBRID
@@ -249,7 +257,8 @@ class B200BotorchRecommender(BayesianRecommender):
 
         assert self._objective is not None and self._context is not None
         cfg, _, pending = self._context
-        if cfg.kind != "qNEI" and (cfg.kind not in _lib.GRAD_KINDS or not self._gradient_scorer_ok()):
+        gradient_kinds = _lib.GRAD_KINDS + _lib.NIPV_KINDS
+        if cfg.kind != "qNEI" and (cfg.kind not in gradient_kinds or not self._gradient_scorer_ok()):
             raise IncompatibleAcquisitionFunctionError(
                 "hybrid search spaces are served with qNoisyExpectedImprovement or the single-target acquisition "
                 f"functions {_lib.GRAD_KINDS} on the B200 engine (got '{cfg.kind}')")
@@ -280,15 +289,17 @@ class B200BotorchRecommender(BayesianRecommender):
         return pd.concat([rec_disc, rec_cont], axis=1)
 
     def _gradient_scorer_ok(self) -> bool:
-        """The gradient path serves the fused path's single targets and the ``ObjectiveScorer`` (desirability,
-        non-affine single targets); the other scorers (Pareto objectives, qNEI / qLogNEI, qNIPV) are not served."""
+        """The gradient path serves the fused path's single targets, the ``ObjectiveScorer`` (desirability, non-affine
+        single targets) and the ``NipvScorer`` (qNIPV); the other scorers (Pareto objectives, qNEI / qLogNEI) are not
+        served."""
+        from baybe_b200.nipv import NipvScorer
         from baybe_b200.objectives import ObjectiveScorer
 
-        return self._scorer is None or isinstance(self._scorer, ObjectiveScorer)
+        return self._scorer is None or isinstance(self._scorer, (ObjectiveScorer, NipvScorer))
 
     def _optimize_gradient(self, searchspace, disc_comp: np.ndarray, batch_size: int):
         """Multi-start L-BFGS-B on ``bb_acq_grad`` (``bb_objective_grad`` for objectives that are not affine in their
-        targets) over disc_comp x the continuous box (``baybe_b200.continuous``): (points in comp-rep column order,
+        targets, ``bb_nipv_grad`` for qNIPV) over disc_comp x the continuous box (``baybe_b200.continuous``): (points in comp-rep column order,
         configuration indices, joint value of [batch; pending])."""
         from baybe.parameters.numerical import _FixedNumericalContinuousParameter
 
@@ -296,7 +307,7 @@ class B200BotorchRecommender(BayesianRecommender):
 
         cfg, _, pending = self._context
         cont = searchspace.continuous
-        if cfg.kind not in _lib.GRAD_KINDS or not self._gradient_scorer_ok():
+        if cfg.kind not in _lib.GRAD_KINDS + _lib.NIPV_KINDS or not self._gradient_scorer_ok():
             raise IncompatibleAcquisitionFunctionError(
                 f"continuous search spaces are served with the single-target acquisition functions {_lib.GRAD_KINDS} "
                 f"on the B200 engine (got '{cfg.kind}')")

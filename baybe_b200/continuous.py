@@ -22,6 +22,9 @@ Objectives that are not affine in their targets (desirability, transformed singl
 ``baybe_b200.objectives.ObjectiveScorer`` in place of the model: raw and final values from its ``scores`` and
 ``joint_value``, gradients from its ``value_and_grad`` (``bb_objective_grad``), base samples of M(1+p) columns from its
 ``base_samples``.  Its pending-point conditioning is built once per greedy step and reused by every evaluation.
+qNIPV comes the same way, as a ``baybe_b200.nipv.NipvScorer``: raw and final values from ``bb_nipv_score``, gradients
+from ``bb_nipv_grad`` over the integration points' image, which is built once per greedy step with the conditioning
+on [pending; earlier batch points].
 
 Deliberate deviation for hybrid spaces: the reference runs a full multi-start optimisation for every discrete
 configuration (its own docstring calls that brute force).  Here the raw sweep ranks every configuration at once and the
@@ -80,15 +83,25 @@ def _scores(gp, cfg: AcqConfig, rows: np.ndarray, pending: np.ndarray | None, se
 
 
 def _is_scorer(gp) -> bool:
+    """The scorers the gradient path serves in place of a model: ``ObjectiveScorer`` (desirability, transformed single
+    targets) and ``NipvScorer`` (qNIPV)."""
+    from baybe_b200.nipv import NipvScorer
     from baybe_b200.objectives import ObjectiveScorer
 
-    return isinstance(gp, ObjectiveScorer)
+    return isinstance(gp, (ObjectiveScorer, NipvScorer))
+
+
+def _models(gp, scorer: bool) -> list:
+    """The models behind `gp`: an ``ObjectiveScorer``'s one per target, a ``NipvScorer``'s one, or `gp` itself."""
+    if not scorer:
+        return [gp]
+    return list(gp.gps) if hasattr(gp, "gps") else [gp.gp]
 
 
 def _polish(gp, cfg: AcqConfig, starts: np.ndarray, free: np.ndarray, lo: np.ndarray, hi: np.ndarray,
             pending: np.ndarray | None, z: torch.Tensor | None, stats: dict | None) -> np.ndarray:
     """L-BFGS-B over the free columns of the stacked starts on -sum(value); returns the final rows.  `gp`: a model
-    (``value_and_grad(cfg, x, z, pending)``) or an ``ObjectiveScorer`` (``value_and_grad(x, pending, z)``)."""
+    (``value_and_grad(cfg, x, z, pending)``) or a scorer (``value_and_grad(x, pending, z)``)."""
     scorer = _is_scorer(gp)
     import time
 
@@ -134,11 +147,12 @@ def recommend_continuous_hybrid(gp, cfg: AcqConfig, disc_comp: np.ndarray, cont_
     ``disc_comp``: (n_configs, d_disc) comp-rep rows of the discrete subspace, which comes first in the comp-rep (a
     continuous space: one row of width 0); ``cont_bounds``: (2, d_cont); ``fixed``: continuous column -> value of the
     fixed parameters.  ``gp``: a ``DeviceGP`` (or a stand-in with ``value_and_grad``, ``score``, ``score_joint``), or an
-    ``ObjectiveScorer`` (then ``cfg`` is its ``cfg``)."""
+    ``ObjectiveScorer`` or ``NipvScorer`` (then ``cfg`` is its ``cfg``)."""
     scorer = _is_scorer(gp)
-    if cfg.kind not in _lib.GRAD_KINDS:
-        raise NotImplementedError(f"the gradient path serves {_lib.GRAD_KINDS}, not {cfg.kind!r}")
-    if any(getattr(m, "task_col", None) is not None for m in (gp.gps if scorer else [gp])):
+    kinds = _lib.GRAD_KINDS + (_lib.NIPV_KINDS if scorer else ())
+    if cfg.kind not in kinds:
+        raise NotImplementedError(f"the gradient path serves {kinds}, not {cfg.kind!r}")
+    if any(getattr(m, "task_col", None) is not None for m in _models(gp, scorer)):
         raise NotImplementedError("the gradient path supports single-task models")
     disc = np.asarray(disc_comp, dtype=np.float64).reshape(len(disc_comp), -1)
     cb = np.asarray(cont_bounds, dtype=np.float64)

@@ -860,6 +860,84 @@ def _(x, xm, var, cross_x, cross_m, linv, keep, handle, index_offset, want_score
     return (x.new_empty(x.shape[0] if want_scores else 0, dtype=torch.float32), x.new_empty(1, dtype=torch.int64))
 
 
+def nipv_image_numel(gp: DeviceGP, M: int, n_cond: int) -> int:
+    """Floats of ``bb_nipv_phi``'s image, (n + n_cond + d) M; raises ``NotImplementedError`` above
+    ``_lib.NIPV_IMAGE_CAP`` bytes."""
+    numel = (gp.n + n_cond + gp.d) * M
+    if 4 * numel > _lib.NIPV_IMAGE_CAP:
+        raise NotImplementedError(
+            f"qNIPV's gradient path keeps an image of (n + |C| + d) x M = {gp.n + n_cond + gp.d} x {M} fp32 values on "
+            f"the device, above its cap of {_lib.NIPV_IMAGE_CAP >> 30} GiB: use fewer integration points")
+    return numel
+
+
+@torch.library.custom_op("baybe_b200::nipv_phi", mutates_args=())
+def _op_nipv_phi(xm: torch.Tensor, cross_m: torch.Tensor | None, linv: torch.Tensor | None,
+                 handle: int) -> torch.Tensor:
+    """``bb_nipv_phi``: integration points xm [M, d] (raw fp32 rows); with |C| conditioning points cross_m [M, |C|] and
+    linv [|C|, |C|] as ``nipv_score``.  Returns the image [(n + |C| + d) * M] fp32."""
+    gp = _gp(handle)
+    M = xm.shape[0]
+    if xm.dim() != 2 or xm.shape[1] != gp.d or xm.dtype != torch.float32 or not xm.is_contiguous():
+        raise ValueError(f"xm must be a contiguous float32 ({M}, {gp.d}) tensor")
+    Cn = 0 if cross_m is None else cross_m.shape[1]
+    if Cn and (tuple(cross_m.shape) != (M, Cn) or linv is None or tuple(linv.shape) != (Cn, Cn)):
+        raise ValueError(f"conditioning needs cross_m ({M}, {Cn}) and linv ({Cn}, {Cn})")
+    f32 = lambda t: None if t is None else t.to(torch.float32).contiguous()  # noqa: E731
+    cross_m, linv = f32(cross_m), f32(linv)
+    img = torch.empty(nipv_image_numel(gp, M, Cn), dtype=torch.float32, device=xm.device)
+    with torch.cuda.device(xm.device):
+        _lib.check(_lib.load().bb_nipv_phi(C.byref(gp.model), _ptr(xm), M, Cn, _ptr(cross_m), _ptr(linv), _ptr(img),
+                                           _stream_ptr()), "bb_nipv_phi")
+    return img
+
+
+@_op_nipv_phi.register_fake
+def _(xm, cross_m, linv, handle):
+    gp = _gp(handle)
+    Cn = 0 if cross_m is None else cross_m.shape[1]
+    return xm.new_empty((gp.n + Cn + gp.d) * xm.shape[0])
+
+
+@torch.library.custom_op("baybe_b200::nipv_grad", mutates_args=())
+def _op_nipv_grad(x: torch.Tensor, img: torch.Tensor, M: int, cond_x: torch.Tensor | None,
+                  cond_beta: torch.Tensor | None, linv: torch.Tensor | None,
+                  handle: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_nipv_grad``: points x [P, d] (raw fp32 rows), ``nipv_phi``'s image of M integration points; with |C|
+    conditioning points their raw rows cond_x [|C|, d], beta [|C|, n_pad] (``bb_joint_posterior``) and linv
+    [|C|, |C|].  Returns IVR [P] (original units, as ``nipv_score``) and its gradient [P, d]."""
+    gp = _gp(handle)
+    P = x.shape[0]
+    if x.dim() != 2 or x.shape[1] != gp.d or x.dtype != torch.float32 or not x.is_contiguous():
+        raise ValueError(f"x must be a contiguous float32 ({P}, {gp.d}) tensor")
+    Cn = 0 if cond_x is None else cond_x.shape[0]
+    if img.numel() != (gp.n + Cn + gp.d) * M:
+        raise ValueError(f"the image must hold (n + |C| + d) * M = {(gp.n + Cn + gp.d) * M} values")
+    if Cn and (tuple(cond_x.shape) != (Cn, gp.d) or cond_beta is None or cond_beta.shape[0] != Cn
+               or linv is None or tuple(linv.shape) != (Cn, Cn)):
+        raise ValueError(f"conditioning needs cond_x ({Cn}, {gp.d}), beta ({Cn}, n_pad) and linv ({Cn}, {Cn})")
+    f32 = lambda t: None if t is None else t.to(torch.float32).contiguous()  # noqa: E731
+    cond_x, cond_beta, linv = f32(cond_x), f32(cond_beta), f32(linv)
+    noise, prior_var = nipv_model_terms(gp)
+    value = torch.empty(P, dtype=torch.float32, device=x.device)
+    grad = torch.empty((P, gp.d), dtype=torch.float32, device=x.device)
+    if P == 0:
+        return value, grad
+    ws_bytes = _lib.nipv_grad_ws_bytes(P, M, gp.n, Cn, gp.d)
+    with torch.cuda.device(x.device):
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=x.device)
+        _lib.check(_lib.load().bb_nipv_grad(C.byref(gp.model), (C.c_float * len(noise))(*noise), prior_var, _ptr(x),
+                                            P, _ptr(img), M, Cn, _ptr(cond_x), _ptr(cond_beta), _ptr(linv),
+                                            _ptr(value), _ptr(grad), _ptr(ws), ws_bytes, _stream_ptr()),
+                   "bb_nipv_grad")
+    return value, grad
+
+
+@_op_nipv_grad.register_fake
+def _(x, img, M, cond_x, cond_beta, linv, handle):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+
+
 @torch.library.custom_op("baybe_b200::parego_score", mutates_args=())
 def _op_parego_score(mu: torch.Tensor, var: torch.Tensor, cross: torch.Tensor | None, linv: torch.Tensor | None,
                      w: torch.Tensor | None, z: torch.Tensor, g: torch.Tensor, batch_terms: torch.Tensor | None,

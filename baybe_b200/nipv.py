@@ -11,6 +11,12 @@ variance does not depend on the fantasised values, so no samples are involved.  
 (``bb_joint_posterior``, plus the noise, then the Cholesky factor), runs ``bb_posterior`` with C as its pending points
 for the candidates and the integration points, and sums k_C(m,m) in float64; ``bb_nipv_score`` (csrc/nipv.cu) ranks
 the candidates by IVR.
+
+On continuous and hybrid spaces (``baybe_b200.continuous``) ``value_and_grad`` gives qNIPV and its gradient with respect
+to the raw rows: ``bb_nipv_phi`` builds the integration points' image phi(m) once per conditioning set and
+``bb_nipv_grad`` (csrc/nipvgrad.cu) streams it for every evaluation.  The scorer keeps the last conditioning it built
+(C rows, L_C^-1, beta_C, the integration points' cross covariances and sum_m k_C(m,m), and the image), so a greedy step
+builds it once: the raw sweep, every L-BFGS-B evaluation and the final scoring reuse it.
 """
 from __future__ import annotations
 
@@ -30,6 +36,16 @@ __all__ = ["NipvScorer", "sample_integration_points"]
 def _nipv_score(*args):
     """``baybe_b200::nipv_score`` (engine.py); a module-level seam so that CPU tests can put a float64 stand-in here."""
     return torch.ops.baybe_b200.nipv_score(*args)
+
+
+def _nipv_phi(*args):
+    """``baybe_b200::nipv_phi`` (engine.py); a module-level seam so that CPU tests can put a float64 stand-in here."""
+    return torch.ops.baybe_b200.nipv_phi(*args)
+
+
+def _nipv_grad(*args):
+    """``baybe_b200::nipv_grad`` (engine.py); a module-level seam so that CPU tests can put a float64 stand-in here."""
+    return torch.ops.baybe_b200.nipv_grad(*args)
 
 
 def sample_integration_points(comp_rep, n_points: int | None, fraction: float | None, method: str = "Random"):
@@ -77,6 +93,7 @@ class NipvScorer(Scorer):
         noise, _ = nipv_model_terms(gp)
         self.noise = np.asarray(noise, dtype=np.float64)
         self.y_var = float(gp.model.y_std) ** 2
+        self._cond = None  # (C rows, _Conditioned) of the last conditioning set
 
     def n_sample_columns(self, n_other: int) -> None:
         return None
@@ -96,27 +113,70 @@ class NipvScorer(Scorer):
         K = 0.5 * (cov + cov.T) + np.diag(self.noise[_tasks(rows, self.gp)] * self.y_var)
         return rows, np.linalg.inv(np.linalg.cholesky(K)), cond
 
+    def conditioned(self, pend: np.ndarray | None, batch: np.ndarray | None) -> "_Conditioned":
+        """What C = [pending; batch] contributes to every evaluation, kept while C stays the same: ``conditioning``,
+        the integration points' cross covariances with C and sum_m k_C(m,m); the image of ``value_and_grad`` is added
+        on its first use."""
+        d = self.gp.d
+        parts = [np.asarray(p, dtype=np.float64).reshape(-1, d) for p in (pend, batch) if p is not None]
+        key = np.concatenate(parts) if parts else np.zeros((0, d))
+        if self._cond is not None and self._cond[0].shape == key.shape and bool((self._cond[0] == key).all()):
+            return self._cond[1]
+        rows, linv, cond = self.conditioning(pend, batch)
+        gp = self.gp
+        if linv is None:
+            _, var_m = gp.posterior(self.xm)
+            cross_m = linv_d = None
+            kc_mm = float(var_m.double().sum())
+        else:
+            px, beta = cond
+            _, var_m, cross_m = gp.cross_covariance(self.xm, px, beta)
+            linv_d = torch.from_numpy(linv).to(self.device)
+            kc_mm = float((var_m.double() - ((cross_m.double() @ linv_d.T) ** 2).sum(1)).sum())
+        c = _Conditioned(rows, cond, linv_d, cross_m, kc_mm)
+        self._cond = (key, c)
+        return c
+
+    def _rows(self, x) -> torch.Tensor:
+        xd = self.gp.prepare(x)
+        if xd.dtype != torch.float32 or not xd.is_contiguous() or xd.stride(-1) != 1:
+            xd = xd.to(torch.float32).contiguous()
+        return xd
+
     def values(self, x, pend: np.ndarray | None, z=None, keep=None, index_offset: int = 0,
                want_scores: bool = True, batch: np.ndarray | None = None):
         """(IVR scores or None, packed best key, report) for every row of x given the pending points and the other
         points of a q-batch; `report` maps IVR to qNIPV (original units)."""
-        rows, linv, cond = self.conditioning(pend, batch)
-        gp, dev = self.gp, self.device
-        xd = gp.prepare(x)
-        if xd.dtype != torch.float32 or not xd.is_contiguous() or xd.stride(-1) != 1:
-            xd = xd.to(torch.float32).contiguous()
-        if linv is None:
+        c = self.conditioned(pend, batch)
+        gp = self.gp
+        xd = self._rows(x)
+        if c.linv is None:
             _, var = gp.posterior(xd)
-            _, var_m = gp.posterior(self.xm)
-            cross = cross_m = linv_d = None
-            kc_mm = float(var_m.double().sum())
+            cross = None
         else:
-            px, beta = cond
-            _, var, cross = gp.cross_covariance(xd, px, beta)
-            _, var_m, cross_m = gp.cross_covariance(self.xm, px, beta)
-            linv_d = torch.from_numpy(linv).to(dev)
-            kc_mm = float((var_m.double() - ((cross_m.double() @ linv_d.T) ** 2).sum(1)).sum())
-        scores, key = _nipv_score(xd, self.xm, var, cross, cross_m, linv_d, keep, gp.handle,
+            _, var, cross = gp.cross_covariance(xd, *c.cond)
+        scores, key = _nipv_score(xd, self.xm, var, cross, c.cross_m, c.linv, keep, gp.handle,
                                   int(index_offset), bool(want_scores))
-        M = self.M
+        M, kc_mm = self.M, c.kc_mm
         return (scores if want_scores else None), key, (lambda v: (np.asarray(v, dtype=np.float64) - kc_mm) / M)
+
+    def value_and_grad(self, x, pend: np.ndarray | None, z=None):
+        """qNIPV(x | pending) [N] and its gradient [N, d] with respect to the raw comp-rep rows x, float64 tensors
+        (``bb_nipv_grad``); `z` is ignored (qNIPV draws no samples).  The value is the one ``scores`` reports."""
+        c = self.conditioned(pend, None)
+        gp = self.gp
+        if c.image is None:
+            c.image = _nipv_phi(self.xm, c.cross_m, c.linv, gp.handle)
+        cond_x, beta = c.cond if c.linv is not None else (None, None)
+        ivr, grad = _nipv_grad(self._rows(x), c.image, self.M, cond_x, beta, c.linv, gp.handle)
+        return (ivr.double() - c.kc_mm) / self.M, grad.double() / self.M
+
+
+class _Conditioned:
+    """One conditioning set of a ``NipvScorer``: its rows, the (rows, beta) pair of ``cross_covariance``, L_C^-1 on the
+    device (None for an empty set), the integration points' cross covariances with it, sum_m k_C(m,m) (original
+    units) and, once built, the image of ``bb_nipv_phi``."""
+
+    def __init__(self, rows, cond, linv, cross_m, kc_mm: float):
+        self.rows, self.cond, self.linv, self.cross_m, self.kc_mm = rows, cond, linv, cross_m, kc_mm
+        self.image = None

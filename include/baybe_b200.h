@@ -528,6 +528,34 @@ int bb_nipv_score(const bb_model* m, const float* noise, float prior_var, const 
                   const float* d_cross_m, const float* d_linv, const uint8_t* d_keep, float* d_score,
                   int64_t* d_best_key, int64_t index_offset, void* d_ws, size_t ws_bytes, void* stream);
 
+/* ---- qNIPV on continuous and hybrid spaces (set-up on the host by baybe_b200/nipv.py): the integration points'
+ * image, built once per conditioning set.  In the notation of bb_nipv_score, standardised units,
+ *   phi(a) = [ L^-1 k(X,a) ; L_C^-1 k_D(C,a) ]   (r = n + n_cond entries).
+ *   m: a non-wide, single-task model with n <= 256 training points (else BB_ERR_UNSUPPORTED).
+ *   d_xm [M][d]: raw comp-rep rows of the integration points, fp32 row-major (M in [1, 2^31)).
+ *   n_cond in [0, BB_MAX_PENDING].  With n_cond > 0: d_cross_m [M][n_cond] and d_linv [n_cond][n_cond] as
+ *     bb_nipv_score takes them.
+ * Writes d_img [(r + d) M] fp32: phi dimension-major ([r][M], entry j of point m at j M + m), then the scaled
+ * coordinates x * scale + shift ([d][M]).  Synchronises nothing. */
+int bb_nipv_phi(const bb_model* m, const float* d_xm, int64_t M, int32_t n_cond, const float* d_cross_m,
+                const float* d_linv, float* d_img, void* stream);
+
+/* ---- value and gradient of qNIPV's integrated variance reduction at P points, for the continuous optimiser.
+ *   m, noise, prior_var: as bb_nipv_score (single-task: noise[0] and prior_var = s_f^2).
+ *   d_x [P][d]: raw comp-rep rows, fp32 row-major (P in [1, 2^31)).
+ *   d_img: bb_nipv_phi's image of the M integration points for the same model and conditioning set.
+ *   n_cond in [0, BB_MAX_PENDING].  With n_cond > 0: d_cond_x [n_cond][d] the raw rows of C, d_cond_beta
+ *     [n_cond][n_pad] the beta bb_joint_posterior returns for C, d_linv [n_cond][n_cond] = L_C^-1 as bb_nipv_score.
+ *   d_ws: caller-owned workspace of ws_bytes >= 4 P (r + d + 1) (1 + min(ceil(M / 64), 264)) bytes, r = n + n_cond
+ *     (else BB_ERR_INVALID).
+ * Writes d_value [P], IVR(x) in original units as bb_nipv_score reports it (qNIPV(x | C) = -(1/M) [sum_m k_C(m,m) -
+ * IVR(x)]), and d_grad [P][d], its gradient with respect to the raw comp-rep coordinates (zero in columns with an
+ * inactive lengthscale).  Every argument is checked before any CUDA call.  Synchronises nothing; no float atomics:
+ * repeated calls are bit-identical. */
+int bb_nipv_grad(const bb_model* m, const float* noise, float prior_var, const float* d_x, int64_t P,
+                 const float* d_img, int64_t M, int32_t n_cond, const float* d_cond_x, const float* d_cond_beta,
+                 const float* d_linv, float* d_value, float* d_grad, void* d_ws, size_t ws_bytes, void* stream);
+
 /* ---- value and gradient of a single-target acquisition function at N points, for the continuous optimiser
  * (L-BFGS-B over the continuous parameters: optimize_acqf's autograd pass, baybe/recommenders/pure/bayesian/botorch/
  * continuous.py:184, and the same with the discrete features held fixed, botorch/hybrid.py:110).
