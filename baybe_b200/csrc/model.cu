@@ -486,8 +486,9 @@ __global__ void k_pending_w(const float* __restrict__ pend_x, int P, int n, int 
     if (tid < s) red[tid] += red[tid + s];
     __syncthreads();
   }
-  if (tid == 0 && mu_out) mu_out[p] = y_mean + y_std * (float)((double)mean_const[tp] + red[0]);
-  if (tid == 0 && mu64_out) mu64_out[p] = (double)y_mean + (double)y_std * ((double)mean_const[tp] + red[0]);
+  const double mu64 = (double)y_mean + (double)y_std * ((double)mean_const[tp] + red[0]);
+  if (tid == 0 && mu_out) mu_out[p] = (float)mu64;
+  if (tid == 0 && mu64_out) mu64_out[p] = mu64;
   for (int j = tid; j < n; j += blockDim.x) {
     double s = 0.0;
     for (int i = 0; i <= j; ++i) s += Linv[(size_t)j * n + i] * kx[i];
@@ -523,6 +524,30 @@ __global__ void k_pending_cov(const double* __restrict__ pn, const double* __res
   const double c = (k - s) * (double)y_std * (double)y_std;
   if (cov) cov[p * P + q] = (float)c;
   if (cov64) cov64[(size_t)p * P + q] = c;
+}
+
+// k_pending_w keeps the normalised row, k(X, x) and L^-1 k(X, x) in dynamic shared memory: 8 (d + 2n) bytes, beside
+// its 2 KB of static shared memory.  Past the default 48 KB (d + 2n > 5888, e.g. 4096-bit fingerprints at n = 1024)
+// the launch needs the opt-in carve-out; shapes beyond even that are refused.
+static int launch_pending_w(const bb_model* m, const char* who, const float* d_x, int R, const uint8_t* B,
+                            const BlobLayout& L, float* beta_out, float* mu_out, double* mu64_out, double* pn,
+                            double* w64, cudaStream_t stream) {
+  const size_t shm = sizeof(double) * ((size_t)m->d + 2 * (size_t)m->n);
+  const size_t static_shm = sizeof(double) * 256;  // red[256]
+  int sms = 0, max_smem = 0;
+  const int rc = device_limits(&sms, &max_smem);
+  if (rc != BB_OK) return rc;
+  BB_CHECK_SUPPORTED(shm + static_shm <= (size_t)max_smem,
+                     "%s: d=%d features and n=%d training points need %zu bytes of shared memory, above the "
+                     "device's %d",
+                     who, m->d, m->n, shm + static_shm, max_smem);
+  BB_SMEM_OPTIN_ONCE(k_pending_w);
+  k_pending_w<<<R, 256, shm, stream>>>(d_x, R, m->n, m->n_pad, m->d, m->n_tasks, m->family, m->task_col, m->d_xn64,
+                                       m->d_train_task, (const double*)(B + L.tcov64), (const float*)(B + L.cnorm),
+                                       m->d_linv, m->d_alpha64, m->d_mean_const, m->y_mean, m->y_std, beta_out,
+                                       mu_out, mu64_out, pn, w64);
+  BB_LAUNCH_CHECK();
+  return BB_OK;
 }
 
 }  // namespace bb
@@ -883,13 +908,9 @@ extern "C" int bb_pending_stats(const bb_model* m, const float* d_pend_x, int32_
   uint8_t* B = (uint8_t*)m->d_blob;
   double* pn = (double*)(B + L.pend_norm);  // normalised pending rows (scratch inside the blob)
   double* w64 = (double*)(B + L.pend_w64);
-  size_t shm = sizeof(double) * (m->d + 2 * m->n);
-  k_pending_w<<<P, 256, shm, stream>>>(d_pend_x, P, m->n, m->n_pad, m->d, m->n_tasks, m->family,
-                                       m->task_col, m->d_xn64, m->d_train_task,
-                                       (const double*)(B + L.tcov64), (const float*)(B + L.cnorm),
-                                       m->d_linv, m->d_alpha64, m->d_mean_const, m->y_mean,
-                                       m->y_std, d_pend_beta, d_pend_mu, nullptr, pn, w64);
-  BB_LAUNCH_CHECK();
+  const int rc = launch_pending_w(m, "bb_pending_stats", d_pend_x, P, B, L, d_pend_beta, d_pend_mu, nullptr, pn, w64,
+                                  stream);
+  if (rc != BB_OK) return rc;
   k_pending_cov<<<P, 32, 0, stream>>>(pn, w64, P, m->n, m->d, m->n_tasks, m->family, m->task_col,
                                       (const double*)(B + L.tcov64), m->y_std, d_pend_cov, nullptr);
   BB_LAUNCH_CHECK();
@@ -912,12 +933,8 @@ extern "C" int bb_joint_posterior(const bb_model* m, const float* d_x, int32_t R
   uint8_t* B = (uint8_t*)m->d_blob;
   double* w64 = d_ws;                           // [R][n] L^-1 k(X, x_r)
   double* pn = d_ws + (size_t)R * m->n_pad;     // [R][d] normalised rows
-  size_t shm = sizeof(double) * (m->d + 2 * m->n);
-  k_pending_w<<<R, 256, shm, stream>>>(d_x, R, m->n, m->n_pad, m->d, m->n_tasks, m->family, m->task_col, m->d_xn64,
-                                       m->d_train_task, (const double*)(B + L.tcov64), (const float*)(B + L.cnorm),
-                                       m->d_linv, m->d_alpha64, m->d_mean_const, m->y_mean, m->y_std, d_beta,
-                                       nullptr, d_mu, pn, w64);
-  BB_LAUNCH_CHECK();
+  const int rc = launch_pending_w(m, "bb_joint_posterior", d_x, R, B, L, d_beta, nullptr, d_mu, pn, w64, stream);
+  if (rc != BB_OK) return rc;
   k_pending_cov<<<dim3(R, (R + 31) / 32), 32, 0, stream>>>(pn, w64, R, m->n, m->d, m->n_tasks, m->family, m->task_col,
                                                           (const double*)(B + L.tcov64), m->y_std, nullptr, d_cov);
   BB_LAUNCH_CHECK();
