@@ -170,6 +170,9 @@ _SIGNATURES = {
                               _vp, _vp, _vp]),
     "bb_objective_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(Objective), _vp,
                                     _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "bb_hvi_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(C.c_float),
+                              C.POINTER(C.c_float), _vp, _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _i32, _vp, _vp,
+                              _vp, _i32, _vp, _vp, _vp]),
     "bb_nipv_phi": (C.c_int, [C.POINTER(Model), _vp, _i64, _i32, _vp, _vp, _vp, _vp]),
     "bb_nipv_grad": (C.c_int, [C.POINTER(Model), C.POINTER(C.c_float), C.c_float, _vp, _i64, _vp, _i64, _i32, _vp, _vp,
                                _vp, _vp, _vp, _vp, _sz, _vp]),

@@ -310,16 +310,16 @@ class _ScoredAcquisitionFunction(AcquisitionFunction):
         scorer = self.scorer(surrogate, searchspace, objective, measurements)
         return _evaluate_with_scorer(self, scorer, candidates, searchspace, pending_experiments, jointly)
 
-    def _check_pareto(self, objective, searchspace, max_targets: int | None = None) -> None:
-        """A multi-output objective on a discrete space and, with `max_targets`, 2 to `max_targets` affine targets
-        (checked before the surrogate fit)."""
+    def _check_pareto(self, objective, searchspace, max_targets: int | None = None, discrete_only: bool = True) -> None:
+        """A multi-output objective on a discrete space (any space type without `discrete_only`) and, with
+        `max_targets`, 2 to `max_targets` affine targets (checked before the surrogate fit)."""
         from baybe_b200.multiobjective import _error, target_orientations
 
         if not getattr(objective, "is_multi_output", False):
             raise _error("IncompatibleAcquisitionFunctionError")(
                 f"'{type(self).__name__}' needs a multi-output (Pareto) objective")
         kind = _space_kind(searchspace)
-        if kind != "DISCRETE":
+        if discrete_only and kind != "DISCRETE":
             raise _error("IncompatibleAcquisitionFunctionError")(
                 f"'{type(self).__name__}' is served on discrete search spaces only by the B200 engine (got {kind})")
         if max_targets is None:
@@ -334,8 +334,9 @@ class _ScoredAcquisitionFunction(AcquisitionFunction):
 @define(frozen=True)
 class _ExpectedHypervolumeImprovement(_ScoredAcquisitionFunction):
     """acquisition/acqfs.py:342-418: Pareto objectives of 2 to 4 targets, scored by ``bb_hvi_score``
-    (``baybe_b200.multiobjective``).  ``reference_point``: None (default factor 0.1), a factor, or coordinates in
-    the oriented objective space; ``alpha``: None or 0.0 (exact partitioning)."""
+    (``baybe_b200.multiobjective``; on continuous and hybrid spaces optimised with ``bb_hvi_grad``).
+    ``reference_point``: None (default factor 0.1), a factor, or coordinates in the oriented objective space;
+    ``alpha``: None or 0.0 (exact partitioning)."""
 
     _scorer_module: ClassVar[str] = "baybe_b200.multiobjective.HviScorer"
     reference_point: float | tuple[float, ...] | None = field(default=None, converter=_reference_point)
@@ -346,7 +347,7 @@ class _ExpectedHypervolumeImprovement(_ScoredAcquisitionFunction):
         reference point and the partitioning of the posterior-mean front."""
         from baybe_b200.multiobjective import build_hvi_scorer
 
-        self._check_pareto(objective, searchspace)
+        self._check_pareto(objective, searchspace, discrete_only=False)
         surrogate.fit(searchspace, objective, measurements)
         gps = [s.device_gp for s in surrogate._surrogates_flat]
         return build_hvi_scorer(self, gps, searchspace, objective, measurements)

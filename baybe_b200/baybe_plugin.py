@@ -135,8 +135,8 @@ class EngineAcquisitionFunction:
 class B200BotorchRecommender(BayesianRecommender):
     """``BotorchRecommender`` with the scoring path on the B200 engine: discrete spaces, and continuous and hybrid
     spaces with the single-target acquisition functions, for single targets and for desirability and transformed
-    targets, and with qNIPV (gradient path, ``baybe_b200.continuous``), or qNEI (hybrid spaces, search by scoring,
-    ``baybe_b200.hybrid``)."""
+    targets, with qNIPV, and with qEHVI / qLogEHVI for Pareto objectives (gradient path, ``baybe_b200.continuous``), or
+    qNEI (hybrid spaces, search by scoring, ``baybe_b200.hybrid``)."""
 
     compatibility: ClassVar[SearchSpaceType] = SearchSpaceType.HYBRID
     supports_discrete_subset_generating_constraints: ClassVar[bool] = True
@@ -257,7 +257,7 @@ class B200BotorchRecommender(BayesianRecommender):
 
         assert self._objective is not None and self._context is not None
         cfg, _, pending = self._context
-        gradient_kinds = _lib.GRAD_KINDS + _lib.NIPV_KINDS
+        gradient_kinds = _lib.GRAD_KINDS + _lib.NIPV_KINDS + _lib.HVI_KINDS
         if cfg.kind != "qNEI" and (cfg.kind not in gradient_kinds or not self._gradient_scorer_ok()):
             raise IncompatibleAcquisitionFunctionError(
                 "hybrid search spaces are served with qNoisyExpectedImprovement or the single-target acquisition "
@@ -290,24 +290,26 @@ class B200BotorchRecommender(BayesianRecommender):
 
     def _gradient_scorer_ok(self) -> bool:
         """The gradient path serves the fused path's single targets, the ``ObjectiveScorer`` (desirability, non-affine
-        single targets) and the ``NipvScorer`` (qNIPV); the other scorers (Pareto objectives, qNEI / qLogNEI) are not
-        served."""
+        single targets), the ``NipvScorer`` (qNIPV) and the ``HviScorer`` (qEHVI / qLogEHVI); the other scorers
+        (qNEHVI, qLogNParEGO, qNEI / qLogNEI) are not served."""
+        from baybe_b200.multiobjective import HviScorer
         from baybe_b200.nipv import NipvScorer
         from baybe_b200.objectives import ObjectiveScorer
 
-        return self._scorer is None or isinstance(self._scorer, (ObjectiveScorer, NipvScorer))
+        return self._scorer is None or isinstance(self._scorer, (ObjectiveScorer, NipvScorer, HviScorer))
 
     def _optimize_gradient(self, searchspace, disc_comp: np.ndarray, batch_size: int):
         """Multi-start L-BFGS-B on ``bb_acq_grad`` (``bb_objective_grad`` for objectives that are not affine in their
-        targets, ``bb_nipv_grad`` for qNIPV) over disc_comp x the continuous box (``baybe_b200.continuous``): (points in comp-rep column order,
-        configuration indices, joint value of [batch; pending])."""
+        targets, ``bb_nipv_grad`` for qNIPV, ``bb_hvi_grad`` for qEHVI / qLogEHVI) over disc_comp x the continuous box
+        (``baybe_b200.continuous``): (points in comp-rep column order, configuration indices, joint value of [batch;
+        pending])."""
         from baybe.parameters.numerical import _FixedNumericalContinuousParameter
 
         from baybe_b200.continuous import recommend_continuous_hybrid
 
         cfg, _, pending = self._context
         cont = searchspace.continuous
-        if cfg.kind not in _lib.GRAD_KINDS + _lib.NIPV_KINDS or not self._gradient_scorer_ok():
+        if cfg.kind not in _lib.GRAD_KINDS + _lib.NIPV_KINDS + _lib.HVI_KINDS or not self._gradient_scorer_ok():
             raise IncompatibleAcquisitionFunctionError(
                 f"continuous search spaces are served with the single-target acquisition functions {_lib.GRAD_KINDS} "
                 f"on the B200 engine (got '{cfg.kind}')")

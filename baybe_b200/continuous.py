@@ -24,7 +24,9 @@ Objectives that are not affine in their targets (desirability, transformed singl
 ``base_samples``.  Its pending-point conditioning is built once per greedy step and reused by every evaluation.
 qNIPV comes the same way, as a ``baybe_b200.nipv.NipvScorer``: raw and final values from ``bb_nipv_score``, gradients
 from ``bb_nipv_grad`` over the integration points' image, which is built once per greedy step with the conditioning
-on [pending; earlier batch points].
+on [pending; earlier batch points].  qEHVI and qLogEHVI of Pareto objectives come as a
+``baybe_b200.multiobjective.HviScorer``: raw and final values from ``bb_hvi_score``, gradients from ``bb_hvi_grad``;
+the per-sample box decompositions of the front joined with the pending samples are built once per greedy step.
 
 Deliberate deviation for hybrid spaces: the reference runs a full multi-start optimisation for every discrete
 configuration (its own docstring calls that brute force).  Here the raw sweep ranks every configuration at once and the
@@ -84,15 +86,17 @@ def _scores(gp, cfg: AcqConfig, rows: np.ndarray, pending: np.ndarray | None, se
 
 def _is_scorer(gp) -> bool:
     """The scorers the gradient path serves in place of a model: ``ObjectiveScorer`` (desirability, transformed single
-    targets) and ``NipvScorer`` (qNIPV)."""
+    targets), ``NipvScorer`` (qNIPV) and ``HviScorer`` (qEHVI / qLogEHVI)."""
+    from baybe_b200.multiobjective import HviScorer
     from baybe_b200.nipv import NipvScorer
     from baybe_b200.objectives import ObjectiveScorer
 
-    return isinstance(gp, (ObjectiveScorer, NipvScorer))
+    return isinstance(gp, (ObjectiveScorer, NipvScorer, HviScorer))
 
 
 def _models(gp, scorer: bool) -> list:
-    """The models behind `gp`: an ``ObjectiveScorer``'s one per target, a ``NipvScorer``'s one, or `gp` itself."""
+    """The models behind `gp`: an ``ObjectiveScorer``'s or ``HviScorer``'s one per target, a ``NipvScorer``'s one, or
+    `gp` itself."""
     if not scorer:
         return [gp]
     return list(gp.gps) if hasattr(gp, "gps") else [gp.gp]
@@ -147,9 +151,9 @@ def recommend_continuous_hybrid(gp, cfg: AcqConfig, disc_comp: np.ndarray, cont_
     ``disc_comp``: (n_configs, d_disc) comp-rep rows of the discrete subspace, which comes first in the comp-rep (a
     continuous space: one row of width 0); ``cont_bounds``: (2, d_cont); ``fixed``: continuous column -> value of the
     fixed parameters.  ``gp``: a ``DeviceGP`` (or a stand-in with ``value_and_grad``, ``score``, ``score_joint``), or an
-    ``ObjectiveScorer`` or ``NipvScorer`` (then ``cfg`` is its ``cfg``)."""
+    ``ObjectiveScorer``, ``NipvScorer`` or ``HviScorer`` (then ``cfg`` is its ``cfg``)."""
     scorer = _is_scorer(gp)
-    kinds = _lib.GRAD_KINDS + (_lib.NIPV_KINDS if scorer else ())
+    kinds = _lib.GRAD_KINDS + (_lib.NIPV_KINDS + _lib.HVI_KINDS if scorer else ())
     if cfg.kind not in kinds:
         raise NotImplementedError(f"the gradient path serves {kinds}, not {cfg.kind!r}")
     if any(getattr(m, "task_col", None) is not None for m in _models(gp, scorer)):

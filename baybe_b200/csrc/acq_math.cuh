@@ -25,6 +25,13 @@ __device__ __forceinline__ float log_fatplus_t(float t) {
   return logf(sp + 0.1f / fmaf(t, t, 1.0f));
 }
 
+// botorch fatminimum(y, u) = -fatmax(-y, -u) = min(y, u) - tau log(1 + (1 + |y - u| / (2 tau))^-2); exactly y for u = +inf
+// (k_hvi, k_hvi_grad)
+__device__ __forceinline__ float fatmin_f(float y, float u, float half_inv_tau, float tau) {
+  const float w = fmaf(fabsf(y - u), half_inv_tau, 1.0f);
+  return fminf(y, u) - tau * __logf(1.0f + 1.0f / (w * w));
+}
+
 // ---- conditional moments of a candidate given P pending points (one warp per candidate) ----------------------------
 // |L^-1 c|^2 with lane j holding c_j (0 for j >= P) and forming (L^-1 c)_j; linv: L_PP^-1 row-major [P][P], lower
 // triangular.  A sum of squares: no cancellation against var for nearly collinear pending points.  Every lane

@@ -152,4 +152,138 @@ __device__ __forceinline__ float linvt_apply_col(const float* linv, int n_pad, c
   return u;
 }
 
+// ---- one model per target with P pending points (k_objective_grad, k_hvi_grad) ------------------------------------
+// A target's model as the multi-target gradient kernels read it.
+struct GradTarget {
+  const float *cand_scale, *cand_shift, *train_m2, *alpha, *linv, *mean_const;
+  const float* pend_beta;  // [P][n_pad]
+  int n, n_pad;
+  float y_mean, y_std, sf2;
+};
+
+// A target's slice of a warp's scratch: a [d_pad] | k, gk, v [n_pad] | c, L^-1 c, gkp, A_c [32] (gkp: 2 s_f^2 dk/dt
+// of k(x, x_p); A_c: dA/dc_p).
+struct TargetScratch {
+  float *a, *k, *gk, *v, *c, *r, *gkp, *ac;
+};
+
+// Forward pass of one target for the point x (its d raw coordinates), P pending points with rows pend_x [P][d] and
+// L_PP^-1 plinv [P][P]: fills the scratch (A_c zeroed) and returns, in every lane, mu, var and
+// sd = sqrt(max(var - |L^-1 c|^2, 0)); the return value says whether the variance clamp is inactive (it passes no
+// gradient when it is).
+template <int FAMILY>
+__device__ __forceinline__ bool target_forward_warp(const GradTarget& md, const float* x, int d, int dp, int P,
+                                                    const float* pend_x, const float* plinv, const TargetScratch& t,
+                                                    float& mu, float& var, float& sd, int lane) {
+  for (int j = lane; j < dp; j += 32)
+    t.a[j] = j < d ? fmaf(__ldg(x + j), __ldg(md.cand_scale + j), __ldg(md.cand_shift + j)) : 0.f;
+  __syncwarp();
+  const float ka =
+      warp_sum(kernel_row_warp<FAMILY>(t.a, md.train_m2, md.alpha, md.n, md.n_pad, d, dp, md.sf2, t.k, t.gk, lane));
+  __syncwarp();
+  const float vv = warp_sum(linv_apply_warp(md.linv, md.n_pad, t.k, t.v, lane));
+  const float sy = md.y_std, sy2 = sy * sy;
+  const float vt = md.sf2 - vv;
+  mu = fmaf(sy, __ldg(md.mean_const) + ka, md.y_mean);
+  var = sy2 * fmaxf(vt, 1e-10f);
+  float cr = 0.f;  // lane q < P: c_q
+  for (int q = 0; q < P; ++q) {
+    float kb = 0.f;
+    for (int i = lane; i < md.n_pad; i += 32) kb = fmaf(t.k[i], __ldg(md.pend_beta + (size_t)q * md.n_pad + i), kb);
+    kb = warp_sum(kb);
+    if (lane == q) cr = kb;
+  }
+  float g = 0.f;
+  if (lane < P) {
+    float tt = 0.f;
+    for (int j = 0; j < d; ++j) {
+      const float b = fmaf(__ldg(pend_x + (size_t)lane * d + j), __ldg(md.cand_scale + j), __ldg(md.cand_shift + j));
+      const float df = t.a[j] - b;
+      tt = fmaf(df, df, tt);
+    }
+    float k, dk;
+    kernel_and_slope<FAMILY>(tt, k, dk);
+    cr = sy2 * (md.sf2 * k - cr);
+    g = 2.f * md.sf2 * dk;
+  }
+  t.c[lane] = lane < P ? cr : 0.f;
+  t.gkp[lane] = g;
+  t.ac[lane] = 0.f;
+  // r = L^-1 c (lane i: r_i), as pending_r2_warp forms it
+  float r = 0.f;
+  for (int k = 0; k < P; ++k) {
+    const float ck = __shfl_sync(kFull, cr, k);
+    if (lane < P && k <= lane) r = fmaf(__ldg(plinv + lane * P + k), ck, r);
+  }
+  t.r[lane] = lane < P ? r : 0.f;
+  const float r2 = warp_sum(lane < P ? r * r : 0.f);
+  sd = P > 0 ? sqrtf(fmaxf(var - r2, 0.f)) : sqrtf(var);
+  __syncwarp();
+  return vt > 1e-10f;
+}
+
+// sd = sqrt(max(var - |r|^2, 0)), r = L^-1 c, with A_sd = dA/dsd summed over the warp: returns A_var = A_sd / (2 sd)
+// and adds -A_sd L^-T r / sd to A_c (lanes < P).
+__device__ __forceinline__ float target_sd_adjoint(float a_sd, float sd, int P, const float* plinv,
+                                                   const TargetScratch& t, int lane) {
+  const float f = sd > 0.f ? a_sd / sd : 0.f;
+  if (lane < P) {
+    float lt = 0.f;
+    for (int i = lane; i < P; ++i) lt = fmaf(__ldg(plinv + i * P + lane), t.r[i], lt);
+    t.ac[lane] = fmaf(-f, lt, t.ac[lane]);
+  }
+  return 0.5f * f;
+}
+
+// Reverse pass through the kernel row: k_i <- gk_i dA/dk_i with
+// dA/dk_i = s_y A_mu alpha_i - 2 s_y^2 A_var u_i - s_y^2 sum_p A_c[p] beta_p,i (lanes over columns).
+__device__ __forceinline__ void target_row_adjoint(const GradTarget& md, float a_mu, float a_var, int P,
+                                                   const TargetScratch& t, int lane) {
+  const float sy = md.y_std, sy2 = sy * sy;
+  const float k_mu = sy * a_mu, k_var = -2.f * sy2 * a_var;
+  for (int i0 = 0; i0 < md.n_pad; i0 += 32) {
+    const int i = i0 + lane;
+    const float u = linvt_apply_col(md.linv, md.n_pad, t.v, i0, i);
+    float kb = fmaf(k_mu, __ldg(md.alpha + i), k_var * u);
+    for (int q = 0; q < P; ++q) kb = fmaf(-sy2 * t.ac[q], __ldg(md.pend_beta + (size_t)q * md.n_pad + i), kb);
+    t.k[i] = t.gk[i] * kb;
+  }
+}
+
+// dA/da_j of one target after target_row_adjoint: the training rows' terms and the direct k(x, x_p) term (multiply
+// by cand_scale[j] for dA/dx_j).
+__device__ __forceinline__ float target_col_grad(const GradTarget& md, int j, int d, int dp, int P,
+                                                 const float* pend_x, const TargetScratch& t) {
+  const float sy2 = md.y_std * md.y_std;
+  const float aj = t.a[j];
+  float g = 0.f;
+  for (int i = 0; i < md.n; ++i) g = fmaf(t.k[i], aj + 0.5f * __ldg(md.train_m2 + (size_t)i * dp + j), g);
+  for (int q = 0; q < P; ++q) {
+    const float b = fmaf(__ldg(pend_x + (size_t)q * d + j), __ldg(md.cand_scale + j), __ldg(md.cand_shift + j));
+    g = fmaf(sy2 * t.ac[q] * t.gkp[q], aj - b, g);
+  }
+  return g;
+}
+
+// Floats of one warp's scratch for M targets: M TargetScratch slices, the sample chunk's adjoints [32][M] and 32
+// per-target scalars (mu | var | sd | A_var, 8 each).
+__host__ __device__ inline int target_warp_floats(int M, int n_pad, int d_pad) {
+  return (M * (d_pad + 3 * n_pad + 4 * 32) + 32 * M + 32 + 3) & ~3;
+}
+
+// Target m's slice of the scratch that starts at wb, laid out as k_objective_grad lays it out.
+__device__ __forceinline__ TargetScratch target_scratch(float* wb, int M, int m, int np, int dp) {
+  TargetScratch t;
+  t.a = wb + m * dp;
+  t.k = wb + M * dp + m * np;
+  t.gk = wb + M * (dp + np) + m * np;
+  t.v = wb + M * (dp + 2 * np) + m * np;
+  float* c0 = wb + M * (dp + 3 * np);
+  t.c = c0 + m * 32;
+  t.r = c0 + M * 32 + m * 32;
+  t.gkp = c0 + 2 * M * 32 + m * 32;
+  t.ac = c0 + 3 * M * 32 + m * 32;
+  return t;
+}
+
 }  // namespace bb

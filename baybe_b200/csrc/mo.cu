@@ -27,12 +27,6 @@ struct HviParams : ScoreParams {  // C = P pending points; w: [M][S][P]
   float a[BB_HVI_MAX_TARGETS], b[BB_HVI_MAX_TARGETS];
 };
 
-// botorch fatminimum(y, u) = -fatmax(-y, -u) = min(y, u) - tau log(1 + (1 + |y - u| / (2 tau))^-2); exactly y for u = +inf
-__device__ __forceinline__ float fatmin_f(float y, float u, float half_inv_tau, float tau) {
-  const float w = fmaf(fabsf(y - u), half_inv_tau, 1.0f);
-  return fminf(y, u) - tau * __logf(1.0f + 1.0f / (w * w));
-}
-
 constexpr int kHviThreads = 256;
 
 template <int M, bool LOG>

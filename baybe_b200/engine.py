@@ -1080,6 +1080,48 @@ def _(x, handles, pend_x, betas, linv, w, pend_terms, z, kind, params, scalarize
     return x.new_empty(x.shape[0]), x.new_empty(x.shape)
 
 
+@torch.library.custom_op("baybe_b200::hvi_grad", mutates_args=())
+def _op_hvi_grad(x: torch.Tensor, handles: list[int], pend_x: torch.Tensor | None, betas: list[torch.Tensor],
+                 linv: torch.Tensor | None, w: torch.Tensor | None, z: torch.Tensor, lower: torch.Tensor,
+                 upper: torch.Tensor, n_cells: torch.Tensor, kind: int, params: list[float], obj_scale: list[float],
+                 obj_shift: list[float]) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_hvi_grad``: raw fp32 rows x [N, d] of the models `handles` (one per target) -> value [N] (what
+    ``hvi_score`` scores), gradient [N, d].  With P pending points their rows pend_x [P, d], one beta [P, n_pad] per
+    model (``pending_stats``), linv [M, P, P] and w [M, S, P]; z [S, M(1+P)]; cells lower/upper [n_dec, C, M] float32
+    with counts n_cells [n_dec] int32 (n_dec = 1 without pending points, else S), as ``hvi_score``."""
+    gps = [_gp(h) for h in handles]
+    M, N = len(gps), x.shape[0]
+    if x.dim() != 2 or x.shape[1] != gps[0].d or x.dtype != torch.float32 or not x.is_contiguous():
+        raise ValueError(f"rows must be a contiguous float32 (N, {gps[0].d}) tensor")
+    P = 0 if pend_x is None else pend_x.shape[0]
+    S = z.shape[0]
+    if z.dim() != 2 or z.shape[1] != M * (1 + P):
+        raise ValueError(f"base samples must be (S, {M * (1 + P)})")
+    if P and len(betas) != M:
+        raise ValueError(f"{P} pending points need one beta per model ({M})")
+    if lower.shape != upper.shape or lower.dim() != 3 or lower.shape[2] != M or n_cells.numel() != lower.shape[0] \
+            or n_cells.dtype != torch.int32 or lower.shape[0] != (1 if P == 0 else S):
+        raise ValueError("cells must be lower/upper [n_dec, C, M] with n_cells [n_dec] (n_dec = 1 or S)")
+    acq = AcqConfig.from_params(kind, params).to_c()
+    models = (C.POINTER(_lib.Model) * M)(*(C.pointer(gp.model) for gp in gps))
+    beta_ptrs = (C.c_void_p * M)(*((b.data_ptr() for b in betas) if P else [None] * M))
+    fa = (C.c_float * M)(*obj_scale)
+    fb = (C.c_float * M)(*obj_shift)
+    value = torch.empty(N, dtype=torch.float32, device=x.device)
+    grad = torch.empty((N, x.shape[1]), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().bb_hvi_grad(models, M, C.byref(acq), fa, fb, _ptr(x), N, P, _ptr(pend_x),
+                                           beta_ptrs if P else None, _ptr(linv), _ptr(w), _ptr(z), S, _ptr(lower),
+                                           _ptr(upper), _ptr(n_cells), lower.shape[1], _ptr(value), _ptr(grad),
+                                           _stream_ptr()), "bb_hvi_grad")
+    return value, grad
+
+
+@_op_hvi_grad.register_fake
+def _(x, handles, pend_x, betas, linv, w, z, lower, upper, n_cells, kind, params, obj_scale, obj_shift):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+
+
 @torch.library.custom_op("baybe_b200::argmax", mutates_args=())
 def _op_argmax(score: torch.Tensor, keep: torch.Tensor | None, index_offset: int) -> torch.Tensor:
     key = torch.empty(1, dtype=torch.int64, device=score.device)

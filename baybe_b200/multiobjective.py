@@ -8,7 +8,9 @@ The host owns what does not depend on the candidate, in float64:
   * an exact box decomposition of the region F does not dominate (``box_decomposition``), and with pending points
     one decomposition of F u P_s per base sample s together with the exact improvement of P_s over F.
 ``bb_hvi_score`` (csrc/mo.cu) evaluates the candidate-dependent improvement of every row on the device; the
-sequential-greedy loop is ``baybe_b200.recommenders.greedy_select``.
+sequential-greedy loop is ``baybe_b200.recommenders.greedy_select``.  On continuous and hybrid spaces
+``HviScorer.value_and_grad`` gives the continuous optimiser (``baybe_b200.continuous``) the same value and its gradient
+with respect to the raw rows (``bb_hvi_grad``, csrc/hvigrad.cu).
 """
 from __future__ import annotations
 
@@ -45,6 +47,12 @@ __all__ = ["compute_ref_point", "box_decomposition", "HviScorer", "build_hvi_sco
 def _hvi_score(*args):
     """``baybe_b200::hvi_score`` (engine.py); a module-level seam so that CPU tests can put a float64 stand-in here."""
     return torch.ops.baybe_b200.hvi_score(*args)
+
+
+def _hvi_grad(gps, *rest):
+    """``baybe_b200::hvi_grad`` (engine.py) on the models' handles; a module-level seam so that CPU tests can put a
+    float64 stand-in here (same arguments, with the models themselves in place of their handles)."""
+    return torch.ops.baybe_b200.hvi_grad(rest[0], [gp.handle for gp in gps], *rest[1:])
 
 
 def compute_ref_point(array, maximize=None, factor: float = 0.1) -> np.ndarray:
@@ -169,13 +177,20 @@ class HviScorer(Scorer):
         self.front = np.asarray(front, dtype=np.float64).reshape(-1, self.M)
         self.lower, self.upper, self.hv_front = box_decomposition(self.front, self.ref)
         self.device = self.gps[0].device
+        self._front_decomps = [(self.lower, self.upper)]
+        self._parts = None  # (pending rows, base samples, _pending_parts result) of the last step
+        self._cells = None  # (decompositions, their padded device tensors) of the last evaluation
 
     # ---- candidate-independent set-up of one evaluation ----------------------------------------------------
     def _pending_parts(self, pend: np.ndarray, z: torch.Tensor):
         """Per target: cross-covariance inputs, L_PP^-1 and L^-T z_P; per sample: decomposition of F u P_s and
-        the exact improvement of P_s over F.  z: (S, M(1+P)) float64."""
-        from baybe_b200.objectives import pending_conditioning
+        the exact improvement of P_s over F.  z: (S, M(1+P)) float64.  The S decompositions are built on the host, so
+        the last result is kept and reused while the pending points and the base samples stay the same (the raw
+        sweep, every L-BFGS-B evaluation and the final scoring of a greedy step)."""
+        from baybe_b200.objectives import _same, pending_conditioning
 
+        if self._parts is not None and _same(self._parts[0], pend) and _same(self._parts[1], z):
+            return self._parts[2]
         S = z.shape[0]
         stats, linv, w, ys = pending_conditioning(self.gps, pend, z)
         ps = self.a * ys + self.b
@@ -184,7 +199,20 @@ class HviScorer(Scorer):
             lo, hi, hv = box_decomposition(np.concatenate([self.front, ps[s]], axis=0), self.ref)
             decomps.append((lo, hi))
             gain[s] = hv - self.hv_front
-        return stats, linv, w, decomps, float(gain.mean())
+        out = (stats, linv, w, decomps, float(gain.mean()))
+        self._parts = (pend.copy(), z.clone(), out)
+        return out
+
+    def _device_cells(self, decomps):
+        """lower, upper [n_dec, C, M] and n_cells [n_dec] of the decompositions on the device (kept for the last
+        list of decompositions)."""
+        if self._cells is not None and self._cells[0] is decomps:
+            return self._cells[1]
+        lower, upper, counts, _ = _padded(decomps, self.M)
+        dev = self.device
+        out = (torch.from_numpy(lower).to(dev), torch.from_numpy(upper).to(dev), torch.from_numpy(counts).to(dev))
+        self._cells = (decomps, out)
+        return out
 
     def values(self, x, pend: np.ndarray | None, z: torch.Tensor, keep=None, index_offset: int = 0,
                want_scores: bool = True):
@@ -197,7 +225,7 @@ class HviScorer(Scorer):
         if P == 0:
             post = [gp.posterior(xd) for gp in self.gps]
             cross = linv = w = None
-            decomps, gain = [(self.lower, self.upper)], 0.0
+            decomps, gain = self._front_decomps, 0.0
         else:
             stats, linv_h, w_h, decomps, gain = self._pending_parts(np.asarray(pend, dtype=np.float64), z)
             post = [gp.cross_covariance(xd, px, beta) for gp, (px, beta) in zip(self.gps, stats)]
@@ -206,14 +234,42 @@ class HviScorer(Scorer):
             w = torch.from_numpy(w_h).to(self.device, torch.float32)
         mu = torch.stack([p[0] for p in post]).contiguous()
         var = torch.stack([p[1] for p in post]).contiguous()
-        lower, upper, counts, C = _padded(decomps, M)
+        lower, upper, counts = self._device_cells(decomps)
         dev = self.device
         scores, key = _hvi_score(
-            mu, var, cross, linv, w, z.to(dev, torch.float32).contiguous(), torch.from_numpy(lower).to(dev),
-            torch.from_numpy(upper).to(dev), torch.from_numpy(counts).to(dev), keep, _lib.ACQ_KIND[self.cfg.kind],
-            self.cfg.params(), [float(v) for v in self.a], [float(v) for v in self.b], int(index_offset),
-            bool(want_scores))
+            mu, var, cross, linv, w, z.to(dev, torch.float32).contiguous(), lower, upper, counts, keep,
+            _lib.ACQ_KIND[self.cfg.kind], self.cfg.params(), [float(v) for v in self.a], [float(v) for v in self.b],
+            int(index_offset), bool(want_scores))
         return (scores if want_scores else None), key, self._reporter(gain)
+
+    def value_and_grad(self, x, pend: np.ndarray | None, z: torch.Tensor):
+        """Acquisition value [N] and its gradient [N, d] with respect to the raw comp-rep rows x (``bb_hvi_grad``),
+        float64 on the host: the value ``scores`` reports for [x; pending] (the kernel's value through the reporter),
+        with the base samples z of ``base_samples`` (M(1+P) columns).  qEHVI's reporter adds a constant; qLogEHVI's,
+        logaddexp(log gain, v), scales the gradient by sigmoid(v - log gain)."""
+        M = self.M
+        P = 0 if pend is None else len(pend)
+        z = torch.as_tensor(z, dtype=torch.float64).reshape(-1, M * (1 + P))
+        xd = self.gps[0].prepare(x).to(torch.float32).contiguous()
+        dev = self.device
+        px, betas, linv, w = None, [], None, None
+        if P == 0:
+            decomps, gain = self._front_decomps, 0.0
+        else:
+            stats, linv_h, w_h, decomps, gain = self._pending_parts(np.asarray(pend, dtype=np.float64), z)
+            px = stats[0][0]
+            betas = [beta for _, beta in stats]
+            linv = torch.from_numpy(linv_h).to(dev, torch.float32)
+            w = torch.from_numpy(w_h).to(dev, torch.float32)
+        lower, upper, counts = self._device_cells(decomps)
+        val, grad = _hvi_grad(self.gps, xd, px, betas, linv, w, z.to(dev, torch.float32).contiguous(), lower, upper,
+                              counts, _lib.ACQ_KIND[self.cfg.kind], self.cfg.params(), [float(v) for v in self.a],
+                              [float(v) for v in self.b])
+        v = val.double().cpu()
+        g = grad.double().cpu()
+        if gain > 0.0 and self.cfg.kind == "qLogEHVI":
+            g = g * torch.sigmoid(v - math.log(gain))[:, None]
+        return torch.from_numpy(np.asarray(self._reporter(gain)(v.numpy()), dtype=np.float64)), g
 
     def _reporter(self, gain: float):
         if gain <= 0.0:

@@ -595,6 +595,30 @@ int bb_objective_grad(const bb_model* const* models, int32_t n_targets, const bb
                       const float* d_pend_terms, const float* d_z, int32_t S, float* d_value, float* d_grad,
                       void* stream);
 
+/* ---- value and gradient of the hypervolume improvement bb_hvi_score reports (qEHVI / qLogEHVI of a Pareto objective)
+ * at N points, for the continuous optimiser.
+ *   models: host array of n_targets = M in [2, BB_HVI_MAX_TARGETS] models, one per target in objective order; each
+ *     non-wide, single-task, n_pad <= 256 (else BB_ERR_UNSUPPORTED); they share d and the kernel family, and may
+ *     differ in n, scaling and hyper-parameters.
+ *   a: BB_ACQ_QEHVI or BB_ACQ_QLOGEHVI (tau_relu, tau_max > 0); obj_scale / obj_shift: HOST arrays [M], the
+ *     orientation o_m = obj_scale[m] y_m + obj_shift[m] as bb_hvi_score takes it.
+ *   d_x [N][d]: raw comp-rep rows, fp32 row-major.
+ *   n_pending = P in [0, BB_MAX_PENDING].  With P > 0: d_pend_x [P][d] raw rows; d_pend_beta: host array of M device
+ *     pointers, entry m the [P][n_pad_m] beta bb_pending_stats returns for model m; d_linv [M][P][P] and d_w [M][S][P]
+ *     as bb_hvi_score takes them.
+ *   d_z [S][M(1+P)]: base samples as bb_hvi_score (S in [1, 1024]).
+ *   d_lower / d_upper / d_n_cells / cell_stride: the cells as bb_hvi_score takes them (one decomposition for P = 0,
+ *     one per sample for P > 0).
+ * The mean, variance and cross covariances of every target are formed from x (as bb_acq_grad).  Writes d_value [N],
+ * the value bb_hvi_score writes to d_score for the same inputs (without the pending points' own improvement, which
+ * the host adds), and d_grad [N][d], its gradient with respect to the raw comp-rep coordinates.  Synchronises
+ * nothing; no float atomics: repeated calls are bit-identical. */
+int bb_hvi_grad(const bb_model* const* models, int32_t n_targets, const bb_acq_spec* a, const float* obj_scale,
+                const float* obj_shift, const float* d_x, int64_t N, int32_t n_pending, const float* d_pend_x,
+                const float* const* d_pend_beta, const float* d_linv, const float* d_w, const float* d_z, int32_t S,
+                const float* d_lower, const float* d_upper, const int32_t* d_n_cells, int32_t cell_stride,
+                float* d_value, float* d_grad, void* stream);
+
 /* ---- test-only diagnostic: plain fp32 SIMT posterior (no tensor cores), used by the GPU
  * tests to separate tensor-core-path errors from formula errors.  Not called by the product. -- */
 int bb_debug_posterior_simt(const bb_model* m, const void* d_x, int32_t layout, int64_t N,
