@@ -41,8 +41,10 @@ NIPV_MAX_TRAIN = 256
 # partial sum per point, so the workspace depends on M only up to that count
 NIPV_GRAD_CTAS = 264
 NIPV_IMAGE_CAP = 4 << 30  # bytes of the integration points' image, (n + |C| + d) M fp32
-# single-target kinds with a gradient path (bb_acq_grad): continuous and hybrid spaces, baybe_b200/continuous.py
+# single-target kinds with a gradient path (bb_acq_grad, bb_acq_grad_large): continuous and hybrid spaces,
+# baybe_b200/continuous.py
 GRAD_KINDS = ("qLogEI", "qEI", "qUCB", "qSR", "qPI", "UCB", "EI", "LogEI", "PI", "PM", "PSTD")
+# bb_acq_grad takes models that are not wide with n_pad up to this; bb_acq_grad_large takes the rest (engine.acq_grad_op)
 GRAD_MAX_NPAD = 256
 MAX_PENDING = 31
 MAX_TRAIN = 1024
@@ -168,6 +170,8 @@ _SIGNATURES = {
                                 _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _sz, _vp]),
     "bb_acq_grad": (C.c_int, [C.POINTER(Model), C.POINTER(AcqSpec), _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _i32,
                               _vp, _vp, _vp]),
+    "bb_acq_grad_large": (C.c_int, [C.POINTER(Model), C.POINTER(AcqSpec), _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp,
+                                    _i32, _vp, _vp, _vp]),
     "bb_objective_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(Objective), _vp,
                                     _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "bb_hvi_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(C.c_float),

@@ -136,7 +136,9 @@ class B200BotorchRecommender(BayesianRecommender):
     """``BotorchRecommender`` with the scoring path on the B200 engine: discrete spaces, and continuous and hybrid
     spaces with the single-target acquisition functions, for single targets and for desirability and transformed
     targets, with qNIPV, and with qEHVI / qLogEHVI for Pareto objectives (gradient path, ``baybe_b200.continuous``), or
-    qNEI (hybrid spaces, search by scoring, ``baybe_b200.hybrid``)."""
+    qNEI (hybrid spaces, search by scoring, ``baybe_b200.hybrid``).  The single-target kinds on a single target run on
+    every single-task model up to 1024 measurements, wide comp-rep encodings included (``bb_acq_grad_large`` past 256
+    training points and for wide models)."""
 
     compatibility: ClassVar[SearchSpaceType] = SearchSpaceType.HYBRID
     supports_discrete_subset_generating_constraints: ClassVar[bool] = True

@@ -13,7 +13,8 @@ serves both: a continuous space is a hybrid space with one empty discrete config
     included.  A hybrid start keeps its discrete configuration.
   * Polish: ``scipy.optimize.minimize(method="L-BFGS-B", jac=True)`` over the stacked starts on -sum(value), as
     botorch's ``gen_candidates_scipy`` stacks its restarts (maxiter 200 [U]); value and gradient come from
-    ``bb_acq_grad``, one call over all starts per evaluation.  Fixed continuous parameters and discrete columns are not
+    ``bb_acq_grad``, or ``bb_acq_grad_large`` for wide models and n_pad > 256 (up to 1024 training points, chosen by
+    ``engine.acq_grad_op``), one call over all starts per evaluation.  Fixed continuous parameters and discrete columns are not
     variables.  The best start wins, judged by the scoring path.
   * q > 1: sequential greedy (``optimize_acqf(sequential=True)``, ``optimize_acqf_mixed``): step j optimises the q = 1
     value given pending = [pending experiments; x_1 ... x_{j-1}].

@@ -15,6 +15,7 @@
 //   grad_x A = (sum_i dA/dk_i dk_i/da + s_y^2 sum_p A_c[p] dk(x, x_p)/da) * scale.
 // v is formed 32 rows at a time: each lane takes every 32nd column of the 32 rows (coalesced loads of L^-1) and a
 // reduce-scatter over the warp leaves row j0 + l in lane l; u needs no reduction (lane l owns column i0 + l).
+// The value and its partials at a point come from acq_point_partials (grad_common.cuh, shared with k_acq_grad_large).
 // With pending points the value is k_acq_joint's (acq.cu): the Cholesky of [[var, c^T], [c, Sigma_PP]] with the
 // candidate first, the same jitter escalation and the same join of the pending points' terms.  Its reverse pass
 // accumulates dA/dL22 over the samples and goes back through the (1+p) Cholesky with
@@ -45,7 +46,8 @@ struct GradParams {
   float* grad;   // [N][d]
 };
 
-// per-warp scratch in floats: a | k (then dA/dk_i * dk_i/dt) | gk | v | 5 x 32 vectors | L22 | dL22 | 2 x sample chunk
+// per-warp scratch in floats: a | k (then dA/dk_i * dk_i/dt) | gk | v | gkp [32] | acq_point_partials' scratch
+// (4 x 32 vectors | L22 | dL22 | 2 x sample chunk)
 __host__ __device__ inline int grad_warp_floats(int n_pad, int d_pad, int P) {
   return (d_pad + 3 * n_pad + 5 * 32 + 2 * P * P + 2 * 32 * (P + 1) + 3) & ~3;
 }
@@ -63,40 +65,17 @@ __global__ void __launch_bounds__(kGradThreads) k_acq_grad(const GradParams p) {
   float* k_w = a_w + p.d_pad;
   float* gk_w = k_w + p.n_pad;
   float* v_w = gk_w + p.n_pad;
-  float* lv = v_w + p.n_pad;  // [32] l = c / sd
-  float* mP = lv + 32;        // [32] pending means
-  float* moP = mP + 32;       // [32] qUCB: sample mean of each pending point's objective
-  float* gkp = moP + 32;      // [32] 2 s_f^2 dk/dt of k(x, x_p)
-  float* acw = gkp + 32;      // [32] A_c[p]
-  float* Lw = acw + 32;       // [P][P] L22
-  float* Lb = Lw + P * P;     // [P][P] dA/dL22
-  float* Wc = Lb + P * P;     // [32][Q] per-sample weights of the current chunk
-  float* Wm = Wc + 32 * Q;    // [32][Q] qUCB: weights of the sample means
+  float* gkp = v_w + p.n_pad;                 // [32] 2 s_f^2 dk/dt of k(x, x_p)
+  const AcqScratch w = acq_scratch(gkp + 32, P);  // acq_point_partials' scratch
   for (int e = threadIdx.x; e < S * Q; e += blockDim.x) {
     const int s = e / Q, k = e - s * Q;
     z_s[s * zs + k] = __ldg(p.z + e);
   }
   __syncthreads();
   const bb_acq_spec a = p.a;
-  const float a1 = a.obj_scale, a0 = a.obj_shift, sy = p.y_std, sy2 = sy * sy;
-  const float ucb_c = sqrtf(a.beta * 1.5707963267948966f);
-  // column means of the base samples (lane k: column k) and, for q = 1, mean |z - mean z|
-  float zb = 0.f, zdev = 0.f;
-  if (is_mc) {
-    if (lane < Q) {
-      for (int s = 0; s < S; ++s) zb += z_s[s * zs + lane];
-      zb /= (float)S;
-    }
-    if (P == 0) {
-      float sz = 0.f;
-      for (int s = lane; s < S; s += 32) sz += z_s[s * zs];
-      const float zm = warp_sum(sz) / (float)S;
-      float sa = 0.f;
-      for (int s = lane; s < S; s += 32) sa += fabsf(z_s[s * zs] - zm);
-      zdev = warp_sum(sa) / (float)S;
-      zb = zm;  // same value in every lane
-    }
-  }
+  const float sy = p.y_std, sy2 = sy * sy;
+  float zb = 0.f, zdev = 0.f;  // column means of the base samples and, for q = 1, mean |z - mean z|
+  if (is_mc) sample_means_warp(z_s, zs, S, P, zb, zdev, lane);
   const int64_t warp_global = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t c = warp_global; c < p.N; c += nwarps) {
@@ -172,280 +151,9 @@ __global__ void __launch_bounds__(kGradThreads) k_acq_grad(const GradParams p) {
     }
     __syncwarp();
     // ---- value and its partial derivatives (A_mu, A_var, A_c) ----
-    float value, g_mu = 0.f, g_var = 0.f;
-    if (!is_mc) {
-      value = analytic_value(a, mu, var);
-      double dmu, dsd;
-      analytic_partials(a, mu, var, dmu, dsd);
-      g_mu = (float)dmu;
-      g_var = (float)(dsd / (2.0 * sqrt((double)var)));
-    } else if (P == 0) {
-      float c0, c1;
-      mc_coef(a, mu, var, c0, c1);
-      const float sd = sqrtf(var);
-      float s0 = 0.f, s1 = 0.f, h0 = 0.f, h1 = 0.f;  // value sums; sums of d(term)/dt and d(term)/dt * z
-      for (int s = lane; s < S; s += 32) {
-        const float zz = z_s[s * zs], t = fmaf(c1, zz, c0);
-        float g = 0.f;
-        if (a.kind == BB_ACQ_QLOGEI) {
-          const float q = 1.f / fmaf(t, t, 1.f);
-          s0 += fmaxf(t, 0.f) + ((fabsf(t) < 30.f) ? log1pf(expf(-fabsf(t))) : 0.f);
-          s1 += q;
-          g = sigmoidf_(t) - 0.2f * (t * q) * q;
-        } else if (a.kind == BB_ACQ_QEI) {
-          s0 += fmaxf(t, 0.f);
-          g = t > 0.f ? 1.f : 0.f;
-        } else if (a.kind == BB_ACQ_QPI) {
-          s0 += sigmoidf_(t);
-          g = dsigmoidf_(t);
-        }
-        h0 += g;
-        h1 = fmaf(g, zz, h1);
-      }
-      s0 = warp_sum(s0);
-      s1 = warp_sum(s1);
-      h0 = warp_sum(h0);
-      h1 = warp_sum(h1);
-      value = mc_finalize(a, mu, var, s0, s1, S, zb, zdev);
-      float d_mu, d_sd;
-      if (a.kind == BB_ACQ_QSR || a.kind == BB_ACQ_QUCB) {
-        d_mu = a1;
-        d_sd = a1 * zb + (a.kind == BB_ACQ_QUCB ? ucb_c * fabsf(a1) * zdev : 0.f);
-      } else {
-        const float inv_tau = a.kind == BB_ACQ_QLOGEI ? 1.f / a.tau_relu : a.kind == BB_ACQ_QPI ? 1.f / a.tau_pi : 1.f;
-        const float norm = a.kind == BB_ACQ_QLOGEI ? 1.f / (s0 + 0.1f * s1) : 1.f / (float)S;
-        d_mu = a1 * inv_tau * h0 * norm;
-        d_sd = a1 * inv_tau * h1 * norm;
-      }
-      g_mu = d_mu;
-      g_var = d_sd / (2.f * sd);
-    } else {
-      // ---- k_acq_joint's forward: Cholesky of the joint covariance, candidate first ----
-      float sd = 0.f;
-      bool ok = false;
-      for (int attempt = 0; attempt < 4 && !ok; ++attempt) {
-        const float jit = attempt == 0 ? 0.f : 1e-6f * __powf(10.f, (float)(attempt - 1));
-        sd = sqrtf(var + jit);
-        const float li = cr / sd;
-        __syncwarp();
-        if (lane < P) {
-          lv[lane] = li;
-          mP[lane] = __ldg(p.pend_mu + lane);
-        }
-        __syncwarp();
-        if (lane < P)
-          for (int j = 0; j <= lane; ++j)
-            Lw[lane * P + j] = __ldg(p.pend_cov + lane * P + j) - li * lv[j] + (j == lane ? jit : 0.f);
-        __syncwarp();
-        bool fail = !(var + jit > 0.f);
-        for (int j = 0; j < P; ++j) {
-          const float dj = Lw[j * P + j];
-          if (!(dj > 0.f)) {
-            fail = true;
-            break;
-          }
-          const float sj = sqrtf(dj);
-          __syncwarp();
-          if (lane == j) Lw[j * P + j] = sj;
-          if (lane > j && lane < P) Lw[lane * P + j] /= sj;
-          __syncwarp();
-          if (lane > j && lane < P) {
-            const float lij = Lw[lane * P + j];
-            for (int k = j + 1; k <= lane; ++k) Lw[lane * P + k] -= lij * Lw[k * P + j];
-          }
-          __syncwarp();
-        }
-        ok = !fail;
-      }
-      __syncwarp();
-      const float zb0 = __shfl_sync(kFull, zb, 0);
-      {
-        float ym = (lane < P) ? fmaf(lv[lane], zb0, mP[lane]) : 0.f;
-        for (int j = 0; j < P; ++j) {
-          const float zbj = __shfl_sync(kFull, zb, 1 + j);
-          if (lane < P && j <= lane) ym = fmaf(Lw[lane * P + j], zbj, ym);
-        }
-        if (lane < P) moP[lane] = fmaf(a1, ym, a0);
-        __syncwarp();
-      }
-      const float mo_c = fmaf(a1, fmaf(sd, zb0, mu), a0);
-      // per-sample terms of point i (0: the candidate) from its objective o
-      auto term = [&](int i, float o) -> float {
-        if (a.kind == BB_ACQ_QLOGEI) return logf(a.tau_relu) + log_fatplus_t((o - a.best_f) / a.tau_relu);
-        if (a.kind == BB_ACQ_QEI) return fmaxf(o - a.best_f, 0.f);
-        if (a.kind == BB_ACQ_QSR) return o;
-        if (a.kind == BB_ACQ_QPI) return 1.0f / (1.0f + __expf(-(o - a.best_f) / a.tau_pi));
-        const float m = i == 0 ? mo_c : moP[i - 1];
-        return m + ucb_c * fabsf(o - m);
-      };
-      auto sample_obj = [&](const float* zr, int i) -> float {  // o of point i >= 1 in sample zr
-        float y = fmaf(lv[i - 1], zr[0], mP[i - 1]);
-        const float* Li = Lw + (i - 1) * P;
-        for (int j = 0; j < i; ++j) y = fmaf(Li[j], zr[1 + j], y);
-        return fmaf(a1, y, a0);
-      };
-      // pass 1: the value, exactly as k_acq_joint forms it
-      float run_max = -INFINITY, run_sum = 0.f;
-      for (int s = lane; s < S; s += 32) {
-        const float* zr = z_s + s * zs;
-        float li_arr[BB_MAX_PENDING + 1];
-        float red = term(0, fmaf(a1, fmaf(sd, zr[0], mu), a0));
-        li_arr[0] = red;
-        for (int i = 1; i < Q; ++i) {
-          const float val = term(i, sample_obj(zr, i));
-          li_arr[i] = val;
-          red = fmaxf(red, val);
-        }
-        if (a.kind == BB_ACQ_QLOGEI) lse_push(fatmax_q(li_arr, Q, red, a.tau_max), run_max, run_sum);
-        else run_sum += red;
-      }
-      float lse = 0.f;
-      if (a.kind == BB_ACQ_QLOGEI) {
-        lse_warp_combine(run_max, run_sum);
-        lse = run_max + logf(run_sum);
-        value = lse - logf((float)S);
-      } else {
-        value = warp_sum(run_sum) / (float)S;
-      }
-      // pass 2: per-sample weights dA/dy_i in chunks of 32 samples, accumulated into dA/d(mu, sd, l, L22)
-      float acc_l = 0.f, acc_m = 0.f, acc_wm = 0.f, acc_mu = 0.f, acc_sd = 0.f;
-      for (int e = lane; e < P * P; e += 32) Lb[e] = 0.f;
-      for (int s0 = 0; s0 < S; s0 += 32) {
-        const int s = s0 + lane;
-        __syncwarp();
-        for (int i = 0; i < Q; ++i) {
-          Wc[lane * Q + i] = 0.f;
-          Wm[lane * Q + i] = 0.f;
-        }
-        if (s < S) {
-          const float* zr = z_s + s * zs;
-          float ob[BB_MAX_PENDING + 1], li_arr[BB_MAX_PENDING + 1];
-          ob[0] = fmaf(a1, fmaf(sd, zr[0], mu), a0);
-          float red = term(0, ob[0]);
-          li_arr[0] = red;
-          int imax = 0;
-          for (int i = 1; i < Q; ++i) {
-            ob[i] = sample_obj(zr, i);
-            const float val = term(i, ob[i]);
-            li_arr[i] = val;
-            if (val > red) {
-              red = val;
-              imax = i;
-            }
-          }
-          float w_s = 1.f / (float)S;  // dA/d(reduced sample)
-          if (a.kind == BB_ACQ_QLOGEI) {
-            const float fm = fatmax_q(li_arr, Q, red, a.tau_max);
-            w_s = expf(fm - lse);
-            const float inv = 1.0f / (2.0f * a.tau_max);
-            float ssum = 0.f;
-            for (int k = 0; k < Q; ++k) {
-              const float w = fmaf(red - li_arr[k], inv, 1.0f);
-              ssum += 1.0f / (w * w);
-            }
-            float rest = 0.f;
-            for (int k = 0; k < Q; ++k) {
-              const float w = fmaf(red - li_arr[k], inv, 1.0f);
-              const float dk = 1.0f / (w * w * w) / ssum;
-              rest += dk;
-              Wc[lane * Q + k] = dk;
-            }
-            Wc[lane * Q + imax] += 1.f - rest;
-            for (int k = 0; k < Q; ++k)
-              Wc[lane * Q + k] *= w_s * a1 * dlog_fatplus_t((ob[k] - a.best_f) / a.tau_relu) / a.tau_relu;
-          } else {
-            float d;
-            const float o = ob[imax];
-            if (a.kind == BB_ACQ_QEI) d = o - a.best_f > 0.f ? 1.f : 0.f;
-            else if (a.kind == BB_ACQ_QSR) d = 1.f;
-            else if (a.kind == BB_ACQ_QPI) {
-              d = dsigmoidf_((o - a.best_f) / a.tau_pi) / a.tau_pi;
-            } else {
-              const float m = imax == 0 ? mo_c : moP[imax - 1];
-              const float sgn = o > m ? 1.f : (o < m ? -1.f : 0.f);
-              d = ucb_c * sgn;
-              Wm[lane * Q + imax] = w_s * a1 * (1.f - d);
-            }
-            Wc[lane * Q + imax] = w_s * a1 * d;
-          }
-        }
-        __syncwarp();
-        const int ns = min(32, S - s0);
-        for (int t = 0; t < ns; ++t) {
-          const float* zr = z_s + (s0 + t) * zs;
-          const float* wr = Wc + t * Q;
-          if (lane < P) {
-            const float w = wr[1 + lane];
-            acc_l = fmaf(w, zr[0], acc_l);
-            acc_wm += Wm[t * Q + 1 + lane];
-            float* Lbr = Lb + lane * P;
-            for (int j = 0; j <= lane; ++j) Lbr[j] = fmaf(w, zr[1 + j], Lbr[j]);
-          } else if (lane == P) {
-            acc_mu += wr[0];
-            acc_sd = fmaf(wr[0], zr[0], acc_sd);
-            acc_m += Wm[t * Q];
-          }
-        }
-      }
-      __syncwarp();
-      // qUCB: the sample means carry weight too (they depend on the inputs like a sample with z = column means)
-      if (a.kind == BB_ACQ_QUCB) {
-        if (lane < P) acc_l = fmaf(acc_wm, zb0, acc_l);
-        for (int j = 0; j < P; ++j) {  // column j + 1's mean sits in lane j + 1
-          const float zbj = __shfl_sync(kFull, zb, 1 + j);
-          if (lane < P && j <= lane) Lb[lane * P + j] = fmaf(acc_wm, zbj, Lb[lane * P + j]);
-        }
-        if (lane == P) {
-          acc_mu += acc_m;
-          acc_sd = fmaf(acc_m, zb0, acc_sd);
-        }
-      }
-      __syncwarp();
-      // ---- back through the Cholesky of A22 = Sigma_PP - l l^T + jit I ----
-      float* Mw = Wc;  // [P][P] tril(L22^T dL22)
-      if (lane < P)
-        for (int j = 0; j <= lane; ++j) {
-          float m = 0.f;
-          for (int k = lane; k < P; ++k) m = fmaf(Lw[k * P + lane], Lb[k * P + j], m);
-          Mw[lane * P + j] = m;
-        }
-      __syncwarp();
-      // w = L22^-1 l (forward substitution), lane i holds w_i
-      float res = lane < P ? lv[lane] : 0.f, wv = 0.f;
-      for (int j = 0; j < P; ++j) {
-        const float wj = __shfl_sync(kFull, res, j) / Lw[j * P + j];
-        if (lane == j) wv = wj;
-        if (lane > j && lane < P) res = fmaf(-Lw[lane * P + j], wj, res);
-      }
-      // h = G w, G = (tril(M) + tril(M, -1)^T) / 2
-      float hv = 0.f;
-      for (int j = 0; j < P; ++j) {
-        const float wj = __shfl_sync(kFull, wv, j);
-        if (lane < P) hv = fmaf(j <= lane ? Mw[lane * P + j] : Mw[j * P + lane], wj, hv);
-      }
-      hv *= 0.5f;
-      // q = L22^-T h (back substitution), lane i holds q_i
-      res = hv;
-      float qv = 0.f;
-      for (int j = P - 1; j >= 0; --j) {
-        const float qj = __shfl_sync(kFull, res, j) / Lw[j * P + j];
-        if (lane == j) qv = qj;
-        if (lane < j) res = fmaf(-Lw[j * P + lane], qj, res);
-      }
-      const float lbar = lane < P ? acc_l - 2.f * qv : 0.f;
-      // l = c / sd: A_c = lbar / sd, and sd picks up -sum_i lbar_i l_i / sd
-      const float sd_l = warp_sum(lane < P ? lbar * lv[lane] : 0.f);
-      const float mu_bar = __shfl_sync(kFull, acc_mu, P), sd_bar = __shfl_sync(kFull, acc_sd, P) - sd_l / sd;
-      g_mu = mu_bar;
-      g_var = sd_bar / (2.f * sd);
-      if (lane < P) acw[lane] = lbar / sd;
-      if (!ok) {
-        value = __int_as_float(0x7fc00000);
-        g_mu = g_var = 0.f;
-        if (lane < P) acw[lane] = 0.f;
-      }
-      __syncwarp();
-    }
+    float value, g_mu, g_var;
+    acq_point_partials(a, mu, var, cr, P, p.pend_mu, p.pend_cov, z_s, zs, S, zb, zdev, w, value, g_mu, g_var,
+                       lane);
     if (!var_free) g_var = 0.f;
     // ---- dA/dk_i, folded with dk_i/dt into k_w: coef_i = gk_i dA/dk_i ----
     const float k_mu = sy * g_mu, k_var = -2.f * sy2 * g_var;
@@ -454,7 +162,7 @@ __global__ void __launch_bounds__(kGradThreads) k_acq_grad(const GradParams p) {
       float u = 0.f;
       for (int j = i0; j < p.n_pad; ++j) u = fmaf(__ldg(p.linv + (size_t)j * p.n_pad + i), v_w[j], u);
       float kb = fmaf(k_mu, __ldg(p.alpha + i), k_var * u);
-      for (int q = 0; q < P; ++q) kb = fmaf(-sy2 * acw[q], __ldg(p.pend_beta + (size_t)q * p.n_pad + i), kb);
+      for (int q = 0; q < P; ++q) kb = fmaf(-sy2 * w.ac[q], __ldg(p.pend_beta + (size_t)q * p.n_pad + i), kb);
       k_w[i] = gk_w[i] * kb;
     }
     __syncwarp();
@@ -465,7 +173,7 @@ __global__ void __launch_bounds__(kGradThreads) k_acq_grad(const GradParams p) {
       for (int i = 0; i < p.n; ++i) g = fmaf(k_w[i], aj + 0.5f * __ldg(p.train_m2 + (size_t)i * p.d_pad + j), g);
       for (int q = 0; q < P; ++q) {
         const float b = fmaf(__ldg(p.pend_x + (size_t)q * p.d + j), __ldg(p.cand_scale + j), __ldg(p.cand_shift + j));
-        g = fmaf(sy2 * acw[q] * gkp[q], aj - b, g);
+        g = fmaf(sy2 * w.ac[q] * gkp[q], aj - b, g);
       }
       p.grad[c * p.d + j] = g * __ldg(p.cand_scale + j);
     }

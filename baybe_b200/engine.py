@@ -408,21 +408,21 @@ class DeviceGP:
                                                     _lib.ACQ_KIND[acq.kind], acq.params())
 
     def value_and_grad(self, acq: AcqConfig, x, z: torch.Tensor | None, pending=None):
-        """Acquisition value [N] and its gradient [N, d] with respect to the raw comp-rep rows x (``bb_acq_grad``).
-        Without pending points the value is ``score``'s; with them (Monte Carlo kinds, z of shape (S, 1 + p)) it is
-        ``score_joint``'s value of [x; pending], candidate first."""
+        """Acquisition value [N] and its gradient [N, d] with respect to the raw comp-rep rows x (``bb_acq_grad``, or
+        ``bb_acq_grad_large`` for wide models and n_pad > 256: ``acq_grad_op``).  Without pending points the value is
+        ``score``'s; with them (Monte Carlo kinds, z of shape (S, 1 + p)) it is ``score_joint``'s value of
+        [x; pending], candidate first."""
         xd = self.prepare(x).to(torch.float32).contiguous()
         zf = None
         if acq.is_mc:
             if z is None:
                 raise ValueError("Monte Carlo acquisition functions need base samples")
             zf = z.to(self.device, torch.float32).contiguous()
+        op = acq_grad_op(self.model)
         if pending is None or len(pending) == 0:
-            return torch.ops.baybe_b200.acq_grad(xd, None, None, None, None, zf, self.handle, _lib.ACQ_KIND[acq.kind],
-                                                 acq.params())
+            return op(xd, None, None, None, None, zf, self.handle, _lib.ACQ_KIND[acq.kind], acq.params())
         px, beta, pmu, pcov = self.pending_stats(pending)
-        return torch.ops.baybe_b200.acq_grad(xd, px, beta, pmu, pcov, zf, self.handle, _lib.ACQ_KIND[acq.kind],
-                                             acq.params())
+        return op(xd, px, beta, pmu, pcov, zf, self.handle, _lib.ACQ_KIND[acq.kind], acq.params())
 
     def argmax(self, scores: torch.Tensor, keep: torch.Tensor | None, index_offset: int = 0) -> torch.Tensor:
         """Packed (score, lowest global index) key of a score vector (``bb_argmax``)."""
@@ -617,6 +617,29 @@ def _op_acq_grad(x: torch.Tensor, pend_x: torch.Tensor | None, pend_beta: torch.
                  kind: int, params: list[float]) -> tuple[torch.Tensor, torch.Tensor]:
     """``bb_acq_grad``: raw fp32 rows x [N, d] -> value [N], gradient [N, d]; with p pending points their rows
     pend_x [p, d] and ``pending_stats`` (beta [p, n_pad], mean [p], covariance [p, p]); z [S, 1 + p] (MC kinds)."""
+    return _acq_grad_call("bb_acq_grad", x, pend_x, pend_beta, pend_mu, pend_cov, z, handle, kind, params)
+
+
+@_op_acq_grad.register_fake
+def _(x, pend_x, pend_beta, pend_mu, pend_cov, z, handle, kind, params):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+
+
+@torch.library.custom_op("baybe_b200::acq_grad_large", mutates_args=())
+def _op_acq_grad_large(x: torch.Tensor, pend_x: torch.Tensor | None, pend_beta: torch.Tensor | None,
+                       pend_mu: torch.Tensor | None, pend_cov: torch.Tensor | None, z: torch.Tensor | None,
+                       handle: int, kind: int, params: list[float]) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_acq_grad_large``: ``acq_grad`` for every single-task model (n_pad up to 1024, wide-feature or not)."""
+    return _acq_grad_call("bb_acq_grad_large", x, pend_x, pend_beta, pend_mu, pend_cov, z, handle, kind, params)
+
+
+@_op_acq_grad_large.register_fake
+def _(x, pend_x, pend_beta, pend_mu, pend_cov, z, handle, kind, params):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+
+
+def _acq_grad_call(entry: str, x, pend_x, pend_beta, pend_mu, pend_cov, z, handle, kind, params):
+    """The body of the ``acq_grad`` and ``acq_grad_large`` ops: the two C entry points take the same arguments."""
     gp = _gp(handle)
     acq = AcqConfig.from_params(kind, params).to_c()
     N = x.shape[0]
@@ -628,16 +651,21 @@ def _op_acq_grad(x: torch.Tensor, pend_x: torch.Tensor | None, pend_beta: torch.
     value = torch.empty(N, dtype=torch.float32, device=x.device)
     grad = torch.empty((N, gp.d), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        _lib.check(_lib.load().bb_acq_grad(C.byref(gp.model), C.byref(acq), _ptr(x), N, P, _ptr(pend_x),
-                                           _ptr(pend_beta), _ptr(pend_mu), _ptr(pend_cov), _ptr(z),
-                                           0 if z is None else z.shape[0], _ptr(value), _ptr(grad), _stream_ptr()),
-                   "bb_acq_grad")
+        _lib.check(getattr(_lib.load(), entry)(C.byref(gp.model), C.byref(acq), _ptr(x), N, P, _ptr(pend_x),
+                                               _ptr(pend_beta), _ptr(pend_mu), _ptr(pend_cov), _ptr(z),
+                                               0 if z is None else z.shape[0], _ptr(value), _ptr(grad),
+                                               _stream_ptr()),
+                   entry)
     return value, grad
 
 
-@_op_acq_grad.register_fake
-def _(x, pend_x, pend_beta, pend_mu, pend_cov, z, handle, kind, params):
-    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+def acq_grad_op(model: _lib.Model):
+    """The gradient op ``DeviceGP.value_and_grad`` runs on a model: ``acq_grad`` (``bb_acq_grad``, one warp per point)
+    for models that are not wide and have n_pad <= ``GRAD_MAX_NPAD``, ``acq_grad_large`` (``bb_acq_grad_large``, one
+    CTA per point) for the rest.  Both compute the same function; task models are rejected by either."""
+    if not model.wide and model.n_pad <= _lib.GRAD_MAX_NPAD:
+        return torch.ops.baybe_b200.acq_grad
+    return torch.ops.baybe_b200.acq_grad_large
 
 
 def _check_keep(keep: torch.Tensor | None, N: int) -> None:

@@ -573,6 +573,18 @@ int bb_acq_grad(const bb_model* m, const bb_acq_spec* a, const float* d_x, int64
                 const float* d_pend_x, const float* d_pend_beta, const float* d_pend_mu, const float* d_pend_cov,
                 const float* d_z, int32_t S, float* d_value, float* d_grad, void* stream);
 
+/* ---- bb_acq_grad for every single-task model: n_pad up to BB_MAX_TRAIN, wide-feature or not.
+ *   m: a single-task model (else BB_ERR_UNSUPPORTED); every other argument, the values and the gradient as
+ *     bb_acq_grad.
+ * One CTA per point (bb_acq_grad: one warp), suited to long kernel rows.  The base samples sit in shared memory when
+ * they fit beside the point's scratch and are read from global memory otherwise; a model whose scratch alone does not
+ * fit returns BB_ERR_UNSUPPORTED.  Every argument is checked before any CUDA call.  Synchronises nothing; no float
+ * atomics: repeated calls are bit-identical. */
+int bb_acq_grad_large(const bb_model* m, const bb_acq_spec* a, const float* d_x, int64_t N, int32_t n_pending,
+                      const float* d_pend_x, const float* d_pend_beta, const float* d_pend_mu,
+                      const float* d_pend_cov, const float* d_z, int32_t S, float* d_value, float* d_grad,
+                      void* stream);
+
 /* ---- value and gradient of the acquisition value bb_objective_score reports (an objective that is not affine in its
  * targets: desirability, transformed single targets) at N points, for the continuous optimiser.
  *   models: host array of n_targets = M in [1, BB_OBJ_MAX_TARGETS] models, one per target in objective order; each
