@@ -240,14 +240,16 @@ __device__ __forceinline__ void mc_table_setup(float* __restrict__ tab, const fl
     if (j > 0) {
       const float a = (float)kMcNT / (float)j;  // a = w - zeta_(9) + 1 = 1/v
       const float w = w0 - 1.0f + a;
-      const float cut = thr - w;  // zeta < thr  <=>  zeta - w < cut
       float acc0 = 0.f, acc1 = 0.f;
 #pragma unroll 4
       for (int e = 0; e < S; e += 2) {
-        const float d0 = fmaf(sgn, z_s[e], -w), d1 = fmaf(sgn, z_s[e + 1], -w);
+        // the tail is zeta < thr, tested on zeta itself: zeta - w rounds, and a zeta one ulp below thr would
+        // round to thr - w and drop out of the large-w entries
+        const float e0 = sgn * z_s[e], e1 = sgn * z_s[e + 1];
+        const float d0 = e0 - w, d1 = e1 - w;
         const float r0 = fast_rcp(d0 * d0), r1 = fast_rcp(d1 * d1);
-        acc0 += d0 < cut ? r0 : 0.f;
-        acc1 += d1 < cut ? r1 : 0.f;
+        acc0 += e0 < thr ? r0 : 0.f;
+        acc1 += e1 < thr ? r1 : 0.f;
       }
       f = (acc0 + acc1) * a * a;
     }
@@ -308,11 +310,11 @@ __device__ __forceinline__ void mc_table_grid_part(float* __restrict__ tab, cons
     if (j > 0) {
       const float a = (float)kMcNT / (float)j;
       const float w = w0 - 1.0f + a;
-      const float cut = thr - w;
       float acc = 0.f;
       for (int e = lane; e < S; e += 32) {
-        const float d0 = fmaf(sgn, z_s[e], -w);
-        acc += d0 < cut ? fast_rcp(d0 * d0) : 0.f;
+        const float e0 = sgn * z_s[e];  // tail test on zeta itself, as in mc_table_setup
+        const float d0 = e0 - w;
+        acc += e0 < thr ? fast_rcp(d0 * d0) : 0.f;
       }
       for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
       f = acc * a * a;
@@ -391,6 +393,9 @@ __device__ __forceinline__ float mc_finalize(const bb_acq_spec& a, float mu, flo
   const float so = a.obj_scale * sd;
   switch (a.kind) {
     case BB_ACQ_QLOGEI:
+      // Domain: where every sample has t < -9.2e18 (|o - best_f| > 9.2e12 at tau = 1e-6), 1/(1+t^2) is below
+      // FLT_MIN and flushes to zero, so the row scores -inf; its float64 value, about log(0.1 tau) - 2 log|t|,
+      // is finite.  Such a row still ranks below every row inside the domain.
       return logf(a.tau_relu) + logf((s0 + 0.1f * s1) / (float)S);
     case BB_ACQ_QEI:
     case BB_ACQ_QPI:

@@ -193,7 +193,8 @@ __device__ __forceinline__ float kernel_from_t(float t) {
 }
 
 // ------------------------------------------------------------------------------------------
-// packed (score, lowest-index) keys: signed-int64 max == (max score, then min index)
+// packed (score, lowest-index) keys: signed-int64 max == (max score, then min index); -0.0 packs as +0.0, so
+// the two zeros tie and the lower index wins, as in torch.argmax.  NaN scores are skipped by every caller.
 // ------------------------------------------------------------------------------------------
 __host__ __device__ __forceinline__ int64_t pack_key(float score, uint32_t local_idx) {
   uint32_t u;
@@ -202,6 +203,7 @@ __host__ __device__ __forceinline__ int64_t pack_key(float score, uint32_t local
 #else
   memcpy(&u, &score, 4);
 #endif
+  if (u == 0x80000000u) u = 0u;
   int32_t s = (int32_t)u;
   s ^= (s >> 31) & 0x7fffffff;  // total order as signed int
   return (int64_t)(((uint64_t)(uint32_t)s << 32) | (uint64_t)(0xffffffffu - local_idx));

@@ -444,10 +444,13 @@ def decode_best(key: torch.Tensor) -> tuple[float, int]:
 
 def pack_best(score: float, idx: int) -> int:
     """Host-side twin of ``pack_key`` (csrc/common.cuh): signed-int64 order == (score, then lowest
-    index).  Used by the CPU tests of the sharded arg-max protocol."""
+    index; -0.0 packs as +0.0, so the zeros tie as in torch.argmax).  Used by the CPU tests of the sharded
+    arg-max protocol."""
     import struct
 
     u = struct.unpack("<i", struct.pack("<f", score))[0]
+    if u == -(1 << 31):  # -0.0
+        u = 0
     s = u ^ ((u >> 31) & 0x7FFFFFFF)
     v = ((s & 0xFFFFFFFF) << 32) | (0xFFFFFFFF - idx)
     return v - (1 << 64) if v >= (1 << 63) else v
