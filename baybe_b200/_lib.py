@@ -44,7 +44,8 @@ NIPV_IMAGE_CAP = 4 << 30  # bytes of the integration points' image, (n + |C| + d
 # single-target kinds with a gradient path (bb_acq_grad, bb_acq_grad_large): continuous and hybrid spaces,
 # baybe_b200/continuous.py
 GRAD_KINDS = ("qLogEI", "qEI", "qUCB", "qSR", "qPI", "UCB", "EI", "LogEI", "PI", "PM", "PSTD")
-# bb_acq_grad takes models that are not wide with n_pad up to this; bb_acq_grad_large takes the rest (engine.acq_grad_op)
+# bb_acq_grad and bb_objective_grad take models that are not wide with n_pad up to this; bb_acq_grad_large and
+# bb_objective_grad_large take the rest (engine.acq_grad_op, engine.objective_grad_op)
 GRAD_MAX_NPAD = 256
 MAX_PENDING = 31
 MAX_TRAIN = 1024
@@ -174,6 +175,8 @@ _SIGNATURES = {
                                     _i32, _vp, _vp, _vp]),
     "bb_objective_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(Objective), _vp,
                                     _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "bb_objective_grad_large": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(Objective),
+                                          _vp, _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "bb_hvi_grad": (C.c_int, [C.POINTER(C.POINTER(Model)), _i32, C.POINTER(AcqSpec), C.POINTER(C.c_float),
                               C.POINTER(C.c_float), _vp, _i64, _i32, _vp, C.POINTER(_vp), _vp, _vp, _vp, _i32, _vp, _vp,
                               _vp, _i32, _vp, _vp, _vp]),

@@ -138,7 +138,8 @@ class B200BotorchRecommender(BayesianRecommender):
     targets, with qNIPV, and with qEHVI / qLogEHVI for Pareto objectives (gradient path, ``baybe_b200.continuous``), or
     qNEI (hybrid spaces, search by scoring, ``baybe_b200.hybrid``).  The single-target kinds on a single target run on
     every single-task model up to 1024 measurements, wide comp-rep encodings included (``bb_acq_grad_large`` past 256
-    training points and for wide models)."""
+    training points and for wide models); so do desirability objectives and transformed targets, each target on its own
+    model (``bb_objective_grad_large``)."""
 
     compatibility: ClassVar[SearchSpaceType] = SearchSpaceType.HYBRID
     supports_discrete_subset_generating_constraints: ClassVar[bool] = True
@@ -301,10 +302,10 @@ class B200BotorchRecommender(BayesianRecommender):
         return self._scorer is None or isinstance(self._scorer, (ObjectiveScorer, NipvScorer, HviScorer))
 
     def _optimize_gradient(self, searchspace, disc_comp: np.ndarray, batch_size: int):
-        """Multi-start L-BFGS-B on ``bb_acq_grad`` (``bb_objective_grad`` for objectives that are not affine in their
-        targets, ``bb_nipv_grad`` for qNIPV, ``bb_hvi_grad`` for qEHVI / qLogEHVI) over disc_comp x the continuous box
-        (``baybe_b200.continuous``): (points in comp-rep column order, configuration indices, joint value of [batch;
-        pending])."""
+        """Multi-start L-BFGS-B on ``bb_acq_grad`` (``bb_objective_grad`` / ``bb_objective_grad_large`` for objectives
+        that are not affine in their targets, ``bb_nipv_grad`` for qNIPV, ``bb_hvi_grad`` for qEHVI / qLogEHVI) over
+        disc_comp x the continuous box (``baybe_b200.continuous``): (points in comp-rep column order, configuration
+        indices, joint value of [batch; pending])."""
         from baybe.parameters.numerical import _FixedNumericalContinuousParameter
 
         from baybe_b200.continuous import recommend_continuous_hybrid

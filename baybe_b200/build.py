@@ -19,7 +19,8 @@ LIB_PATH = OUT_DIR / "libbaybe_b200.so"
 STAMP = OUT_DIR / "build.stamp"
 
 SOURCES = ["model.cu", "fused.cu", "wide.cu", "aux_kernels.cu", "acq.cu", "mo.cu", "objective.cu", "nei.cu", "parego.cu", "peer.cu", "stream.cu",
-           "boxdec.cu", "nipv.cu", "grad.cu", "objgrad.cu", "nipvgrad.cu", "hvigrad.cu", "gradlarge.cu"]
+           "boxdec.cu", "nipv.cu", "grad.cu", "objgrad.cu", "nipvgrad.cu", "hvigrad.cu", "gradlarge.cu",
+           "objgradlarge.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",

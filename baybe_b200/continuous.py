@@ -21,7 +21,8 @@ serves both: a continuous space is a hybrid space with one empty discrete config
 
 Objectives that are not affine in their targets (desirability, transformed single targets) come as a
 ``baybe_b200.objectives.ObjectiveScorer`` in place of the model: raw and final values from its ``scores`` and
-``joint_value``, gradients from its ``value_and_grad`` (``bb_objective_grad``), base samples of M(1+p) columns from its
+``joint_value``, gradients from its ``value_and_grad`` (``bb_objective_grad``, or ``bb_objective_grad_large`` when a target's
+model is wide or has n_pad > 256, chosen by ``engine.objective_grad_op``), base samples of M(1+p) columns from its
 ``base_samples``.  Its pending-point conditioning is built once per greedy step and reused by every evaluation.
 qNIPV comes the same way, as a ``baybe_b200.nipv.NipvScorer``: raw and final values from ``bb_nipv_score``, gradients
 from ``bb_nipv_grad`` over the integration points' image, which is built once per greedy step with the conditioning

@@ -286,6 +286,155 @@ __device__ __forceinline__ TargetScratch target_scratch(float* wb, int M, int m,
   return t;
 }
 
+// ---- one CTA of 256 threads per point (k_acq_grad_large in gradlarge.cu, k_objective_grad_large in objgradlarge.cu) -
+// Each piece is one model's; the caller synchronises the CTA between them.  Every per-element sum runs in the order of
+// the warp-per-point pieces above (kernel_row_warp, linv_apply_warp, linvt_apply_col), so on the shapes both mappings
+// take (d < 32) v, u and the pending products agree bit for bit.
+constexpr int kCtaThreads = 256;
+constexpr int kCtaWarps = kCtaThreads / 32;
+
+// block b of nb in snake order over the warps: round r gives warp w block r W + w (r even) or r W + W - 1 - w (r odd)
+__device__ __forceinline__ int snake_block(int r, int warp) {
+  return r * kCtaWarps + ((r & 1) ? kCtaWarps - 1 - warp : warp);
+}
+
+// The kernel row of the point a (a_w: its d scaled coordinates): k_w[i] = k_i, gk_w[i] = gk_i (0 past n).  A thread per
+// training row for d < 32, a warp per row (lanes over columns) from d = 32 on, so that wide rows are read coalesced.
+template <int FAMILY>
+__device__ __forceinline__ void kernel_row_cta(const float* a_w, const float* train_m2, int n, int n_pad, int d,
+                                               int d_pad, float sf2, float* k_w, float* gk_w) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (d < 32) {
+    for (int i = threadIdx.x; i < n_pad; i += blockDim.x) {
+      float t = 0.f;
+      for (int j = 0; j < d; ++j) {
+        const float df = a_w[j] + 0.5f * __ldg(train_m2 + (size_t)i * d_pad + j);
+        t = fmaf(df, df, t);
+      }
+      float k, dk;
+      kernel_and_slope<FAMILY>(t, k, dk);
+      k_w[i] = i < n ? sf2 * k : 0.f;
+      gk_w[i] = i < n ? 2.f * sf2 * dk : 0.f;
+    }
+  } else {
+    for (int i = warp; i < n_pad; i += kCtaWarps) {
+      float t = 0.f;
+      if (i < n)
+        for (int j = lane; j < d; j += 32) {
+          const float df = a_w[j] + 0.5f * __ldg(train_m2 + (size_t)i * d_pad + j);
+          t = fmaf(df, df, t);
+        }
+      t = warp_sum(t);
+      float k, dk;
+      kernel_and_slope<FAMILY>(t, k, dk);
+      if (lane == 0) {
+        k_w[i] = i < n ? sf2 * k : 0.f;
+        gk_w[i] = i < n ? 2.f * sf2 * dk : 0.f;
+      }
+    }
+  }
+}
+
+// v = L^-1 k: the warps take the 32-row blocks of the lower triangle in snake order, so that each reads about the same
+// share of it; each block as linv_apply_warp forms it.  The same pass forms kb_s[q] = k . beta_q of the P pending
+// points (warp q mod 8).
+__device__ __forceinline__ void linv_apply_cta(const float* linv, int n_pad, const float* k_w, float* v_w, int P,
+                                               const float* pend_beta, float* kb_s) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nb = n_pad >> 5;
+  const int rounds = (nb + kCtaWarps - 1) / kCtaWarps;
+  for (int r = 0; r < rounds; ++r) {
+    const int jb = snake_block(r, warp);
+    if (jb >= nb) continue;
+    const int j0 = jb << 5;
+    float rr[32];
+#pragma unroll
+    for (int q = 0; q < 32; ++q) rr[q] = 0.f;
+    for (int i0 = 0; i0 <= j0; i0 += 32) {
+      const float ki = k_w[i0 + lane];
+      const float* Lr = linv + (size_t)j0 * n_pad + i0 + lane;
+#pragma unroll
+      for (int q = 0; q < 32; ++q) rr[q] = fmaf(__ldg(Lr + (size_t)q * n_pad), ki, rr[q]);
+    }
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) {  // reduce-scatter: lane l ends with row j0 + l
+      const bool up = (lane & off) != 0;
+#pragma unroll
+      for (int q = 0; q < off; ++q) {
+        const float send = up ? rr[q] : rr[q + off];
+        const float keep = up ? rr[q + off] : rr[q];
+        rr[q] = keep + __shfl_xor_sync(kFull, send, off);
+      }
+    }
+    v_w[j0 + lane] = rr[0];
+  }
+  for (int q = warp; q < P; q += kCtaWarps) {
+    float kb = 0.f;
+    for (int i = lane; i < n_pad; i += 32) kb = fmaf(k_w[i], __ldg(pend_beta + (size_t)q * n_pad + i), kb);
+    kb = warp_sum(kb);
+    if (lane == 0) kb_s[q] = kb;
+  }
+}
+
+// u = L^-T v over the 32-column blocks in snake order (lane l owns column i0 + l, no reduction), folded with the slope
+// into the kernel row: k_w[i] = gk_i dA/dk_i, dA/dk_i = k_mu alpha_i + k_var u_i - sum_q acs[q] beta_q,i (k_mu = s_y
+// A_mu, k_var = -2 s_y^2 A_var, acs[q] = s_y^2 A_c[q]).
+__device__ __forceinline__ void linvt_fold_cta(const float* linv, const float* alpha, int n_pad, const float* v_w,
+                                               const float* gk_w, float k_mu, float k_var, int P,
+                                               const float* pend_beta, const float* acs, float* k_w) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nb = n_pad >> 5;
+  const int rounds = (nb + kCtaWarps - 1) / kCtaWarps;
+  for (int r = 0; r < rounds; ++r) {
+    const int ib = snake_block(r, warp);
+    if (ib >= nb) continue;
+    const int i0 = ib << 5, i = i0 + lane;
+    float u = 0.f;
+    for (int j = i0; j < n_pad; ++j) u = fmaf(__ldg(linv + (size_t)j * n_pad + i), v_w[j], u);
+    float kb = fmaf(k_mu, __ldg(alpha + i), k_var * u);
+    for (int q = 0; q < P; ++q) kb = fmaf(-acs[q], __ldg(pend_beta + (size_t)q * n_pad + i), kb);
+    k_w[i] = gk_w[i] * kb;
+  }
+}
+
+// Reverse pass through the folded kernel row, first half: with G = 256 / d row groups of d threads (d < 256), group g
+// sums the rows i = g mod G of column j into part[g d + j].  Every thread of the CTA calls it (it synchronises).
+__device__ __forceinline__ void row_groups_cta(const float* k_w, const float* a_w, const float* train_m2, int n, int d,
+                                               int d_pad, float* part) {
+  const int G = d < kCtaThreads ? kCtaThreads / d : 1;
+  if (G > 1) {
+    const int j = threadIdx.x % d, g = threadIdx.x / d;
+    if (g < G) {
+      const float aj = a_w[j];
+      float acc = 0.f;
+      for (int i = g; i < n; i += G) acc = fmaf(k_w[i], aj + 0.5f * __ldg(train_m2 + (size_t)i * d_pad + j), acc);
+      part[g * d + j] = acc;
+    }
+    __syncthreads();
+  }
+}
+
+// Second half: dA/da_j, the row groups summed in order (or the rows in order, one thread per column, for d >= 256),
+// plus the direct terms acs[q] gkp[q] (a_j - b_qj) of k(x, x_p).  Multiply by cand_scale[j] for dA/dx_j.
+__device__ __forceinline__ float col_grad_cta(int j, const float* k_w, const float* a_w, const float* train_m2, int n,
+                                              int d, int d_pad, const float* part, int P, const float* pend_x,
+                                              const float* cand_scale, const float* cand_shift, const float* acs,
+                                              const float* gkp) {
+  const int G = d < kCtaThreads ? kCtaThreads / d : 1;
+  const float aj = a_w[j];
+  float g = 0.f;
+  if (G > 1) {
+    for (int r = 0; r < G; ++r) g += part[r * d + j];
+  } else {
+    for (int i = 0; i < n; ++i) g = fmaf(k_w[i], aj + 0.5f * __ldg(train_m2 + (size_t)i * d_pad + j), g);
+  }
+  for (int q = 0; q < P; ++q) {
+    const float b = fmaf(__ldg(pend_x + (size_t)q * d + j), __ldg(cand_scale + j), __ldg(cand_shift + j));
+    g = fmaf(acs[q] * gkp[q], aj - b, g);
+  }
+  return g;
+}
+
 // ---- single-target value and partials at one point (k_acq_grad in grad.cu, k_acq_grad_large in gradlarge.cu) ------
 
 // Column means of the base samples z [S][zs] (lane k < 1 + P: column k) and, for P = 0, the mean of column 0 in every

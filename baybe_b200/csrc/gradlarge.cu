@@ -26,8 +26,6 @@
 
 namespace bb {
 
-constexpr int kLargeThreads = 256;
-constexpr int kLargeWarps = kLargeThreads / 32;
 constexpr int kLargeMaxNPad = BB_MAX_TRAIN;
 
 struct GradLargeParams {
@@ -48,18 +46,13 @@ struct GradLargeParams {
 };
 
 // per-CTA scratch in floats: a [d_pad] | k (then gk dA/dk), gk, v [n_pad] | c_p, k . beta_p, gkp, 4 scalars [32] |
-// acq_point_partials' scratch | the column-gradient partials [kLargeThreads]
+// acq_point_partials' scratch | the column-gradient partials [kCtaThreads]
 __host__ __device__ inline int grad_large_floats(int n_pad, int d_pad, int P) {
-  return (d_pad + 3 * n_pad + 4 * 32 + acq_scratch_floats(P) + kLargeThreads + 3) & ~3;
-}
-
-// block b of nb in snake order over the warps: round r gives warp w block r W + w (r even) or r W + W - 1 - w (r odd)
-__device__ __forceinline__ int snake_block(int r, int warp) {
-  return r * kLargeWarps + ((r & 1) ? kLargeWarps - 1 - warp : warp);
+  return (d_pad + 3 * n_pad + 4 * 32 + acq_scratch_floats(P) + kCtaThreads + 3) & ~3;
 }
 
 template <int FAMILY>
-__global__ void __launch_bounds__(kLargeThreads) k_acq_grad_large(const GradLargeParams p) {
+__global__ void __launch_bounds__(kCtaThreads) k_acq_grad_large(const GradLargeParams p) {
   extern __shared__ __align__(16) float smem_l[];
   const int P = p.P, Q = P + 1;
   const bool is_mc = p.a.kind <= BB_ACQ_QPI;
@@ -75,7 +68,7 @@ __global__ void __launch_bounds__(kLargeThreads) k_acq_grad_large(const GradLarg
   float* gkp = kb_s + 32;       // [32] 2 s_f^2 dk/dt of k(x, x_p)
   float* sc = gkp + 32;         // [4] k_mu, k_var
   const AcqScratch w = acq_scratch(sc + 32, P);
-  float* part = sc + 32 + acq_scratch_floats(P);  // [kLargeThreads]
+  float* part = sc + 32 + acq_scratch_floats(P);  // [kCtaThreads]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float* z = p.z_smem ? z_s : p.z;
   if (p.z_smem) {
@@ -89,77 +82,15 @@ __global__ void __launch_bounds__(kLargeThreads) k_acq_grad_large(const GradLarg
   const float sy = p.y_std, sy2 = sy * sy;
   float zb = 0.f, zdev = 0.f;  // warp 0 only
   if (is_mc && warp == 0) sample_means_warp(z, zs, S, P, zb, zdev, lane);
-  const int nb = p.n_pad >> 5;
-  const int rounds = (nb + kLargeWarps - 1) / kLargeWarps;
-  // row groups of the column-gradient pass: G groups of d threads (d < kLargeThreads), else one thread per column
-  const int G = p.d < kLargeThreads ? kLargeThreads / p.d : 1;
   for (int64_t c = blockIdx.x; c < p.N; c += gridDim.x) {
     // ---- 1. a, the kernel row and its slope ----
     for (int j = threadIdx.x; j < p.d_pad; j += blockDim.x)
       a_w[j] = j < p.d ? fmaf(__ldg(p.x + c * p.d + j), __ldg(p.cand_scale + j), __ldg(p.cand_shift + j)) : 0.f;
     __syncthreads();
-    if (p.d < 32) {
-      for (int i = threadIdx.x; i < p.n_pad; i += blockDim.x) {
-        float t = 0.f;
-        for (int j = 0; j < p.d; ++j) {
-          const float df = a_w[j] + 0.5f * __ldg(p.train_m2 + (size_t)i * p.d_pad + j);
-          t = fmaf(df, df, t);
-        }
-        float k, dk;
-        kernel_and_slope<FAMILY>(t, k, dk);
-        k_w[i] = i < p.n ? p.sf2 * k : 0.f;
-        gk_w[i] = i < p.n ? 2.f * p.sf2 * dk : 0.f;
-      }
-    } else {
-      for (int i = warp; i < p.n_pad; i += kLargeWarps) {
-        float t = 0.f;
-        if (i < p.n)
-          for (int j = lane; j < p.d; j += 32) {
-            const float df = a_w[j] + 0.5f * __ldg(p.train_m2 + (size_t)i * p.d_pad + j);
-            t = fmaf(df, df, t);
-          }
-        t = warp_sum(t);
-        float k, dk;
-        kernel_and_slope<FAMILY>(t, k, dk);
-        if (lane == 0) {
-          k_w[i] = i < p.n ? p.sf2 * k : 0.f;
-          gk_w[i] = i < p.n ? 2.f * p.sf2 * dk : 0.f;
-        }
-      }
-    }
+    kernel_row_cta<FAMILY>(a_w, p.train_m2, p.n, p.n_pad, p.d, p.d_pad, p.sf2, k_w, gk_w);
     __syncthreads();
     // ---- 2. v = L^-1 k over row blocks, and k . beta_p ----
-    for (int r = 0; r < rounds; ++r) {
-      const int jb = snake_block(r, warp);
-      if (jb >= nb) continue;
-      const int j0 = jb << 5;
-      float rr[32];
-#pragma unroll
-      for (int q = 0; q < 32; ++q) rr[q] = 0.f;
-      for (int i0 = 0; i0 <= j0; i0 += 32) {
-        const float ki = k_w[i0 + lane];
-        const float* Lr = p.linv + (size_t)j0 * p.n_pad + i0 + lane;
-#pragma unroll
-        for (int q = 0; q < 32; ++q) rr[q] = fmaf(__ldg(Lr + (size_t)q * p.n_pad), ki, rr[q]);
-      }
-#pragma unroll
-      for (int off = 16; off >= 1; off >>= 1) {  // reduce-scatter: lane l ends with row j0 + l
-        const bool up = (lane & off) != 0;
-#pragma unroll
-        for (int q = 0; q < off; ++q) {
-          const float send = up ? rr[q] : rr[q + off];
-          const float keep = up ? rr[q + off] : rr[q];
-          rr[q] = keep + __shfl_xor_sync(kFull, send, off);
-        }
-      }
-      v_w[j0 + lane] = rr[0];
-    }
-    for (int q = warp; q < P; q += kLargeWarps) {
-      float kb = 0.f;
-      for (int i = lane; i < p.n_pad; i += 32) kb = fmaf(k_w[i], __ldg(p.pend_beta + (size_t)q * p.n_pad + i), kb);
-      kb = warp_sum(kb);
-      if (lane == 0) kb_s[q] = kb;
-    }
+    linv_apply_cta(p.linv, p.n_pad, k_w, v_w, P, p.pend_beta, kb_s);
     __syncthreads();
     // ---- 3. one warp: mu, var, c_p, the value and its partials ----
     if (warp == 0) {
@@ -199,41 +130,13 @@ __global__ void __launch_bounds__(kLargeThreads) k_acq_grad_large(const GradLarg
     }
     __syncthreads();
     // ---- 4. u = L^-T v over column blocks; k_w[i] <- gk_i dA/dk_i ----
-    const float k_mu = sc[0], k_var = sc[1];
-    for (int r = 0; r < rounds; ++r) {
-      const int ib = snake_block(r, warp);
-      if (ib >= nb) continue;
-      const int i0 = ib << 5, i = i0 + lane;
-      float u = 0.f;
-      for (int j = i0; j < p.n_pad; ++j) u = fmaf(__ldg(p.linv + (size_t)j * p.n_pad + i), v_w[j], u);
-      float kb = fmaf(k_mu, __ldg(p.alpha + i), k_var * u);
-      for (int q = 0; q < P; ++q) kb = fmaf(-cr_s[q], __ldg(p.pend_beta + (size_t)q * p.n_pad + i), kb);
-      k_w[i] = gk_w[i] * kb;
-    }
+    linvt_fold_cta(p.linv, p.alpha, p.n_pad, v_w, gk_w, sc[0], sc[1], P, p.pend_beta, cr_s, k_w);
     __syncthreads();
     // ---- 5. dA/dx: row groups x columns, then the groups summed in order ----
-    if (G > 1) {
-      const int j = threadIdx.x % p.d, g = threadIdx.x / p.d;
-      if (g < G) {
-        const float aj = a_w[j];
-        float acc = 0.f;
-        for (int i = g; i < p.n; i += G) acc = fmaf(k_w[i], aj + 0.5f * __ldg(p.train_m2 + (size_t)i * p.d_pad + j), acc);
-        part[g * p.d + j] = acc;
-      }
-      __syncthreads();
-    }
+    row_groups_cta(k_w, a_w, p.train_m2, p.n, p.d, p.d_pad, part);
     for (int j = threadIdx.x; j < p.d; j += blockDim.x) {
-      const float aj = a_w[j];
-      float g = 0.f;
-      if (G > 1) {
-        for (int r = 0; r < G; ++r) g += part[r * p.d + j];
-      } else {
-        for (int i = 0; i < p.n; ++i) g = fmaf(k_w[i], aj + 0.5f * __ldg(p.train_m2 + (size_t)i * p.d_pad + j), g);
-      }
-      for (int q = 0; q < P; ++q) {
-        const float b = fmaf(__ldg(p.pend_x + (size_t)q * p.d + j), __ldg(p.cand_scale + j), __ldg(p.cand_shift + j));
-        g = fmaf(cr_s[q] * gkp[q], aj - b, g);
-      }
+      const float g = col_grad_cta(j, k_w, a_w, p.train_m2, p.n, p.d, p.d_pad, part, P, p.pend_x, p.cand_scale,
+                                   p.cand_shift, cr_s, gkp);
       p.grad[c * p.d + j] = g * __ldg(p.cand_scale + j);
     }
     __syncthreads();
@@ -310,7 +213,7 @@ extern "C" int bb_acq_grad_large(const bb_model* m, const bb_acq_spec* a, const 
   if (blocks > (int64_t)sms * 8) blocks = (int64_t)sms * 8;
   return dispatch_family<true>(m->family, [&](auto fam) {
     BB_SMEM_OPTIN_ONCE(k_acq_grad_large<decltype(fam)::value>);
-    k_acq_grad_large<decltype(fam)::value><<<(int)blocks, kLargeThreads, smem, (cudaStream_t)stream>>>(p);
+    k_acq_grad_large<decltype(fam)::value><<<(int)blocks, kCtaThreads, smem, (cudaStream_t)stream>>>(p);
     BB_LAUNCH_CHECK();
     return BB_OK;
   });

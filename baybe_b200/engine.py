@@ -1083,6 +1083,36 @@ def _op_objective_grad(x: torch.Tensor, handles: list[int], pend_x: torch.Tensor
     """``bb_objective_grad``: raw fp32 rows x [N, d] of the models `handles` (one per target) -> value [N], gradient
     [N, d].  With P pending points their rows pend_x [P, d], one beta [P, n_pad] per model (``pending_stats``), linv
     [M, P, P], w [M, S, P] and pend_terms [S, P] (as ``objective_score``); z [S, M(1+P)] (None for analytic kinds)."""
+    return _objective_grad_call("bb_objective_grad", x, handles, pend_x, betas, linv, w, pend_terms, z, kind, params,
+                                scalarizer, ops, args, n_ops, weights)
+
+
+@_op_objective_grad.register_fake
+def _(x, handles, pend_x, betas, linv, w, pend_terms, z, kind, params, scalarizer, ops, args, n_ops, weights):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+
+
+@torch.library.custom_op("baybe_b200::objective_grad_large", mutates_args=())
+def _op_objective_grad_large(x: torch.Tensor, handles: list[int], pend_x: torch.Tensor | None,
+                             betas: list[torch.Tensor], linv: torch.Tensor | None, w: torch.Tensor | None,
+                             pend_terms: torch.Tensor | None, z: torch.Tensor | None, kind: int, params: list[float],
+                             scalarizer: int, ops: list[int], args: list[float], n_ops: list[int],
+                             weights: list[float]) -> tuple[torch.Tensor, torch.Tensor]:
+    """``bb_objective_grad_large``: ``objective_grad`` for every mix of single-task models (n_pad up to 1024,
+    wide-feature or not)."""
+    return _objective_grad_call("bb_objective_grad_large", x, handles, pend_x, betas, linv, w, pend_terms, z, kind,
+                                params, scalarizer, ops, args, n_ops, weights)
+
+
+@_op_objective_grad_large.register_fake
+def _(x, handles, pend_x, betas, linv, w, pend_terms, z, kind, params, scalarizer, ops, args, n_ops, weights):
+    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+
+
+def _objective_grad_call(entry: str, x, handles, pend_x, betas, linv, w, pend_terms, z, kind, params, scalarizer, ops,
+                         args, n_ops, weights):
+    """The body of the ``objective_grad`` and ``objective_grad_large`` ops: the two C entry points take the same
+    arguments."""
     gps = [_gp(h) for h in handles]
     M, N = len(gps), x.shape[0]
     if x.dim() != 2 or x.shape[1] != gps[0].d or x.dtype != torch.float32 or not x.is_contiguous():
@@ -1099,16 +1129,21 @@ def _op_objective_grad(x: torch.Tensor, handles: list[int], pend_x: torch.Tensor
     value = torch.empty(N, dtype=torch.float32, device=x.device)
     grad = torch.empty((N, x.shape[1]), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        _lib.check(_lib.load().bb_objective_grad(models, M, C.byref(acq), C.byref(obj), _ptr(x), N, P, _ptr(pend_x),
-                                                 beta_ptrs if P else None, _ptr(linv), _ptr(w), _ptr(pend_terms),
-                                                 _ptr(z), 0 if z is None else z.shape[0], _ptr(value), _ptr(grad),
-                                                 _stream_ptr()), "bb_objective_grad")
+        _lib.check(getattr(_lib.load(), entry)(models, M, C.byref(acq), C.byref(obj), _ptr(x), N, P, _ptr(pend_x),
+                                               beta_ptrs if P else None, _ptr(linv), _ptr(w), _ptr(pend_terms),
+                                               _ptr(z), 0 if z is None else z.shape[0], _ptr(value), _ptr(grad),
+                                               _stream_ptr()), entry)
     return value, grad
 
 
-@_op_objective_grad.register_fake
-def _(x, handles, pend_x, betas, linv, w, pend_terms, z, kind, params, scalarizer, ops, args, n_ops, weights):
-    return x.new_empty(x.shape[0]), x.new_empty(x.shape)
+def objective_grad_op(models):
+    """The gradient op ``ObjectiveScorer.value_and_grad`` runs on the models of an objective's targets (one each):
+    ``objective_grad`` (``bb_objective_grad``, one warp per point) when every model is not wide and has n_pad <=
+    ``GRAD_MAX_NPAD``, ``objective_grad_large`` (``bb_objective_grad_large``, one CTA per point) otherwise.  Both
+    compute the same function; task models are rejected by either."""
+    if all(not m.wide and m.n_pad <= _lib.GRAD_MAX_NPAD for m in models):
+        return torch.ops.baybe_b200.objective_grad
+    return torch.ops.baybe_b200.objective_grad_large
 
 
 @torch.library.custom_op("baybe_b200::hvi_grad", mutates_args=())

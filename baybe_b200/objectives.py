@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from baybe_b200 import _lib
-from baybe_b200.engine import AcqConfig
+from baybe_b200.engine import AcqConfig, objective_grad_op
 from baybe_b200.scoring import Scorer
 
 __all__ = ["CompiledObjective", "compile_objective", "evaluate_program", "scalarize", "evaluate_objective",
@@ -34,10 +34,11 @@ def _objective_score(*args):
 
 
 def _objective_grad(*args):
-    """``baybe_b200::objective_grad`` (engine.py) on the models' handles; a module-level seam so that CPU tests can put
-    a float64 stand-in here (same arguments, with the models themselves in place of their handles)."""
+    """The gradient op ``engine.objective_grad_op`` picks for the models (``baybe_b200::objective_grad``, or
+    ``objective_grad_large`` for wide models and n_pad > 256) on their handles; a module-level seam so that CPU tests
+    can put a float64 stand-in here (same arguments, with the models themselves in place of their handles)."""
     gps, rest = args[0], args[1:]
-    return torch.ops.baybe_b200.objective_grad(rest[0], [gp.handle for gp in gps], *rest[1:])
+    return objective_grad_op([gp.model for gp in gps])(rest[0], [gp.handle for gp in gps], *rest[1:])
 
 
 class CompiledObjective:
@@ -370,7 +371,8 @@ class ObjectiveScorer(Scorer):
 
     def value_and_grad(self, x, pend: np.ndarray | None, z: torch.Tensor | None):
         """Acquisition value [N] and its gradient [N, d] with respect to the raw comp-rep rows x
-        (``bb_objective_grad``): the value ``values`` reports for [x; pending], with the base samples z of
+        (``bb_objective_grad``, or ``bb_objective_grad_large`` for wide models and n_pad > 256:
+        ``engine.objective_grad_op``): the value ``values`` reports for [x; pending], with the base samples z of
         ``base_samples`` (M(1+P) columns; None for analytic kinds)."""
         P = 0 if pend is None else len(pend)
         if P and not self.cfg.is_mc:

@@ -607,6 +607,20 @@ int bb_objective_grad(const bb_model* const* models, int32_t n_targets, const bb
                       const float* d_pend_terms, const float* d_z, int32_t S, float* d_value, float* d_grad,
                       void* stream);
 
+/* ---- bb_objective_grad for every mix of single-task models: n_pad up to BB_MAX_TRAIN, wide-feature or not.
+ *   models: as bb_objective_grad, each single-task (else BB_ERR_UNSUPPORTED) with n_pad <= BB_MAX_TRAIN; they share d,
+ *     d_pad and the kernel family and may mix n_pad <= 256 with larger n_pad and wide with non-wide models.  Every
+ *     other argument, the values and the gradient as bb_objective_grad.
+ * One CTA per point (bb_objective_grad: one warp), suited to long kernel rows.  A shape whose scratch (the candidate's
+ * base samples [S][M], each target's kernel slope and L^-1 k, and a [M][d_pad]) does not fit in shared memory returns
+ * BB_ERR_UNSUPPORTED with the sizes in the message.  Every argument is checked before any CUDA call.  Synchronises
+ * nothing; no float atomics: repeated calls are bit-identical. */
+int bb_objective_grad_large(const bb_model* const* models, int32_t n_targets, const bb_acq_spec* a,
+                            const bb_objective* obj, const float* d_x, int64_t N, int32_t n_pending,
+                            const float* d_pend_x, const float* const* d_pend_beta, const float* d_linv,
+                            const float* d_w, const float* d_pend_terms, const float* d_z, int32_t S, float* d_value,
+                            float* d_grad, void* stream);
+
 /* ---- value and gradient of the hypervolume improvement bb_hvi_score reports (qEHVI / qLogEHVI of a Pareto objective)
  * at N points, for the continuous optimiser.
  *   models: host array of n_targets = M in [2, BB_HVI_MAX_TARGETS] models, one per target in objective order; each
